@@ -32,6 +32,11 @@ _SIGNATURES = {
     "bevb200_bev_pool_lift_prepare": (c_int, [_P, _P] + [c_int] * 6 + [_P] * 7 + [c_size_t, _P]),
     "bevb200_bev_pool_lift_columns_workspace_bytes": (c_size_t, [c_int] * 3),
     "bevb200_bev_pool_lift_columns": (c_int, [c_int] * 7 + [_P, _P] + [c_int] * 4 + [_P] * 7 + [c_int, _P, _P, c_size_t, _P]),
+    "bevb200_bev_pool_lift_columns_backward_workspace_bytes": (c_size_t, [c_int] * 3),
+    "bevb200_bev_pool_lift_columns_backward": (c_int, [c_int] * 7 + [_P] * 3 + [c_int] * 4 + [_P] * 5
+                                               + [c_int, _P, _P, _P, c_size_t, _P]),
+    "bevb200_bev_pool_lift_backward_workspace_bytes": (c_size_t, [c_int] * 2),
+    "bevb200_bev_pool_lift_backward": (c_int, [c_int] * 8 + [_P] * 3 + [c_int] * 2 + [_P] * 6 + [_P, c_size_t, _P]),
     "bevb200_bev_pool_prepare_workspace_bytes": (c_size_t, [c_int]),
     "bevb200_bev_pool_prepare_geom": (c_int, [_P, c_int, c_int, _P, _P, _P, c_int] + [_P] * 7
                                       + [c_size_t, _P]),

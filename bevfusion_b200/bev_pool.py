@@ -15,6 +15,7 @@ import ctypes
 import os
 
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import _C
 
@@ -260,6 +261,26 @@ def bev_pool(feats, coords, B, D, H, W):
     return x
 
 
+class _LiftPool(torch.autograd.Function):
+    """out = BEVPoolPlan.lift_pool(depth, ctx) with gradients for depth and ctx.  Saves depth and ctx, never the
+    lifted volume; the forward is the inference forward, bit for bit."""
+
+    @staticmethod
+    def forward(fctx, plan, depth, ctx):
+        out = plan._lift_pool_forward(depth, ctx)
+        fctx.plan = plan
+        fctx.save_for_backward(depth, ctx)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(fctx, out_grad):
+        depth, ctx = fctx.saved_tensors
+        _, want_depth, want_ctx = fctx.needs_input_grad
+        ddepth, dctx = fctx.plan._lift_pool_backward(out_grad.contiguous(), depth, ctx, want_depth, want_ctx)
+        return None, ddepth, dctx
+
+
 class BEVPoolPlan:
     """Precomputed pooling plan for a fixed camera geometry (native API).
 
@@ -319,10 +340,19 @@ class BEVPoolPlan:
         return tables
 
     def lift_pool(self, depth, ctx):
-        """Fused LSS lift + pool (inference): `depth` [B, N, D, fH, fW] softmax volume and `ctx`
-        [B, N, fH, fW, C] channels-last context features -> raw op output [B, nz, nx, ny, C], equal
-        to pool(depth.unsqueeze(-1) * ctx.unsqueeze(2)) without materialising that volume
-        (lss.py:68-73 / depth_lss.py:92-97 followed by base.py:141-176)."""
+        """Fused LSS lift + pool: `depth` [B, N, D, fH, fW] softmax volume and `ctx` [B, N, fH, fW, C]
+        channels-last context features -> raw op output [B, nz, nx, ny, C], equal to
+        pool(depth.unsqueeze(-1) * ctx.unsqueeze(2)) without materialising that volume
+        (lss.py:68-73 / depth_lss.py:92-97 followed by base.py:141-176).
+
+        Differentiable in `depth` and `ctx` (training): when grad is enabled and either requires grad, the
+        backward computes their gradients straight from the output gradient, again without the volume or
+        its gradient (saved for backward: depth, ctx and this plan)."""
+        if torch.is_grad_enabled() and (depth.requires_grad or ctx.requires_grad):
+            return _LiftPool.apply(self, depth, ctx)
+        return self._lift_pool_forward(depth, ctx)
+
+    def _lift_pool_forward(self, depth, ctx):
         _C.require_cuda(depth, "depth", torch.float32)
         _C.require_cuda(ctx, "ctx", torch.float32)
         B, N, D, fH, fW = depth.shape
@@ -355,6 +385,37 @@ class BEVPoolPlan:
                 _C.ptr(ws), ws.numel(), _C.current_stream(depth.device))
         _C.check(rc, "bev_pool_lift")
         return out
+
+    def _lift_pool_backward(self, out_grad, depth, ctx, want_depth, want_ctx):
+        """(ddepth, dctx) of lift_pool from the gradient of its output; a gradient not wanted is None.
+        The column kernel runs wherever the column formulation can (fH <= 64), the pixel kernel otherwise."""
+        _C.require_cuda(out_grad, "out_grad", torch.float32)
+        B, N, D, fH, fW = depth.shape
+        c = ctx.shape[-1]
+        t = self.tables
+        Bq, Dq, Hq, Wq = t.dims
+        assert tuple(out_grad.shape) == (Bq, Dq, Hq, Wq, c)
+        dev = depth.device
+        L = _C.lib()
+        with torch.cuda.device(dev):
+            ddepth = torch.empty_like(depth) if want_depth else None
+            dctx = torch.empty_like(ctx) if want_ctx else None
+            if fH <= 64:
+                col_begin, seg_key, seg_mask, _, _, n_seg = self._lift_tables(B * N, D, fH, fW)
+                ws = _ws(L.bevb200_bev_pool_lift_columns_backward_workspace_bytes(n_seg, t.n_intervals, c), dev)
+                rc = L.bevb200_bev_pool_lift_columns_backward(
+                    Bq, Dq, Hq, Wq, t.n_kept, c, t.n_intervals, _C.ptr(out_grad), _C.ptr(depth), _C.ptr(ctx), B * N, D,
+                    fH, fW, _C.ptr(t.geom), _C.ptr(t.starts), _C.ptr(col_begin), _C.ptr(seg_key), _C.ptr(seg_mask),
+                    n_seg, _C.ptr(ddepth), _C.ptr(dctx), _C.ptr(ws), ws.numel(), _C.current_stream(dev))
+                _C.check(rc, "bev_pool_lift_columns_backward")
+            else:
+                ws = _ws(L.bevb200_bev_pool_lift_backward_workspace_bytes(t.n_total, c), dev)
+                rc = L.bevb200_bev_pool_lift_backward(
+                    Bq, Dq, Hq, Wq, t.n_kept, t.n_total, c, t.n_intervals, _C.ptr(out_grad), _C.ptr(depth),
+                    _C.ptr(ctx), D, fH * fW, _C.ptr(t.perm), _C.ptr(t.geom), _C.ptr(t.starts), _C.ptr(t.lengths),
+                    _C.ptr(ddepth), _C.ptr(dctx), _C.ptr(ws), ws.numel(), _C.current_stream(dev))
+                _C.check(rc, "bev_pool_lift_backward")
+        return ddepth, dctx
 
     def lift(self, depth, ctx, out=None):
         """lift_pool + the module output layout of __call__: depth [B, N, D, fH, fW], ctx [B, N, fH, fW, C]

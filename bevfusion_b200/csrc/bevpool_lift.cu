@@ -20,6 +20,7 @@
 //   per frame, kernel 2 (one warp per interval): adds the interval's T rows in slot order (fixed order: the result
 //     is reproducible), writes the cell, zero-fills the empty cells in between.
 // HBM / L2 traffic per frame: depth + ctx once (13.4 MB), T written and read once (~2 x 20 MB), the BEV grid once.
+// The backward (gradients of depth and ctx, section "backward" below) runs over the same segment tables.
 #include <cub/cub.cuh>
 
 #include "common.cuh"
@@ -240,19 +241,224 @@ __global__ void __launch_bounds__(256)
 struct PoolDimsL {
   int b, d, h, w;
 };
+// cell of the sorted row s (the first row of an interval), -1 outside the grid
+__device__ __forceinline__ int32_t lift_cell_of(const int32_t *__restrict__ geom_feats, int s, int n, PoolDimsL dm) {
+  long long c = -1;
+  if (s >= 0 && s < n) {
+    const int4 g = *reinterpret_cast<const int4 *>(geom_feats + 4ll * s);   // (x, y, z, b): bev_pool_cuda.cu:32-36
+    if ((unsigned)g.x < (unsigned)dm.h && (unsigned)g.y < (unsigned)dm.w && (unsigned)g.z < (unsigned)dm.d &&
+        (unsigned)g.w < (unsigned)dm.b)
+      c = (((long long)g.w * dm.d + g.z) * dm.h + g.x) * dm.w + g.y;
+  }
+  return (int32_t)c;
+}
 __global__ void lift_interval_cells_kernel(const int32_t *__restrict__ geom_feats, const int32_t *__restrict__ starts,
                                            int n, int n_intervals, PoolDimsL dm, int32_t *__restrict__ cells) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_intervals; i += gridDim.x * blockDim.x) {
-    const int s = starts[i];
-    long long c = -1;
-    if (s >= 0 && s < n) {
-      const int4 g = *reinterpret_cast<const int4 *>(geom_feats + 4ll * s);   // (x, y, z, b): bev_pool_cuda.cu:32-36
-      if ((unsigned)g.x < (unsigned)dm.h && (unsigned)g.y < (unsigned)dm.w && (unsigned)g.z < (unsigned)dm.d &&
-          (unsigned)g.w < (unsigned)dm.b)
-        c = (((long long)g.w * dm.d + g.z) * dm.h + g.x) * dm.w + g.y;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_intervals; i += gridDim.x * blockDim.x)
+    cells[i] = lift_cell_of(geom_feats, starts[i], n, dm);
+}
+
+// ---- backward ------------------------------------------------------------------------------------
+// With G = dL/dout and cell(p) the BEV cell of the kept frustum point p = (cam, d, h, w):
+//     ddepth[cam, d, h, w] = ctx[cam, h, w, :] . G[cell(p), :]        (0 for a filtered point)
+//     dctx[cam, h, w, :]   = sum over kept d of depth[cam, d, h, w] * G[cell(p), :]
+// Every (d, h) of a column lies in at most one segment, so one CTA per image column writes every output element of
+// the column exactly once: no memset, no float atomics, and a fixed summation order.
+
+// cell of every segment (through its interval); -1 would mean "outside the grid" (cannot occur for prepared tables)
+__global__ void lift_seg_cells_kernel(const unsigned long long *__restrict__ seg_key, int n_seg,
+                                      const int32_t *__restrict__ geom_feats, const int32_t *__restrict__ starts, int n,
+                                      PoolDimsL dm, int32_t *__restrict__ seg_cell) {
+  for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < n_seg; s += gridDim.x * blockDim.x)
+    seg_cell[s] = lift_cell_of(geom_feats, starts[(uint32_t)(seg_key[s] & 0xffffffffull)], n, dm);
+}
+
+// Shared memory of the column backward: fixed part + per staged segment.  Rows of ctx_s and g_s are padded to Q + 1
+// float4 so that the threads of a warp, which walk h (ctx_s) or the segment (g_s), hit distinct banks.
+struct LiftBwdSmem {
+  size_t fixed, per_seg;
+};
+static LiftBwdSmem lift_bwd_smem(int q, int fh, int depth_bins) {
+  LiftBwdSmem s;
+  s.fixed = (size_t)fh * (q + 1) * 16 + (size_t)fh * q * 16 + (size_t)depth_bins * 8;   // ctx_s, acc_s, cov_s
+  s.per_seg = (size_t)(q + 1) * 16 + (size_t)fh * 4 + 8 + 4;                             // g_s, dep_s, mask_s, d_s
+  return s;
+}
+
+// One CTA per image column.  The column's segments are processed in chunks of at most `smax` (the G rows of a
+// column need not fit in shared memory: C = 256, many depth bins, or up to D * fh segments of jittered geometry).
+// Per chunk: stage the segments' G rows and their depth values; ddepth of every (segment, h in mask) is a C-long dot
+// product written straight to global memory; dctx accumulates in shared memory, one (h, float4) per task, over the
+// segments in order.  At the end the (d, h) no segment covers get ddepth = 0 and dctx is written once.
+template <int Q>
+__global__ void __launch_bounds__(256)
+    lift_columns_bwd_kernel(const float4 *__restrict__ out_grad, const float *__restrict__ depth,
+                            const float4 *__restrict__ ctx, LiftGeom g, const int32_t *__restrict__ col_begin,
+                            const unsigned long long *__restrict__ seg_key,
+                            const unsigned long long *__restrict__ seg_mask, const int32_t *__restrict__ seg_cell,
+                            int smax, float *__restrict__ ddepth, float4 *__restrict__ dctx) {
+  constexpr int QP = Q + 1;
+  extern __shared__ __align__(16) uint8_t lift_bwd_smem_raw[];
+  float4 *ctx_s = reinterpret_cast<float4 *>(lift_bwd_smem_raw);                  // [fh][QP]
+  float4 *acc_s = ctx_s + g.fh * QP;                                               // [fh][Q]
+  float4 *g_s = acc_s + g.fh * Q;                                                  // [smax][QP]
+  unsigned long long *cov_s = reinterpret_cast<unsigned long long *>(g_s + smax * QP);   // [D]
+  unsigned long long *mask_s = cov_s + g.depth_bins;                               // [smax]
+  float *dep_s = reinterpret_cast<float *>(mask_s + smax);                         // [smax][fh]
+  int *d_s = reinterpret_cast<int *>(dep_s + smax * g.fh);                         // [smax]
+  const int col = blockIdx.x, cam = col / g.fw, w = col % g.fw;
+  const int s0 = col_begin[col], s1 = col_begin[col + 1];
+  const bool want_dd = ddepth != nullptr, want_dc = dctx != nullptr;
+  const long long dstride = g.fw;                                                  // ddepth / depth: h -> h + 1
+  const long long dbase = (long long)cam * g.depth_bins * g.fh * g.fw + w;        // (cam, d = 0, h = 0, w)
+  if (want_dd) {
+    for (int e = threadIdx.x; e < g.fh * Q; e += blockDim.x) {
+      const int h = e / Q, q = e - h * Q;
+      ctx_s[h * QP + q] = __ldg(ctx + ((long long)(cam * g.fh + h) * g.fw + w) * Q + q);
     }
-    cells[i] = (int32_t)c;
+    for (int d = threadIdx.x; d < g.depth_bins; d += blockDim.x) cov_s[d] = 0ull;
   }
+  if (want_dc)
+    for (int e = threadIdx.x; e < g.fh * Q; e += blockDim.x) acc_s[e] = make_float4(0.f, 0.f, 0.f, 0.f);
+  __syncthreads();
+  for (int sa = s0; sa < s1; sa += smax) {
+    const int n = min(smax, s1 - sa);
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+      const unsigned long long m = seg_mask[sa + i];
+      const int d = (int)((seg_key[sa + i] >> 32) % (unsigned long long)g.depth_bins);
+      mask_s[i] = m;
+      d_s[i] = d;
+      if (want_dd) atomicOr(&cov_s[d], m);   // integer OR: order-independent
+    }
+    for (int e = threadIdx.x; e < n * Q; e += blockDim.x) {
+      const int i = e / Q, q = e - i * Q;
+      const int cell = seg_cell[sa + i];
+      g_s[i * QP + q] = cell >= 0 ? __ldg(out_grad + (long long)cell * Q + q) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    __syncthreads();
+    if (want_dc)
+      for (int e = threadIdx.x; e < n * g.fh; e += blockDim.x) {
+        const int i = e / g.fh, h = e - i * g.fh;
+        dep_s[e] = (mask_s[i] >> h) & 1ull ? __ldg(depth + dbase + ((long long)d_s[i] * g.fh + h) * dstride) : 0.f;
+      }
+    if (want_dd)
+      for (int e = threadIdx.x; e < n * g.fh; e += blockDim.x) {
+        const int i = e / g.fh, h = e - i * g.fh;
+        if (!((mask_s[i] >> h) & 1ull)) continue;
+        const float4 *cr = ctx_s + h * QP, *gr = g_s + i * QP;
+        float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 4
+        for (int q = 0; q < Q; ++q) {
+          const float4 c4 = cr[q], g4 = gr[q];
+          a.x = fmaf(c4.x, g4.x, a.x); a.y = fmaf(c4.y, g4.y, a.y);
+          a.z = fmaf(c4.z, g4.z, a.z); a.w = fmaf(c4.w, g4.w, a.w);
+        }
+        ddepth[dbase + ((long long)d_s[i] * g.fh + h) * dstride] = (a.x + a.y) + (a.z + a.w);
+      }
+    __syncthreads();   // dep_s complete
+    if (want_dc)
+      for (int e = threadIdx.x; e < g.fh * Q; e += blockDim.x) {
+        const int h = e / Q, q = e - h * Q;
+        float4 a = acc_s[e];
+        for (int i = 0; i < n; ++i) {   // segments in order: fixed summation order
+          const float wgt = dep_s[i * g.fh + h];
+          const float4 g4 = g_s[i * QP + q];
+          a.x = fmaf(wgt, g4.x, a.x); a.y = fmaf(wgt, g4.y, a.y);
+          a.z = fmaf(wgt, g4.z, a.z); a.w = fmaf(wgt, g4.w, a.w);
+        }
+        acc_s[e] = a;
+      }
+    __syncthreads();   // g_s / dep_s / mask_s are overwritten by the next chunk
+  }
+  if (want_dd)
+    for (int e = threadIdx.x; e < g.depth_bins * g.fh; e += blockDim.x) {
+      const int d = e / g.fh, h = e - d * g.fh;
+      if (!((cov_s[d] >> h) & 1ull)) ddepth[dbase + ((long long)d * g.fh + h) * dstride] = 0.f;
+    }
+  if (want_dc)
+    for (int e = threadIdx.x; e < g.fh * Q; e += blockDim.x) {
+      const int h = e / Q, q = e - h * Q;
+      dctx[((long long)(cam * g.fh + h) * g.fw + w) * Q + q] = acc_s[e];
+    }
+}
+
+// Pixel backward (any feature height: the form of the row forward).  First the cell of every frustum point in
+// ORIGINAL order (-1 for the filtered ones, which perm lists after the kept ones) ...
+__global__ void lift_point_cells_kernel(const int32_t *__restrict__ perm, const int32_t *__restrict__ geom_feats,
+                                        const int32_t *__restrict__ starts, const int32_t *__restrict__ lengths,
+                                        int n, int n_total, int n_intervals, PoolDimsL dm,
+                                        int32_t *__restrict__ point_cell) {
+  const int lane = lane_id(), warps = (gridDim.x * blockDim.x) >> 5;
+  for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n_intervals; i += warps) {   // warp per interval
+    const int s0 = starts[i], len = lengths[i];
+    const int32_t c = lift_cell_of(geom_feats, s0, n, dm);
+    for (int s = s0 + lane; s < s0 + len && s < n; s += 32) point_cell[perm[s]] = c;
+  }
+  for (int s = n + blockIdx.x * blockDim.x + threadIdx.x; s < n_total; s += gridDim.x * blockDim.x)
+    point_cell[perm[s]] = -1;
+}
+
+// ... then one warp per pixel walks the depth bins in ascending order: ddepth is a warp-reduced dot of the pixel's
+// context row (held in registers) with the cell's G row, dctx accumulates in registers.
+template <int Q>
+__global__ void __launch_bounds__(256)
+    lift_pixels_bwd_kernel(const float4 *__restrict__ out_grad, const float *__restrict__ depth,
+                           const float4 *__restrict__ ctx, const int32_t *__restrict__ point_cell, int n_pixels,
+                           int depth_bins, int ppc, float *__restrict__ ddepth, float4 *__restrict__ dctx) {
+  constexpr int QPL = (Q + 31) / 32;
+  const int lane = lane_id(), warps = (gridDim.x * blockDim.x) >> 5;
+  const bool want_dd = ddepth != nullptr, want_dc = dctx != nullptr;
+  for (int px = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; px < n_pixels; px += warps) {
+    const int cam = px / ppc, pix = px - cam * ppc;
+    float4 cr[QPL], acc[QPL];
+#pragma unroll
+    for (int u = 0; u < QPL; ++u) {
+      const int q = lane + 32 * u;
+      cr[u] = want_dd && q < Q ? __ldg(ctx + (long long)px * Q + q) : make_float4(0.f, 0.f, 0.f, 0.f);
+      acc[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    for (int d = 0; d < depth_bins; ++d) {
+      const long long p = ((long long)cam * depth_bins + d) * ppc + pix;
+      const int cell = point_cell[p];
+      if (cell < 0) {
+        if (want_dd && lane == 0) ddepth[p] = 0.f;
+        continue;
+      }
+      float4 g4[QPL];
+#pragma unroll
+      for (int u = 0; u < QPL; ++u) {
+        const int q = lane + 32 * u;
+        g4[u] = q < Q ? __ldg(out_grad + (long long)cell * Q + q) : make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+      if (want_dd) {
+        float a = 0.f;
+#pragma unroll
+        for (int u = 0; u < QPL; ++u)
+          a += (cr[u].x * g4[u].x + cr[u].y * g4[u].y) + (cr[u].z * g4[u].z + cr[u].w * g4[u].w);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+        if (lane == 0) ddepth[p] = a;
+      }
+      if (want_dc) {
+        const float wgt = __ldg(depth + p);
+#pragma unroll
+        for (int u = 0; u < QPL; ++u) {
+          acc[u].x = fmaf(wgt, g4[u].x, acc[u].x); acc[u].y = fmaf(wgt, g4[u].y, acc[u].y);
+          acc[u].z = fmaf(wgt, g4[u].z, acc[u].z); acc[u].w = fmaf(wgt, g4[u].w, acc[u].w);
+        }
+      }
+    }
+    if (want_dc)
+#pragma unroll
+      for (int u = 0; u < QPL; ++u) {
+        const int q = lane + 32 * u;
+        if (q < Q) dctx[(long long)px * Q + q] = acc[u];
+      }
+  }
+}
+
+static bool lift_channels_ok(int c) {
+  return c == 16 || c == 32 || c == 64 || c == 80 || c == 96 || c == 128 || c == 160 || c == 256;
 }
 
 struct LiftWs {
@@ -421,6 +627,127 @@ int bevb200_bev_pool_lift_columns(int b, int d, int h, int w, int n, int c, int 
 size_t bevb200_bev_pool_lift_columns_workspace_bytes(int n_segments, int n_intervals, int c) {
   if (n_segments < 0 || n_intervals < 0 || c <= 0) return 0;
   return align_up((size_t)n_segments * c * sizeof(float)) + align_up((size_t)n_intervals * sizeof(int32_t)) + 256;
+}
+
+size_t bevb200_bev_pool_lift_columns_backward_workspace_bytes(int n_segments, int n_intervals, int c) {
+  if (n_segments < 0 || n_intervals < 0 || !lift_channels_ok(c)) return 0;
+  return align_up((size_t)(n_segments > 0 ? n_segments : 1) * sizeof(int32_t)) + 256;   // cell of every segment
+}
+
+int bevb200_bev_pool_lift_columns_backward(int b, int d, int h, int w, int n, int c, int n_intervals,
+                                           const float *out_grad, const float *depth, const float *ctx, int cameras,
+                                           int depth_bins, int feature_h, int feature_w, const int32_t *geom_feats,
+                                           const int32_t *interval_starts, const int32_t *col_begin,
+                                           const uint64_t *seg_key, const uint64_t *seg_mask, int n_segments,
+                                           float *ddepth, float *dctx, void *workspace, size_t workspace_bytes,
+                                           void *stream) {
+  BEVB200_REQUIRE(b > 0 && d > 0 && h > 0 && w > 0 && n >= 0 && n_intervals >= 0 && n_segments >= 0, "bad sizes");
+  BEVB200_REQUIRE(cameras > 0 && depth_bins > 0 && feature_h > 0 && feature_w > 0, "bad lift dims");
+  BEVB200_REQUIRE(feature_h <= 64, "feature height > 64: use bevb200_bev_pool_lift_backward");
+  BEVB200_REQUIRE(lift_channels_ok(c), "bev_pool_lift_columns_backward: channel count not in {16,32,64,80,96,128,160,256}");
+  BEVB200_REQUIRE((long long)b * d * h * w < (1ll << 31), "grid has too many cells");
+  BEVB200_REQUIRE((long long)cameras * feature_w * depth_bins < (1ll << 31), "too many (column, depth) pairs");
+  if (ddepth == nullptr && dctx == nullptr) return BEVB200_OK;
+  BEVB200_REQUIRE(out_grad && col_begin && seg_key && seg_mask && geom_feats && interval_starts, "null input");
+  BEVB200_REQUIRE(ctx || !ddepth, "ddepth needs ctx");
+  BEVB200_REQUIRE(depth || !dctx, "dctx needs depth");
+  BEVB200_REQUIRE(((uintptr_t)ctx % 16 == 0) && ((uintptr_t)dctx % 16 == 0) && ((uintptr_t)out_grad % 16 == 0),
+                  "ctx / dctx / out_grad must be 16-byte aligned");
+  const size_t need = bevb200_bev_pool_lift_columns_backward_workspace_bytes(n_segments, n_intervals, c) - 256;
+  if (workspace == nullptr || workspace_bytes < need) {
+    snprintf(g_last_error, sizeof(g_last_error), "bev_pool_lift_columns_backward: workspace too small (%zu < %zu)",
+             workspace_bytes, need);
+    return BEVB200_EWORKSPACE;
+  }
+  const int q = c / 4;
+  const LiftBwdSmem sm = lift_bwd_smem(q, feature_h, depth_bins);
+  // chunk size: all of a column's segments at once when that stays within ~100 KB (two CTAs per SM), else as many
+  // as the 227 KB of one CTA allow
+  constexpr size_t kTwoPerSM = 100 * 1024, kMaxSmem = 220 * 1024;
+  long long smax = sm.fixed < kTwoPerSM ? (long long)((kTwoPerSM - sm.fixed) / sm.per_seg) : 0;
+  if (smax < 32 && sm.fixed < kMaxSmem) smax = (long long)((kMaxSmem - sm.fixed) / sm.per_seg);
+  if (smax > 256) smax = 256;
+  BEVB200_REQUIRE(smax >= 1, "image column does not fit in shared memory");
+  const size_t smem = sm.fixed + (size_t)smax * sm.per_seg;
+  cudaStream_t st = (cudaStream_t)stream;
+  LiftGeom g{depth_bins, feature_h, feature_w, cameras * feature_w};
+  int32_t *seg_cell = (int32_t *)workspace;
+  if (n_segments > 0) {
+    PoolDimsL dm{b, d, h, w};
+    BEVB200_LAUNCH(lift_seg_cells_kernel, grid_for(n_segments, 256), 256, 0, st, (const unsigned long long *)seg_key,
+                   n_segments, geom_feats, interval_starts, n, dm, seg_cell);
+  }
+#define LIFT_BWD_LAUNCH(Q)                                                                                             \
+  do {                                                                                                                 \
+    BEVB200_CUDA(cudaFuncSetAttribute(lift_columns_bwd_kernel<Q>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+    BEVB200_LAUNCH(lift_columns_bwd_kernel<Q>, g.ncols, 256, smem, st, (const float4 *)out_grad, depth,                \
+                   (const float4 *)ctx, g, col_begin, (const unsigned long long *)seg_key,                             \
+                   (const unsigned long long *)seg_mask, seg_cell, (int)smax, ddepth, (float4 *)dctx);                 \
+  } while (0)
+  switch (c) {
+    case 16: LIFT_BWD_LAUNCH(4); break;
+    case 32: LIFT_BWD_LAUNCH(8); break;
+    case 64: LIFT_BWD_LAUNCH(16); break;
+    case 80: LIFT_BWD_LAUNCH(20); break;
+    case 96: LIFT_BWD_LAUNCH(24); break;
+    case 128: LIFT_BWD_LAUNCH(32); break;
+    case 160: LIFT_BWD_LAUNCH(40); break;
+    case 256: LIFT_BWD_LAUNCH(64); break;
+  }
+#undef LIFT_BWD_LAUNCH
+  return BEVB200_OK;
+}
+
+size_t bevb200_bev_pool_lift_backward_workspace_bytes(int n_total, int c) {
+  if (n_total < 0 || !lift_channels_ok(c)) return 0;
+  return align_up((size_t)(n_total > 0 ? n_total : 1) * sizeof(int32_t)) + 256;   // cell of every frustum point
+}
+
+int bevb200_bev_pool_lift_backward(int b, int d, int h, int w, int n, int n_total, int c, int n_intervals,
+                                   const float *out_grad, const float *depth, const float *ctx, int depth_bins,
+                                   int pixels_per_camera, const int32_t *perm, const int32_t *geom_feats,
+                                   const int32_t *interval_starts, const int32_t *interval_lengths, float *ddepth,
+                                   float *dctx, void *workspace, size_t workspace_bytes, void *stream) {
+  BEVB200_REQUIRE(b > 0 && d > 0 && h > 0 && w > 0 && n >= 0 && n_total >= n && n_intervals >= 0, "bad sizes");
+  BEVB200_REQUIRE(depth_bins > 0 && pixels_per_camera > 0 && n_total % ((long long)depth_bins * pixels_per_camera) == 0,
+                  "bad lift dims");
+  BEVB200_REQUIRE(lift_channels_ok(c), "bev_pool_lift_backward: channel count not in {16,32,64,80,96,128,160,256}");
+  BEVB200_REQUIRE((long long)b * d * h * w < (1ll << 31), "grid has too many cells");
+  if (ddepth == nullptr && dctx == nullptr) return BEVB200_OK;
+  BEVB200_REQUIRE(out_grad && perm && geom_feats && interval_starts && interval_lengths, "null input");
+  BEVB200_REQUIRE(ctx || !ddepth, "ddepth needs ctx");
+  BEVB200_REQUIRE(depth || !dctx, "dctx needs depth");
+  BEVB200_REQUIRE(((uintptr_t)ctx % 16 == 0) && ((uintptr_t)dctx % 16 == 0) && ((uintptr_t)out_grad % 16 == 0),
+                  "ctx / dctx / out_grad must be 16-byte aligned");
+  const size_t need = bevb200_bev_pool_lift_backward_workspace_bytes(n_total, c) - 256;
+  if (workspace == nullptr || workspace_bytes < need) {
+    snprintf(g_last_error, sizeof(g_last_error), "bev_pool_lift_backward: workspace too small (%zu < %zu)",
+             workspace_bytes, need);
+    return BEVB200_EWORKSPACE;
+  }
+  if (n_total == 0) return BEVB200_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  int32_t *point_cell = (int32_t *)workspace;
+  PoolDimsL dm{b, d, h, w};
+  BEVB200_LAUNCH(lift_point_cells_kernel, grid_for((long long)n_total, 256), 256, 0, st, perm, geom_feats,
+                 interval_starts, interval_lengths, n, n_total, n_intervals, dm, point_cell);
+  const int n_pixels = (int)(n_total / depth_bins);
+  const int grid = grid_for((long long)n_pixels * 32, 256, kNumSMs * 16);
+#define LIFT_PIX_LAUNCH(Q)                                                                                             \
+  BEVB200_LAUNCH(lift_pixels_bwd_kernel<Q>, grid, 256, 0, st, (const float4 *)out_grad, depth, (const float4 *)ctx,   \
+                 point_cell, n_pixels, depth_bins, pixels_per_camera, ddepth, (float4 *)dctx)
+  switch (c) {
+    case 16: LIFT_PIX_LAUNCH(4); break;
+    case 32: LIFT_PIX_LAUNCH(8); break;
+    case 64: LIFT_PIX_LAUNCH(16); break;
+    case 80: LIFT_PIX_LAUNCH(20); break;
+    case 96: LIFT_PIX_LAUNCH(24); break;
+    case 128: LIFT_PIX_LAUNCH(32); break;
+    case 160: LIFT_PIX_LAUNCH(40); break;
+    case 256: LIFT_PIX_LAUNCH(64); break;
+  }
+#undef LIFT_PIX_LAUNCH
+  return BEVB200_OK;
 }
 
 }  // extern "C"

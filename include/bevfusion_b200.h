@@ -115,7 +115,8 @@ BEVB200_API int bevb200_bev_channels_first(const float *in, float *out, int batc
  *   ctx    [B*N*fH*fW, c] fp32, channels-last context features
  *   original point index i -> pixel row (i / (depth_bins*pixels_per_camera)) * pixels_per_camera
  *                                       + i % pixels_per_camera
- * Tables as for bevb200_bev_pool_perm (from bevb200_bev_pool_prepare_geom).  Forward only. */
+ * Tables as for bevb200_bev_pool_perm (from bevb200_bev_pool_prepare_geom).  Backward:
+ * bevb200_bev_pool_lift_backward (any feature height) and bevb200_bev_pool_lift_columns_backward below. */
 BEVB200_API int bevb200_bev_pool_lift(int b, int d, int h, int w, int n, int c, int n_intervals,
                           const float *depth, const float *ctx, int depth_bins,
                           int pixels_per_camera, const int32_t *perm, const int32_t *geom_feats,
@@ -152,6 +153,38 @@ BEVB200_API int bevb200_bev_pool_lift_columns(int b, int d, int h, int w, int n,
                                   const uint64_t *seg_key, const uint64_t *seg_mask, const int32_t *seg_slot,
                                   const int32_t *interval_slot_begin, int n_segments, float *out,
                                   void *workspace, size_t workspace_bytes, void *stream);
+
+/* Backward of the fused lift + pool.  With G = out_grad [b, d, h, w, c] fp32 (the gradient of the raw pooled output)
+ * and cell(p) the cell of the kept frustum point p = (cam, d, h, w):
+ *     ddepth[cam, d, h, w] = sum_c ctx[cam, h, w, c] * G[cell(p), c]     (0 where p is filtered)
+ *     dctx[cam, h, w, :]   = sum over the kept d of depth[cam, d, h, w] * G[cell(p), :]
+ * without the lifted volume or its gradient.  ddepth [cameras, depth_bins, feature_h, feature_w] and
+ * dctx [cameras, feature_h, feature_w, c] fp32 are fully written (no pre-zeroing); either may be NULL, and that
+ * gradient is skipped.  c in {16, 32, 64, 80, 96, 128, 160, 256}; ctx, dctx and out_grad 16-byte aligned.  No float
+ * atomics: the result is bit-reproducible run to run.  No host synchronisation (graph-capturable).
+ *   bevb200_bev_pool_lift_columns_backward   feature_h <= 64, over the segment tables of bevb200_bev_pool_lift_prepare
+ *       (seg_slot / interval_slot_begin are not needed).  One CTA per image column; the column's G rows are staged in
+ *       shared memory in chunks, so any number of depth bins / segments per column works.
+ *       workspace: bevb200_bev_pool_lift_columns_backward_workspace_bytes() (one int per segment).
+ *   bevb200_bev_pool_lift_backward           any feature_h, over the plain tables of bevb200_bev_pool_prepare_*
+ *       (perm [n_total] including the filtered tail, as for bevb200_bev_pool_grad_perm); depth / ctx laid out as for
+ *       bevb200_bev_pool_lift.  One warp per pixel walks the depth bins in order.
+ *       workspace: bevb200_bev_pool_lift_backward_workspace_bytes() (one int per frustum point).
+ * The workspace queries return 0 for bad sizes or an unsupported channel count. */
+BEVB200_API size_t bevb200_bev_pool_lift_columns_backward_workspace_bytes(int n_segments, int n_intervals, int c);
+BEVB200_API int bevb200_bev_pool_lift_columns_backward(int b, int d, int h, int w, int n, int c, int n_intervals,
+                                  const float *out_grad, const float *depth, const float *ctx, int cameras,
+                                  int depth_bins, int feature_h, int feature_w, const int32_t *geom_feats,
+                                  const int32_t *interval_starts, const int32_t *col_begin, const uint64_t *seg_key,
+                                  const uint64_t *seg_mask, int n_segments, float *ddepth, float *dctx,
+                                  void *workspace, size_t workspace_bytes, void *stream);
+BEVB200_API size_t bevb200_bev_pool_lift_backward_workspace_bytes(int n_total, int c);
+BEVB200_API int bevb200_bev_pool_lift_backward(int b, int d, int h, int w, int n, int n_total, int c,
+                                  int n_intervals, const float *out_grad, const float *depth, const float *ctx,
+                                  int depth_bins, int pixels_per_camera, const int32_t *perm,
+                                  const int32_t *geom_feats, const int32_t *interval_starts,
+                                  const int32_t *interval_lengths, float *ddepth, float *dctx, void *workspace,
+                                  size_t workspace_bytes, void *stream);
 
 
 /* bev_pool precompute.  Replaces, on device and in one call, the index glue of
