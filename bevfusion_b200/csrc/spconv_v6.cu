@@ -1,4 +1,5 @@
-// Sparse convolution forward on the Hopper tensor cores (warp-level mma.sync), BF16x3 and TF32 precisions.
+// Sparse convolution forward on the Hopper tensor cores, BF16x3 and TF32 precisions: a warp-specialised wgmma
+// kernel (spconv_wg_kernel, BF16x3 at Cout >= 64, described above it) and the mma.sync kernel below.
 //
 //   out[o, :] = epilogue( sum_k features[nbr[k, o], :] @ W[k] )          (spconv_ops.h:260-361)
 //
@@ -129,7 +130,6 @@ __global__ void __launch_bounds__(kV6Threads, 2) spconv_v6_kernel(const V6Params
   using Sh = V6Shape<MODE, COUT>;
   constexpr int S = Sh::kStages, kB = Sh::kB, kStage = Sh::kStage;
   constexpr int NT = COUT / 16;                   // n8 tiles per warp (the two warp halves split the columns)
-  constexpr bool kMergedW = MODE == 0 && COUT <= 64;
   extern __shared__ __align__(128) uint8_t smem_raw[];
   const uint32_t smem = smem_u32(smem_raw);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -174,18 +174,8 @@ __global__ void __launch_bounds__(kV6Threads, 2) spconv_v6_kernel(const V6Params
         cp_async16_row(a + (uint32_t)(r * 128 + ((cc ^ (r & 7)) << 4)),
                        fbase + (unsigned long long)(uint32_t)max(src, 0) * row_bytes + coff, src);
       }
-      if constexpr (kMergedW) {
-        // packed [pair of K blocks][hi | lo][Cout][64 bf16] -> stage rows n = [hi 32 k | lo 32 k] of this K block
-        const uint8_t *pair = p.wpacked + (size_t)(kb >> 1) * 2 * COUT * 128;
-        for (int i = tid; i < COUT * 8; i += kV6Threads) {
-          const int n = i >> 3, lc = i & 7;
-          cp_async16(b + (uint32_t)(n * 128 + ((lc ^ (n & 7)) << 4)),
-                     pair + (lc >> 2) * COUT * 128 + n * 128 + ((((kb & 1) * 4 + (lc & 3)) ^ (n & 7)) << 4));
-        }
-      } else {
-        const uint8_t *src = p.wpacked + (size_t)kb * kB;
-        for (int i = tid; i < kB / 16; i += kV6Threads) cp_async16(b + (uint32_t)i * 16u, src + (size_t)i * 16);
-      }
+      const uint8_t *src = p.wpacked + (size_t)kb * kB;
+      for (int i = tid; i < kB / 16; i += kV6Threads) cp_async16(b + (uint32_t)i * 16u, src + (size_t)i * 16);
     };
 
     float acc[2][NT][4];
@@ -336,6 +326,184 @@ __global__ void __launch_bounds__(kV6Threads, 2) spconv_v6_kernel(const V6Params
   }
 }
 
+// ---- BF16x3 forward on warpgroup MMAs (mode 0) -----------------------------------------------
+// Warp-specialised and persistent: warpgroup 0 is the producer, warpgroups 1 and 2 the consumers.  A tile is
+// kTileM output rows; each consumer warpgroup owns kMT m64 blocks of it and keeps their accumulators (Cout / 2
+// fp32 per thread and block) in registers across all K blocks.  Per K block one ring stage holds
+//   * A: the tile's gathered rows, 128 B each, laid out as before (16-byte chunk c of row r at c ^ (r & 7)), which
+//     is the K-major SWIZZLE_128B layout wgmma reads: the four k16 slices of a row (hi / lo of the two 16-channel
+//     groups) are the same descriptor moved 0 / 32 / 64 / 96 B along the row;
+//   * B: the K block's packed weight rows (Cout x 128 B, same swizzle), one bulk copy.
+// The producer gathers the rows with 16-byte cp.async (zero fill for missing neighbours), each thread arriving on
+// the stage's "full" barrier when its copies land (cp.async.mbarrier.arrive.noinc); one thread adds the weight
+// copy's bytes to the same barrier.  Consumers wait on "full", issue the 3 x 2 x kMT wgmmas of the block, keep one
+// block in flight (wait_group 1) and then release the previous stage on its "empty" barrier.  The tile's epilogue
+// goes through a small per-warp transpose buffer, so the producer keeps filling the ring meanwhile.
+constexpr int kWgThreads = 384;
+constexpr int kWgMinKBlocks = 16;               // fewer K blocks per tile: spconv_v6_kernel
+constexpr int kWgSmemMax = 227 * 1024;        // opt-in dynamic shared memory per block on sm_90
+
+template <int COUT>
+struct WgShape {
+  static_assert(COUT == 64 || COUT == 128, "Cout <= 32 runs on spconv_v6_kernel");
+  static constexpr int kMT = 2;                                // m64 blocks per consumer warpgroup
+  static constexpr int kTileM = 2 * 64 * kMT;                  // 256 rows share one weight stage
+  static constexpr int kA = kTileM * 128;
+  static constexpr int kB = COUT * 128;
+  static constexpr int kStage = kA + kB;                       // multiple of 1024: every stage stays atom-aligned
+  static constexpr int kSlice = 32;                            // columns per epilogue transpose step
+  static constexpr int kLd = kSlice + 4;
+  static constexpr int kEpi = 8 * 16 * kLd * 4;                // one 16-row buffer per consumer warp
+  static constexpr int kFixed = 1024 + kEpi + 2 * 8 * 8;       // alignment slack, transpose buffers, barriers
+  static constexpr int kStages = (kWgSmemMax - kFixed) / kStage > 8 ? 8 : (kWgSmemMax - kFixed) / kStage;
+  static constexpr int kSmem = kFixed + kStages * kStage;
+  static_assert(kStage % 1024 == 0 && kStages >= 2, "ring does not fit");
+};
+
+template <int COUT>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[COUT / 2], uint64_t da, uint64_t db, int accumulate) {
+  if constexpr (COUT == 64) wgmma_bf16_n64(d, da, db, accumulate);
+  else wgmma_bf16_n128(d, da, db, accumulate);
+}
+
+template <int COUT>
+__global__ void __launch_bounds__(kWgThreads, 1) spconv_wg_kernel(const V6Params p) {
+  using Sh = WgShape<COUT>;
+  constexpr int S = Sh::kStages, MT = Sh::kMT, TM = Sh::kTileM;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t bars = smem + S * Sh::kStage;                 // full[S], then empty[S]
+  float *epi = reinterpret_cast<float *>(smem_raw + (bars - smem_u32(smem_raw)) + 2 * 8 * 8);
+  const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
+  const int nkb = p.nkb;
+
+  if (tid == 0) {
+    for (int s = 0; s < S; ++s) {
+      mbar_init(bars + 8 * s, 128 + 1);                        // 128 producer threads + the weight copy
+      mbar_init(bars + 8 * (S + s), 8);                        // one arrive per consumer warp
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  // Programmatic dependent launch: the previous kernel of the stream may still be draining until here; its
+  // results (feature image, row count) are only touched below.  Without the launch attribute both are no-ops.
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+
+  int n_out = p.n_out;
+  if (p.n_out_dev) n_out = min(n_out, __ldg(p.n_out_dev));
+  const int n_tiles = (n_out + TM - 1) / TM;
+
+  if (wg == 0) {
+    // ------------------------------------ producer ------------------------------------------------
+    setmaxnreg_dec<40>();
+    // rows pr + 16 j of the tile, logical 16-byte chunk cc of the K block = channels kb * 32 + 4 cc .. + 3 of the
+    // concatenation over kernel offsets (c_in < 32: one K block spans 32 / c_in offsets)
+    constexpr int J = TM / 16;
+    const int cc = tid & 7, pr = tid >> 3;
+    const unsigned long long fbase = reinterpret_cast<unsigned long long>(p.rows);
+    const uint32_t row_bytes = (uint32_t)p.c_in * 4u;
+    const int cin_mask = p.c_in - 1;
+    auto load_idx = [&](int tile, int kb, int (&idx)[J]) {
+      const int k = (kb * 32 + 4 * cc) >> p.cin_shift;
+#pragma unroll
+      for (int j = 0; j < J; ++j) {
+        const int row = tile * TM + pr + 16 * j;
+        idx[j] = -1;
+        if (k < p.kvol && row < n_out) idx[j] = __ldg(p.nbr + (long long)k * p.nbr_stride + row);
+      }
+    };
+    int idx[J];
+    int tile = blockIdx.x, kb = 0;
+    if (tile < n_tiles) load_idx(tile, 0, idx);
+    for (uint32_t it = 0; tile < n_tiles; ++it) {
+      const uint32_t s = it % S, full = bars + 8 * s;
+      mbar_wait(bars + 8 * (S + s), ((it / S) & 1) ^ 1);     // the consumers are done with the stage
+      const uint32_t a = smem + s * Sh::kStage;
+      if (tid == 0) {
+        mbar_arrive_expect_tx(full, Sh::kB);
+        bulk_copy_g2s(a + Sh::kA, p.wpacked + (size_t)kb * Sh::kB, Sh::kB, full);
+      }
+      const unsigned coff = (unsigned)(((kb * 32 + 4 * cc) & cin_mask) << 2);
+#pragma unroll
+      for (int j = 0; j < J; ++j) {
+        const int r = pr + 16 * j;
+        const int src = idx[j] >= p.n_in ? -1 : idx[j];
+        cp_async16_row(a + (uint32_t)(r * 128 + ((cc ^ (r & 7)) << 4)),
+                       fbase + (unsigned long long)(uint32_t)max(src, 0) * row_bytes + coff, src);
+      }
+      cp_async_mbar_arrive_noinc(full);
+      if (++kb == nkb) { kb = 0; tile += gridDim.x; }
+      if (tile < n_tiles) load_idx(tile, kb, idx);           // next stage's indices: the load overlaps the wait
+    }
+  } else {
+    // ------------------------------------ consumers -----------------------------------------------
+    setmaxnreg_inc<232>();
+    const int cw = wg - 1, warp = (tid >> 5) & 3;
+    float acc[MT][COUT / 2];
+    uint32_t it = 0;
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+      for (int kb = 0; kb < nkb; ++kb, ++it) {
+        const uint32_t s = it % S;
+        mbar_wait(bars + 8 * s, (it / S) & 1);
+        // the rows arrived through cp.async (generic proxy) and are read by wgmma (async proxy)
+        fence_proxy_async_smem();
+        wgmma_fence();
+        const uint32_t a = smem + s * Sh::kStage + cw * (MT * 64 * 128), b = smem + s * Sh::kStage + Sh::kA;
+#pragma unroll
+        for (int g = 0; g < 2; ++g) {       // the two 16-channel groups of the K block: A [hi | lo], W [hi, hi | lo, lo]
+          const uint64_t bh = wgmma_desc_sw128(b + 32 * g), bl = wgmma_desc_sw128(b + 64 + 32 * g);
+#pragma unroll
+          for (int m = 0; m < MT; ++m) {
+            const uint64_t ah = wgmma_desc_sw128(a + m * (64 * 128) + 64 * g), al = wgmma_desc_sw128(a + m * (64 * 128) + 64 * g + 32);
+            wgmma_bf16<COUT>(acc[m], al, bh, kb > 0 || g > 0);
+            wgmma_bf16<COUT>(acc[m], ah, bl, 1);
+            wgmma_bf16<COUT>(acc[m], ah, bh, 1);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (kb > 0 && lane == 0) mbar_arrive(bars + 8 * (S + (it - 1) % S));
+      }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int m = 0; m < MT; ++m) wgmma_pin(acc[m]);
+      if (lane == 0) mbar_arrive(bars + 8 * (S + (it - 1) % S));
+
+      // ------------------------------- epilogue of the tile ----------------------------------------
+      // fragment of block m: rows 16 warp + lane / 4 (+ 8), columns 8 i + 2 (lane % 4) (+ 1)
+      constexpr int SW = Sh::kSlice, LD = Sh::kLd, CH = SW / 16;
+      float *buf = epi + (cw * 4 + warp) * 16 * LD;
+#pragma unroll
+      for (int m = 0; m < MT; ++m) {
+        const int rbase = tile * TM + cw * (MT * 64) + 64 * m + 16 * warp;
+#pragma unroll
+        for (int c0 = 0; c0 < COUT; c0 += SW) {
+#pragma unroll
+          for (int i = 0; i < SW / 8; ++i) {
+            const int r = lane >> 2, c = 8 * i + 2 * (lane & 3), q = 4 * (c0 / 8 + i);
+            *reinterpret_cast<float2 *>(buf + r * LD + c) = make_float2(acc[m][q], acc[m][q + 1]);
+            *reinterpret_cast<float2 *>(buf + (r + 8) * LD + c) = make_float2(acc[m][q + 2], acc[m][q + 3]);
+          }
+          __syncwarp();
+          const int r = lane / CH, j = lane % CH;
+          if (lane < 16 * CH && rbase + r < n_out) {
+            float v[16];
+#pragma unroll
+            for (int e = 0; e < 16; e += 4) {
+              const float4 q = *reinterpret_cast<const float4 *>(buf + r * LD + 16 * j + e);
+              v[e] = q.x; v[e + 1] = q.y; v[e + 2] = q.z; v[e + 3] = q.w;
+            }
+            v6_store_chunk<16>(p, v, rbase + r, c0 + 16 * j);
+          }
+          __syncwarp();
+        }
+      }
+    }
+  }
+}
+
 // ---- operand images --------------------------------------------------------------------------
 // fp32 rows [n, c_in] -> split image [n, c_eff * 4 B], c_eff = c_in rounded up to 16 (zero padded).
 // One thread per (row, 8 channels): 16 B of hi and 16 B of lo.
@@ -362,7 +530,7 @@ __global__ void spconv_v6_split_rows_kernel(const float *__restrict__ in, int n_
   }
 }
 
-// Weight image of the three-product form (Cout = 128): one stage per 32-wide K block, row n =
+// Weight image of the three-product form: one stage (Cout rows of 128 B, contiguous) per 32-wide K block, row n =
 // [W_hi kk 0-15 | W_hi kk 16-31 | W_lo kk 0-15 | W_lo kk 16-31] (32 B each), SWIZZLE_128B.
 __global__ void spconv_v6_pack_rows_kernel(const float *__restrict__ w, int kvol, int c_in, int c_in_eff,
                                            int c_out, int nkb, uint16_t *__restrict__ packed) {
@@ -388,32 +556,6 @@ __global__ void spconv_v6_pack_rows_kernel(const float *__restrict__ w, int kvol
   }
 }
 
-// Merged weight image (Cout <= 64), the layout generation 5 uses: [nb64][hi | lo][Cout][64 bf16]; K index
-// kk = kb64*64 + c, 16-byte chunk (c / 8) XOR (n & 7), element (c % 8) inside the chunk.  One stage
-// (hi image then lo image, 2 * Cout rows of 128 B) serves two 32-wide K blocks.
-__global__ void spconv_v6_pack_merged_kernel(const float *__restrict__ w, int kvol, int c_in, int c_in_eff,
-                                             int c_out, int nb64, uint16_t *__restrict__ packed) {
-  const long long total = (long long)nb64 * c_out * 64;
-  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total;
-       t += (long long)gridDim.x * blockDim.x) {
-    const int c = (int)(t % 64);
-    const int n = (int)((t / 64) % c_out);
-    const int kb = (int)(t / (64ll * c_out));
-    const int kk = kb * 64 + c;
-    const int k = kk / c_in_eff, ci = kk % c_in_eff;
-    const float v = (k < kvol && ci < c_in) ? w[((long long)k * c_in + ci) * c_out + n] : 0.f;
-    uint32_t u = __float_as_uint(v);
-    u += 0x7fffu + ((u >> 16) & 1u);
-    const uint32_t hb = u >> 16;
-    const float lo = v - __uint_as_float(hb << 16);
-    uint32_t ul = __float_as_uint(lo);
-    ul += 0x7fffu + ((ul >> 16) & 1u);
-    const int pos = n * 64 + ((((c >> 3) ^ (n & 7)) << 3) | (c & 7));
-    packed[((long long)kb * 2 + 0) * c_out * 64 + pos] = (uint16_t)hb;
-    packed[((long long)kb * 2 + 1) * c_out * 64 + pos] = (uint16_t)(ul >> 16);
-  }
-}
-
 int spconv_v6_cin_eff(int c_in) {
   for (int e = 16; e <= 128; e <<= 1)
     if (c_in <= e) return e;
@@ -427,22 +569,14 @@ static int v6_nkb(int c_eff, int kvol) { return (kvol * c_eff + 31) / 32; }
 
 size_t spconv_v6_packed_bytes(int c_in, int c_out, int kvol) {
   if (!spconv_v6_shape_ok(c_in, c_out, kvol)) return 0;
-  const int nkb = v6_nkb(spconv_v6_cin_eff(c_in), kvol);
-  if (c_out <= 64) return (size_t)((nkb + 1) / 2) * 2 * c_out * 128;
-  return (size_t)nkb * c_out * 128;
+  return (size_t)v6_nkb(spconv_v6_cin_eff(c_in), kvol) * c_out * 128;
 }
 
 int spconv_v6_pack_weights(const float *weight, int c_in, int c_out, int kvol, void *packed, cudaStream_t st) {
   const int ce = spconv_v6_cin_eff(c_in);
   const int nkb = v6_nkb(ce, kvol);
-  if (c_out <= 64) {
-    const int nb64 = (nkb + 1) / 2;
-    BEVB200_LAUNCH(spconv_v6_pack_merged_kernel, grid_for((long long)nb64 * c_out * 64, 256), 256, 0, st,
-                   weight, kvol, c_in, ce, c_out, nb64, (uint16_t *)packed);
-  } else {
-    BEVB200_LAUNCH(spconv_v6_pack_rows_kernel, grid_for((long long)nkb * c_out * 32, 256), 256, 0, st, weight,
-                   kvol, c_in, ce, c_out, nkb, (uint16_t *)packed);
-  }
+  BEVB200_LAUNCH(spconv_v6_pack_rows_kernel, grid_for((long long)nkb * c_out * 32, 256), 256, 0, st, weight, kvol,
+                 c_in, ce, c_out, nkb, (uint16_t *)packed);
   return BEVB200_OK;
 }
 
@@ -501,6 +635,35 @@ static int v6_launch(const V6Params &p, cudaStream_t st) {
   BEVB200_REQUIRE(false, "output channel count has no tensor-core form");
 }
 
+template <int COUT>
+static int wg_launch_one(const V6Params &p, cudaStream_t st) {
+  using Sh = WgShape<COUT>;
+  const int n_tiles = (p.n_out + Sh::kTileM - 1) / Sh::kTileM;
+  BEVB200_CUDA(cudaFuncSetAttribute(spconv_wg_kernel<COUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, Sh::kSmem));
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3((unsigned)(n_tiles < kNumSMs ? n_tiles : kNumSMs));
+  cfg.blockDim = dim3((unsigned)kWgThreads);
+  cfg.dynamicSmemBytes = Sh::kSmem;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  BEVB200_CUDA(cudaLaunchKernelEx(&cfg, spconv_wg_kernel<COUT>, p));
+  ++g_launch_count;
+  return BEVB200_OK;
+}
+
+static int wg_launch(const V6Params &p, cudaStream_t st) {
+  switch (p.c_out) {
+    case 64: return wg_launch_one<64>(p, st);
+    case 128: return wg_launch_one<128>(p, st);
+  }
+  BEVB200_REQUIRE(false, "output channel count has no tensor-core form");
+}
+
 static void v6_common(V6Params &p, const void *rows, const void *packed, const int32_t *nbr, long long nbr_stride,
                       int n_in, int n_out, const int32_t *n_out_dev, int c_in, int c_out, int kvol, const float *scale,
                       const float *shift, const float *residual, int relu, float *out) {
@@ -549,7 +712,10 @@ int spconv_v6_forward_ex(const void *features_split, const void *packed, const i
             residual, relu, out);
   p.residual_split = (const uint8_t *)residual_split;
   p.out_split = (uint8_t *)out_split;
-  return v6_launch<0>(p, st);
+  // The warpgroup-MMA kernel wins where the tensor work per gathered row is large (Cout >= 64) and a tile has K
+  // blocks enough to amortise its pipeline fill and epilogue.  At Cout <= 32 the row gather bounds both kernels
+  // and two mma.sync CTAs per SM keep more of it in flight; the k(1,1,3) conv_out (12 K blocks) is faster there too.
+  return p.c_out >= 64 && p.nkb >= kWgMinKBlocks ? wg_launch(p, st) : v6_launch<0>(p, st);
 }
 
 // TF32 (tf32x3 = false) / 3xTF32 forward on zero-padded fp32 rows [n_in][c_in] (c_in a power of two, 8 .. 128) and

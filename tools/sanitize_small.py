@@ -23,7 +23,7 @@ flat = rng.choice(vol, size=n, replace=False)
 idx = np.stack([flat // (shape[0] * shape[1] * shape[2]), (flat // (shape[1] * shape[2])) % shape[0],
                 (flat // shape[2]) % shape[1], flat % shape[2]], 1).astype(np.int32)
 ti = torch.from_numpy(idx).to(dev)
-for (cin, cout) in ((16, 32), (64, 64), (5, 16)):
+for (cin, cout) in ((16, 32), (64, 64), (5, 16), (64, 128)):
     f = torch.randn(n, cin, device=dev)
     for subm, ks, st, pd in ((True, 3, 1, 1), (False, 3, 2, 1), (False, [1, 1, 3], [1, 1, 2], 0)):
         rb, _ = ops.get_rulebook(ti, Bn, shape, ks, st, pd, 1, 0, subm)
