@@ -162,25 +162,6 @@ int spconv_forward_simt(const float *features, const float *weight, const int32_
   return BEVB200_EUNSUPPORTED;
 }
 
-// ---- dense() ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-    sparse_to_dense_kernel(const float *__restrict__ features, const int32_t *__restrict__ indices,
-                           int n, int c, int batch, int X, int Y, int Z, int z_major,
-                           long long out_batch_stride, float *__restrict__ out) {
-  // grid (row tiles, channel groups): a thread handles one site and the channels ch0, ch0+gridDim.y, ..
-  // (site fastest across the warp: neighbouring sites -> nearby stores; no per-element division)
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const int4 p = *reinterpret_cast<const int4 *>(indices + 4ll * i);  // (b, x, y, z)
-    if ((unsigned)p.x >= (unsigned)batch || (unsigned)p.y >= (unsigned)X ||
-        (unsigned)p.z >= (unsigned)Y || (unsigned)p.w >= (unsigned)Z)
-      continue;
-    const long long site = z_major ? ((long long)p.w * X + p.y) * Y + p.z : ((long long)p.y * Y + p.z) * Z + p.w;
-    const long long plane = (long long)X * Y * Z;
-    float *o = out + p.x * out_batch_stride + site;
-    for (int ch = blockIdx.y; ch < c; ch += gridDim.y) o[ch * plane] = features[(long long)i * c + ch];
-  }
-}
-
 }  // namespace bevb200
 
 using namespace bevb200;
@@ -249,29 +230,6 @@ int bevb200_spconv_forward_packed(const float *features, const float *packed_wei
   return spconv_forward_tc(features, nullptr, packed_weight, nbr, n_in, n_out, c_in, c_out,
                            kernel_volume, scale, shift, residual, relu, precision, out,
                            (cudaStream_t)stream);
-}
-
-int bevb200_sparse_to_dense(const float *features, const int32_t *indices, int n, int c,
-                            int batch_size, const int32_t *spatial_shape_host, int z_major,
-                            long long out_batch_stride, float *out, void *stream) {
-  BEVB200_REQUIRE(n >= 0 && c > 0 && batch_size > 0 && spatial_shape_host && out, "bad argument");
-  const int X = spatial_shape_host[0], Y = spatial_shape_host[1], Z = spatial_shape_host[2];
-  BEVB200_REQUIRE(X > 0 && Y > 0 && Z > 0, "bad spatial shape");
-  cudaStream_t st = (cudaStream_t)stream;
-  const long long per_batch = (long long)c * X * Y * Z;
-  if (out_batch_stride == 0) out_batch_stride = per_batch;
-  BEVB200_REQUIRE(out_batch_stride >= per_batch, "output batch stride too small");
-  if (out_batch_stride == per_batch) {
-    BEVB200_CUDA(cudaMemsetAsync(out, 0, (size_t)batch_size * per_batch * sizeof(float), st));
-  } else {  // channel slice of a wider [B, C_total, ...] buffer (the fuser's concatenated input)
-    BEVB200_CUDA(cudaMemset2DAsync(out, (size_t)out_batch_stride * sizeof(float), 0,
-                                   (size_t)per_batch * sizeof(float), batch_size, st));
-  }
-  if (n == 0) return BEVB200_OK;
-  BEVB200_REQUIRE(features && indices, "null argument");
-  BEVB200_LAUNCH(sparse_to_dense_kernel, dim3(grid_for(n, 256, kNumSMs), c < 32 ? c : 32), 256, 0, st,
-                 features, indices, n, c, batch_size, X, Y, Z, z_major, out_batch_stride, out);
-  return BEVB200_OK;
 }
 
 }  // extern "C"

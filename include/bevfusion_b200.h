@@ -353,13 +353,18 @@ BEVB200_API int bevb200_dynamic_scatter_backward(const float *grad_reduced_feats
  *
  * Two calls because the number of outputs of a strided conv is data dependent:
  *   1. bevb200_rulebook_prepare: marks the active output sites in a bitmap over the
- *      dense output grid, ranks them, and writes n_out (device int32[1]).  SubM:
+ *      dense output grid, ranks them with a single-pass scan (bits and popcount prefix
+ *      interleaved per 32 sites), and writes n_out (device int32[1]).  SubM:
  *      n_out = n_in and the output sites are the input sites in input order
  *      (spconv_ops.h:76-101).  Strided: output rows are ordered by ascending flat index
  *      ((b*X + x)*Y + y)*Z + z -- the order of the reference's GPU path after
  *      torch::_unique (spconv_ops.h:130-136, indice.cu.h:112-127).
  *   2. bevb200_rulebook_fill: writes out_indices [n_out, 4] (b, x, y, z) and
- *      nbr [K, n_out] using the state left in `workspace` by step 1.
+ *      nbr [K, n_out] using the state left in `workspace` by step 1.  SubM gathers each
+ *      output's neighbours from the bitmap.  Strided scatters from the inputs, as the
+ *      reference does, so an input row just outside the input grid still feeds the
+ *      border outputs it reaches.
+ * The encoder plan (bevb200_encoder_forward) builds its rulebooks with the same kernels.
  */
 BEVB200_API size_t bevb200_rulebook_workspace_bytes(int n_in, int batch_size, const int32_t *out_shape_host);
 BEVB200_API int bevb200_rulebook_prepare(const int32_t *indices, int n_in, int batch_size,
@@ -406,15 +411,16 @@ BEVB200_API int bevb200_pairs_to_nbr(const int32_t *indice_pairs, const int32_t 
  *     y += residual[o, c]                (SparseBasicBlock identity, sparse_block.py:105)
  *     y = max(y, 0) if relu
  * precision: BEVB200_PREC_FP32  exact fp32 FFMA accumulation (SIMT)
- *            BEVB200_PREC_TF32X3 tcgen05 tensor cores, 3xTF32 split (fp32-class accuracy)
- *            BEVB200_PREC_TF32   tcgen05 single-pass TF32 (fast mode, ~1e-3 rel)
- *            BEVB200_PREC_BF16X3 tcgen05 bf16 hi/lo split: half the MMAs and operand bytes of TF32X3,
- *                                per-product error ~2^-17 (measured ~1e-5 relative per layer)
+ *            BEVB200_PREC_TF32X3 mma.sync tensor cores, 3xTF32 split (fp32-class accuracy)
+ *            BEVB200_PREC_TF32   mma.sync single-pass TF32 (fast mode, ~1e-3 rel)
+ *            BEVB200_PREC_BF16X3 bf16 hi/lo split on mma.sync (wgmma for c_out 64 / 128 with >= 16 K blocks of 32):
+ *                                half the MMAs and operand bytes of TF32X3, per-product error ~2^-17
+ *                                (measured ~1e-5 relative per layer)
  */
 #define BEVB200_PREC_FP32 0
 #define BEVB200_PREC_TF32X3 1
 #define BEVB200_PREC_TF32 2
-#define BEVB200_PREC_BF16X3 3 /* tcgen05 kind::f16: a = bf16 hi + bf16 lo, hi*hi + hi*lo + lo*hi (3 MMAs per 16 K) */
+#define BEVB200_PREC_BF16X3 3 /* bf16 MMAs: a = bf16 hi + bf16 lo, hi*hi + hi*lo + lo*hi (3 MMAs per 16 K) */
 BEVB200_API int bevb200_spconv_forward(const float *features, const float *weight, const int32_t *nbr,
                            int n_in, int n_out, int c_in, int c_out, int kernel_volume,
                            const float *scale, const float *shift, const float *residual,

@@ -144,6 +144,17 @@ def test_rulebook_edge_cases(cuda):
     assert num.cpu().tolist() == [0] * 13 + [1] + [0] * 13
     rb, _ = ops.get_rulebook(one, 1, [8, 8, 4], 3, 2, 1, 1, 0, False)
     assert rb.n_out == 1 and rb.outids.cpu().tolist() == [[0, 0, 0, 0]]
+    # a row one step outside the grid: a strided conv scatters from its inputs like the reference, so the row
+    # still feeds the border output it reaches; SubM finds in-grid neighbours of it but never the row itself
+    outside = torch.tensor([[0, -1, 0, 0], [0, 0, 0, 0]], dtype=torch.int32, device=cuda)
+    rb, _ = ops.get_rulebook(outside[:1], 1, [8, 8, 4], 3, 2, 1, 1, 0, False)
+    nbr = rb.nbr.cpu().numpy()
+    assert rb.n_out == 1 and rb.outids.cpu().tolist() == [[0, 0, 0, 0]]
+    assert nbr[4, 0] == 0 and (np.delete(nbr[:, 0], 4) == -1).all()
+    rb, _ = ops.get_rulebook(outside, 1, [8, 8, 4], 3, 1, 1, 1, 0, True)
+    nbr = rb.nbr.cpu().numpy()
+    assert nbr[22, 0] == 1 and (np.delete(nbr[:, 0], 22) == -1).all()
+    assert nbr[13, 1] == 1 and (np.delete(nbr[:, 1], 13) == -1).all()
     # fully dense block: every interior voxel has 27 neighbours
     dense = random_sparse(6 * 6 * 6, [6, 6, 6], 1, seed=0)
     rb, _ = ops.get_rulebook(torch.from_numpy(dense).to(cuda), 1, [6, 6, 6], 3, 1, 1, 1, 0, True)

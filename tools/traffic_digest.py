@@ -45,7 +45,7 @@ def total(pred):
     return sum(g["bytes"] for n, g in groups.items() if pred(n))
 out = {"source": "profiles/r2_launches.md (ncu launch list of tools/frame_once.py, commit %s)" % commit,
        "spconv_bytes": total(lambda n: n.startswith("spconv_v6_kernel")),
-       "encoder_bytes": total(lambda n: n.startswith(("spconv_v6", "enc_"))),
+       "encoder_bytes": total(lambda n: n.startswith(("spconv_v6", "enc_", "rb_", "sparse_to_dense"))),
        "bev_pool_plan_bytes": total(lambda n: n.startswith(("bevpool_fwd_tma", "pool_interval_cells"))),
        "spconv_share_of_frame": round(sum(g["us"] for n, g in groups.items() if n.startswith("spconv_v6_kernel")) / total_us, 4)}
 json.dump(out, open("profiles/r2_traffic.json", "w"), indent=1)
