@@ -485,12 +485,20 @@ BEVB200_API int bevb200_spconv_forward_split(const void *features_split, const v
  *     weight_grad[k]    = sum_o features[nbr[k, o], :]^T (x) out_grad[o, :] [K, c_in, c_out]
  * nbr_t [K, n_in] is the transposed neighbour table from bevb200_rulebook_transpose()
  * (nbr_t[k, j] = the output row that input row j feeds through offset k, or -1).
+ * Precondition: each input row feeds at most one output per offset (nbr[k, :] holds no valid row twice), as in
+ * every rulebook of a sparse conv; the transpose keeps one writer per (k, j) and is undefined otherwise.
+ * Entries of nbr outside [0, n_in) are missing neighbours.  input_grad and weight_grad are overwritten, not
+ * accumulated into; an input row that feeds no output gets 0 and an offset without pairs gets dW[k] = 0.
  * The input gradient runs the forward implicit-GEMM kernel on (out_grad, W^T, nbr_t) in the
  * requested precision.  The weight gradient sums chunks of rows into per-chunk partials and adds those in
- * ascending chunk order: no atomics, bit-reproducible run to run -- on the tensor cores for BEVB200_PREC_BF16X3 /
- * _TF32 and c_in, c_out in {32, 64, 128} (spconv_wgrad_tc.cu: mma.sync on ldmatrix.trans fragments of the bf16 hi/lo
- * images of the gathered feature rows and the out-grad rows; BEVB200_WGRAD_TC=0 keeps the SIMT kernel), else SIMT.
- * workspace: bevb200_spconv_backward_workspace_bytes() (the transposed weights, the operand images, the partials). */
+ * ascending chunk order: no atomics, bit-reproducible run to run.  It runs on the tensor cores
+ * (spconv_wgrad_tc.cu: mma.sync on ldmatrix.trans fragments of the bf16 hi/lo images of the gathered feature rows
+ * and the out-grad rows) when precision is BEVB200_PREC_BF16X3 or BEVB200_PREC_TF32, 1 <= c_in <= 128,
+ * c_out in {16, 32, 64, 128}, kernel_volume <= 27 and features and out_grad are 16-byte aligned; everything else,
+ * and BEVB200_WGRAD_TC=0, takes the exact-fp32 SIMT kernels.  So BEVB200_PREC_TF32 computes dW at BF16x3-class
+ * accuracy (~1e-5 relative); only its input gradient is single-pass TF32.
+ * workspace: bevb200_spconv_backward_workspace_bytes() (the transposed weights, the operand images, the partials);
+ * a smaller workspace returns BEVB200_EWORKSPACE. */
 BEVB200_API int bevb200_rulebook_transpose(const int32_t *nbr, int kernel_volume, int n_out, int n_in,
                                int32_t *nbr_t, void *stream);
 BEVB200_API size_t bevb200_spconv_backward_workspace_bytes(int n_in, int n_out, int c_in, int c_out, int kernel_volume);
