@@ -12,7 +12,7 @@ HEADER_PATH = os.path.join(_HERE, "..", "include", "bevfusion_b200.h")
 
 _lib = None
 
-c_void_p, c_int, c_size_t = ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t
+c_void_p, c_int, c_size_t, c_float = ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t, ctypes.c_float
 _P = c_void_p  # every device / host pointer is passed as an address
 
 # symbol -> (restype, argtypes); kept in the same order as the header
@@ -58,6 +58,11 @@ _SIGNATURES = {
                                                  c_int, _P, _P]),
     "bevb200_dynamic_voxelize": (c_int, [_P, c_int, c_int, _P, _P, _P, _P]),
     "bevb200_voxel_mean": (c_int, [_P, _P, _P] + [c_int] * 4 + [_P, _P, _P]),
+    "bevb200_pillar_packed_bytes": (c_size_t, [c_int] * 3),
+    "bevb200_pillar_pack_weights": (c_int, [_P] * 6 + [c_int] * 3 + [_P, _P]),
+    "bevb200_pillar_features": (c_int, [_P, _P, _P, c_int, _P, c_int, c_int] + [c_float] * 4 + [_P, _P, _P]),
+    "bevb200_hard_voxelize_pillars": (c_int, [_P, c_int, c_int, _P, _P, c_int, c_int] + [c_float] * 4
+                                      + [_P, _P, c_int, c_int, _P, _P, c_size_t, _P]),
     "bevb200_rulebook_workspace_bytes": (c_size_t, [c_int, c_int, _P]),
     "bevb200_rulebook_prepare": (c_int, [_P, c_int, c_int] + [_P] * 6 + [c_int, _P, _P, c_size_t, _P]),
     "bevb200_rulebook_fill": (c_int, [_P, c_int, c_int] + [_P] * 6 + [c_int, c_int, _P, _P, _P,

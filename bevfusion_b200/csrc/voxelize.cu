@@ -18,31 +18,12 @@
 //   K4 (scan)       exclusive popcount scan over the ballot words = first-appearance order
 //   K5 vox_scatter  voxel id = rank of its first point; slot = position in the list; copy the
 //                   point row, write coors / num_points (only voxel id < max_voxels).
-#include "common.cuh"
+#include "voxelize.cuh"
 
 namespace bevb200 {
 
 constexpr unsigned long long kEmptyKey = 0xffffffffffffffffull;
 constexpr int kListEmpty = 0x7f7f7f7f;  // memset(0x7f) pattern, larger than any point index
-
-struct VoxParams {
-  float vs[3], lo[3];
-  int grid[3];
-};
-
-__device__ __forceinline__ bool point_coords(const float *__restrict__ p, const VoxParams &vp,
-                                             int c[3]) {
-  bool ok = true;
-#pragma unroll
-  for (int k = 0; k < 3; ++k) {
-    // voxelization_cuda.cu:37,43,50: floor((p - min) / voxel) evaluated in fp32
-    float v = floorf(__fdiv_rn(__fsub_rn(p[k], vp.lo[k]), vp.vs[k]));
-    // out-of-range (and NaN) points are dropped; compare in float so huge values cannot wrap
-    ok = ok && (v >= 0.f) && (v < (float)vp.grid[k]);
-    c[k] = ok ? (int)v : -1;
-  }
-  return ok;
-}
 
 __device__ __forceinline__ uint32_t hash64(unsigned long long k) {
   k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
@@ -238,7 +219,7 @@ __global__ void voxel_mean_kernel(const float *__restrict__ voxels,
   }
 }
 
-static int make_params(const float *vs, const float *range, VoxParams *vp) {
+int make_params(const float *vs, const float *range, VoxParams *vp) {
   for (int k = 0; k < 3; ++k) {
     vp->vs[k] = vs[k];
     vp->lo[k] = range[k];
@@ -248,14 +229,6 @@ static int make_params(const float *vs, const float *range, VoxParams *vp) {
   }
   return 0;
 }
-
-struct VoxWs {
-  unsigned long long *keys;
-  int32_t *slot_pvid, *point_slot, *point_pvid, *lists, *counts, *pvid_counter;
-  uint32_t *first_bits, *word_prefix, *tiles, *total;
-  uint32_t table_size;
-  size_t nwords;
-};
 
 static size_t vox_layout(int n, int P, void *ws, size_t ws_bytes, VoxWs *out) {
   Arena a(ws, ws_bytes);
@@ -279,21 +252,9 @@ static size_t vox_layout(int n, int P, void *ws, size_t ws_bytes, VoxWs *out) {
   return a.off;
 }
 
-}  // namespace bevb200
-
-using namespace bevb200;
-
-extern "C" {
-
-size_t bevb200_hard_voxelize_workspace_bytes(int num_points, int max_points) {
-  if (num_points < 0 || max_points <= 0) return 0;
-  return vox_layout(num_points, max_points, nullptr, 0, nullptr);
-}
-
-// K1-K4, shared by the plain and the mean-fused entry points
-static int vox_front(const char *who, const float *points, int n, int num_features,
-                     const VoxParams &vp, int max_points, void *workspace, size_t workspace_bytes,
-                     cudaStream_t st, VoxWs *wout) {
+// K1-K4, shared by the plain, the mean-fused and the pillar-fused entry points
+int vox_front(const char *who, const float *points, int n, int num_features, const VoxParams &vp,
+              int max_points, void *workspace, size_t workspace_bytes, cudaStream_t st, VoxWs *wout) {
   VoxWs w;
   size_t need = vox_layout(n, max_points, workspace, workspace_bytes, &w);
   if (workspace == nullptr || workspace_bytes < need) {
@@ -317,6 +278,17 @@ static int vox_front(const char *who, const float *points, int n, int num_featur
   if (rc) return rc;
   *wout = w;
   return BEVB200_OK;
+}
+
+}  // namespace bevb200
+
+using namespace bevb200;
+
+extern "C" {
+
+size_t bevb200_hard_voxelize_workspace_bytes(int num_points, int max_points) {
+  if (num_points < 0 || max_points <= 0) return 0;
+  return vox_layout(num_points, max_points, nullptr, 0, nullptr);
 }
 
 int bevb200_hard_voxelize(const float *points, int num_points, int num_features,

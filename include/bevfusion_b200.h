@@ -290,6 +290,44 @@ BEVB200_API int bevb200_voxel_mean(const float *voxels, const int32_t *coors, co
                        int num_voxels, int max_points, int num_features, int batch_idx,
                        float *feats, int32_t *coords4, void *stream);
 
+/* ---- PointPillars pillar feature net (mmdet3d/models/backbones/pillar_encoder.py:20-258) -----------
+ * The shipped PillarFeatureNet: in_channels F, feat_channels [64, 64], with_distance False, eval-mode
+ * BN folded into per-channel scale / shift.  Per pillar v with n = num_points[v] and P slots:
+ *   rows = [raw F, xyz - sum_slots(xyz) / n, x - (cx*vx + x_off), y - (cy*vy + y_off)], slots >= n zero
+ *   x1 = relu(s1 * (rows W1^T) + t1)            [P, 32]   (a zero row gives relu(t1))
+ *   out = max_slots relu(s2 * ([x1, max_slots x1] W2^T) + t2)   [64]
+ * Padded slots take part in both maxes (a pillar with n < P has one extra row, n == P none).  Exact fp32,
+ * bit-reproducible (no atomics).
+ *
+ * bevb200_pillar_packed_bytes() is 0 unless 3 <= in_channels <= 8, c1 == 32 (layer-1 units) and c2 == 64;
+ * bevb200_pillar_pack_weights() builds the packed image from device fp32 w1 [32, F+5], w2 [64, 64]
+ * (nn.Linear layout) and the folded BN scale / shift of each layer, BEVB200_EUNSUPPORTED otherwise. */
+BEVB200_API size_t bevb200_pillar_packed_bytes(int in_channels, int c1, int c2);
+BEVB200_API int bevb200_pillar_pack_weights(const float *w1, const float *scale1, const float *shift1,
+                                const float *w2, const float *scale2, const float *shift2, int in_channels,
+                                int c1, int c2, float *packed, void *stream);
+
+/* PillarFeatureNet.forward (:141-176): voxels [cap, P, F] fp32, num_points [cap] int32 (>= 1),
+ * coords4 [cap, 4] int32 (b, x, y, z); out_rows [cap, 64] fp32.  Pillars v < min(*n_dev, cap) are
+ * computed (n_dev nullable: cap), other rows are left untouched.  1 <= P <= 32 and 3 <= F <= 8, else
+ * BEVB200_EUNSUPPORTED. */
+BEVB200_API int bevb200_pillar_features(const float *voxels, const int32_t *num_points, const int32_t *coords4,
+                            int cap, const int32_t *n_dev, int max_points, int num_features, float vx,
+                            float vy, float x_off, float y_off, const float *packed, float *out_rows,
+                            void *stream);
+
+/* Hard voxelization + pillar feature net + PointPillarsScatter for one sample: the pillars of
+ * bevb200_hard_voxelize (same order and caps) go through the net above straight from the point rows,
+ * without the [M, P, F] voxel tensor, and land in canvas [64, nx, ny] fp32 at (x, y).  The caller
+ * zeroes the canvas.  The voxel grid must be (nx, ny, 1), else BEVB200_EINVAL / BEVB200_EUNSUPPORTED.
+ * voxel_num is the device pillar count; no host synchronisation.  Workspace as bevb200_hard_voxelize. */
+BEVB200_API int bevb200_hard_voxelize_pillars(const float *points, int num_points, int num_features,
+                                  const float *voxel_size_host, const float *coors_range_host,
+                                  int max_points, int max_voxels, float vx, float vy, float x_off,
+                                  float y_off, const float *packed, float *canvas, int nx, int ny,
+                                  int32_t *voxel_num, void *workspace, size_t workspace_bytes,
+                                  void *stream);
+
 /* ---- LiDAR depth images for the depth-aware camera lift ------------------------------------
  * BaseDepthTransform.forward's per-sample loop (mmdet3d/models/vtransforms/base.py:279-329):
  * undo the lidar augmentation, project every point into every camera with lidar2image, clamp z to
