@@ -63,6 +63,14 @@ _SIGNATURES = {
     "bevb200_pillar_features": (c_int, [_P, _P, _P, c_int, _P, c_int, c_int] + [c_float] * 4 + [_P, _P, _P]),
     "bevb200_hard_voxelize_pillars": (c_int, [_P, c_int, c_int, _P, _P, c_int, c_int] + [c_float] * 4
                                       + [_P, _P, c_int, c_int, _P, _P, c_size_t, _P]),
+    "bevb200_radar_packed_bytes": (c_size_t, [c_int, c_int, _P]),
+    "bevb200_radar_pack_weights": (c_int, [_P, _P, _P, c_int, c_int, _P, _P, _P]),
+    "bevb200_radar_features_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "bevb200_radar_features": (c_int, [_P, _P, _P, c_int, _P, c_int, c_int, c_int, _P] + [c_float] * 4
+                               + [_P] * 5 + [c_size_t, _P]),
+    "bevb200_hard_voxelize_radar_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "bevb200_hard_voxelize_radar": (c_int, [_P, c_int, c_int, _P, _P, c_int, c_int, c_int, _P] + [c_float] * 4
+                                    + [_P, _P, _P, _P, c_int, c_int, _P, _P, c_size_t, _P]),
     "bevb200_rulebook_workspace_bytes": (c_size_t, [c_int, c_int, _P]),
     "bevb200_rulebook_prepare": (c_int, [_P, c_int, c_int] + [_P] * 6 + [c_int, _P, _P, c_size_t, _P]),
     "bevb200_rulebook_fill": (c_int, [_P, c_int, c_int] + [_P] * 6 + [c_int, c_int, _P, _P, _P,

@@ -154,3 +154,42 @@ def uniform_cloud(n, seed=0, margin=2.0, rng_range=(-54.0, -54.0, -5.0, 54.0, 54
     xyz = rng.uniform(lo, hi, size=(n, 3))
     extra = rng.uniform(0, 1, size=(n, nf - 3))
     return np.concatenate([xyz, extra], axis=1).astype(np.float32)
+
+
+def radar_cloud(seed=0, radars=5, sweeps=6, per_sweep=110, clusters=4, cluster_points=60, out_of_range=0.03):
+    """Synthetic nuScenes-style radar cloud [N, 45] fp32 laid out like `radar_use_dims` (loading.py:618-652):
+    x, y, z, rcs, vx_comp, vy_comp, time_diff, dynprop one-hot x8, ambig_state one-hot x5, invalid_state
+    one-hot x18, pdh0 ordinal x7.  `radars` sensors around the ego x `sweeps` sweeps of about `per_sweep`
+    returns each (a few thousand points in all), a fraction `out_of_range` outside +-51.2 m, and `clusters`
+    dense groups of `cluster_points` returns in one 0.8 m pillar each, so that some pillars exceed P = 20."""
+    rng = np.random.default_rng(seed)
+    yaws = np.deg2rad([0.0, 50.0, -50.0, 130.0, -130.0])[:radars]
+    rows = []
+    for s in range(sweeps):
+        for yaw in yaws:
+            k = rng.poisson(per_sweep)
+            az = yaw + rng.uniform(-0.6, 0.6, k)
+            r = rng.gamma(2.0, 12.0, k) + 1.0
+            rows.append(np.stack([r * np.cos(az), r * np.sin(az), rng.normal(0.5, 0.6, k),
+                                  np.full(k, 0.05 * s)], 1))
+    for c in range(clusters):
+        centre = (rng.integers(-60, 60, 2) + 0.5) * 0.8
+        off = rng.uniform(-0.35, 0.35, (cluster_points, 2))
+        rows.append(np.stack([centre[0] + off[:, 0], centre[1] + off[:, 1], rng.normal(0.5, 0.3, cluster_points),
+                              np.full(cluster_points, 0.05 * (c % sweeps))], 1))
+    base = np.concatenate(rows, 0)
+    n = base.shape[0]
+    far = rng.uniform(size=n) < out_of_range
+    base[far, :2] *= rng.uniform(1.6, 3.0, (int(far.sum()), 1))
+    rcs = rng.uniform(-10.0, 40.0, n)
+    vel = rng.normal(0.0, 3.0, (n, 2))
+    def one_hot(k, width):
+        out = np.zeros((n, width))
+        out[np.arange(n), k] = 1.0
+        return out
+    pdh = rng.integers(0, 8, n)
+    pts = np.concatenate([base[:, :3], rcs[:, None], vel, base[:, 3:4],
+                          one_hot(rng.integers(0, 8, n), 8), one_hot(rng.integers(0, 5, n), 5),
+                          one_hot(rng.integers(0, 18, n), 18),
+                          (pdh[:, None] > np.arange(7)[None, :]).astype(np.float64)], 1).astype(np.float32)
+    return pts[rng.permutation(n)]

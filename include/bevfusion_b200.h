@@ -328,6 +328,52 @@ BEVB200_API int bevb200_hard_voxelize_pillars(const float *points, int num_point
                                   int32_t *voxel_num, void *workspace, size_t workspace_bytes,
                                   void *stream);
 
+/* ---- Radar feature net (mmdet3d/models/backbones/radar_encoder.py:47-220) ---------------------------
+ * RadarFeatureNet with in_channels F and feat_channels [C_0 .. C_{L-1}], eval-mode BN folded into
+ * per-channel scale / shift.  Per pillar v with n = num_points[v], coords (b, cx, cy, z) and P slots:
+ *   row = [(xyz - pc_min) / pc_span, features 3..F-1, x - (cx*vx + x_off), y - (cy*vy + y_off)]
+ *         (the centre offsets from the raw x, y), nan_to_num (NaN -> 0, +-inf -> +-FLT_MAX)
+ *   x_{l+1} = relu(s_l * (x_l W_l^T) + t_l) for every row;   out = max over the rows   [C_{L-1}]
+ * Padded slots are zero rows: a pillar with n < P also takes the max with the "virtual" row (the zero
+ * row through every layer, computed once by the pack step), one with n == P does not.  The linears run
+ * as BF16x3 mma.sync (lo*W_hi + hi*W_lo + hi*W_hi, fp32 accumulate); the result is bit-reproducible and
+ * identical between the two forms below.  pc_min / pc_span are HOST float[3] (pc_span = pc_max - pc_min,
+ * computed in double and rounded once).
+ *
+ * bevb200_radar_packed_bytes() is 0 unless 1 <= n_layers <= 4, every width (host int[n_layers]) is a
+ * multiple of 16 in 16..128 and 3 <= in_channels <= 126; bevb200_radar_pack_weights() builds the packed
+ * image from host arrays of n_layers device pointers: weights[l] fp32 [C_l, C_{l-1}] (nn.Linear layout,
+ * C_{-1} = F + 2), scales[l] / shifts[l] fp32 [C_l].  Unsupported shapes give BEVB200_EUNSUPPORTED. */
+BEVB200_API size_t bevb200_radar_packed_bytes(int in_channels, int n_layers, const int *widths);
+BEVB200_API int bevb200_radar_pack_weights(const float *const *weights, const float *const *scales,
+                                           const float *const *shifts, int in_channels, int n_layers,
+                                           const int *widths, void *packed, void *stream);
+
+/* RadarFeatureNet.forward (:141-184): voxels [cap, P, F] fp32, num_points [cap] int32, coords4 [cap, 4]
+ * int32 (b, x, y, z); out_rows [cap, C_{L-1}] fp32 is zeroed, then pillars v < min(*n_dev, cap) are
+ * computed (n_dev nullable: cap).  Slots >= n of voxels are never read.  1 <= P <= 32, else
+ * BEVB200_EUNSUPPORTED.  Workspace: bevb200_radar_features_workspace_bytes(cap, P) device bytes. */
+BEVB200_API size_t bevb200_radar_features_workspace_bytes(int cap, int max_points);
+BEVB200_API int bevb200_radar_features(const float *voxels, const int32_t *num_points, const int32_t *coords4,
+                                       int cap, const int32_t *n_dev, int max_points, int num_features,
+                                       int n_layers, const int *widths, float vx, float vy, float x_off,
+                                       float y_off, const float *pc_min, const float *pc_span, const void *packed,
+                                       float *out_rows, void *workspace, size_t workspace_bytes, void *stream);
+
+/* Hard voxelization + radar feature net + PointPillarsScatter for one sample: the pillars of
+ * bevb200_hard_voxelize (same order and caps) go through the net above straight from the point rows,
+ * without the [M, P, F] voxel tensor, and land in canvas [C_{L-1}, nx, ny] fp32 at (x, y).  The caller
+ * zeroes the canvas.  The voxel grid must be (nx, ny, 1).  voxel_num is the device pillar count; no host
+ * synchronisation.  Workspace: bevb200_hard_voxelize_radar_workspace_bytes(num_points, P) device bytes. */
+BEVB200_API size_t bevb200_hard_voxelize_radar_workspace_bytes(int num_points, int max_points);
+BEVB200_API int bevb200_hard_voxelize_radar(const float *points, int num_points, int num_features,
+                                            const float *voxel_size_host, const float *coors_range_host,
+                                            int max_points, int max_voxels, int n_layers, const int *widths,
+                                            float vx, float vy, float x_off, float y_off, const float *pc_min,
+                                            const float *pc_span, const void *packed, float *canvas, int nx,
+                                            int ny, int32_t *voxel_num, void *workspace, size_t workspace_bytes,
+                                            void *stream);
+
 /* ---- LiDAR depth images for the depth-aware camera lift ------------------------------------
  * BaseDepthTransform.forward's per-sample loop (mmdet3d/models/vtransforms/base.py:279-329):
  * undo the lidar augmentation, project every point into every camera with lidar2image, clamp z to
