@@ -182,6 +182,9 @@ int bevb200_encoder_create(int in_channels, const int32_t *sparse_shape_host, co
     cv.c_in_eff = spconv_v6_cin_eff(cv.d.c_in);
     if (i > 0 && cv.c_in_eff != cv.d.c_in) return fail("inner channel counts must be multiples of 16");
     if (cv.d.residual_from >= i) return fail("residual_from must name an earlier conv");
+    // a level's two split images alternate conv by conv, so conv i - 3's output is overwritten by conv i - 1's
+    if (cv.d.residual_from >= 0 && cv.d.residual_from < i - 2)
+      return fail("residual_from must name one of the two previous convs");
     cv.level_in = level;
     if (!cv.d.subm) {
       ELevel nl;

@@ -610,7 +610,8 @@ BEVB200_API int bevb200_sparse_to_dense(const float *features, const int32_t *in
  *
  * A plan is a chain of convs (conv i reads the output of conv i-1): SubMConv3d or strided
  * SparseConv3d, each followed by y = acc * scale + shift (folded eval-mode BN / bias), an optional
- * residual add of the OUTPUT of an earlier conv (SparseBasicBlock identity) and an optional ReLU.
+ * residual add of the OUTPUT of one of the two previous convs (SparseBasicBlock identity) and an
+ * optional ReLU.
  * No row count ever returns to the host: buffers are sized by caps (level 0 = max_voxels; a strided
  * conv makes at most prod(ceil(k/s)) outputs per input row and one per output site; level_caps_host,
  * nullable, may tighten the caps of the levels >= 1), kernels read their counts from device memory,
@@ -633,7 +634,9 @@ typedef struct {
   int32_t ksize[3], stride[3], padding[3], dilation[3];
   int32_t subm;          /* 1: SubMConv3d (stride 1, padding k/2 forced, spconv_ops.h:74-83) */
   int32_t relu;
-  int32_t residual_from; /* -1, or j < i: add the output of conv j before the ReLU */
+  int32_t residual_from; /* -1, or j = i - 1 or i - 2 (on the same level): add the output of conv j
+                            before the ReLU.  Earlier convs are refused: each level keeps two
+                            split images, and conv j + 2 overwrites conv j's. */
 } bevb200_encoder_conv_t;
 typedef struct bevb200_encoder bevb200_encoder_t;
 BEVB200_API int bevb200_encoder_create(int in_channels, const int32_t *sparse_shape_host,

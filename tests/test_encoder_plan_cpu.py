@@ -64,6 +64,10 @@ def test_create_rejects_bad_chains():
     assert make([(5, 24, 1, -1)]) != 0                            # no tensor-core form for 24 channels
     assert make([(5, 16, 1, -1), (16, 32, 0, 0)]) != 0            # residual across levels / widths
     assert make([(5, 16, 1, 0)]) != 0                             # residual_from must be earlier
+    # a level's two split images alternate: a residual from two convs back is the furthest that survives
+    assert make([(5, 16, 1, -1), (16, 16, 1, -1), (16, 16, 1, 0)]) == 0
+    assert make([(5, 16, 1, -1), (16, 16, 1, -1), (16, 16, 1, -1), (16, 16, 1, 0)]) != 0
+    assert b"two previous convs" in L.bevb200_last_error()
 
 
 def test_unsupported_orders_fall_back():

@@ -1,7 +1,8 @@
 """GPU tests of the BF16x3 sparse-conv forward through its C entry point bevb200_spconv_forward_split, on random
 neighbour tables.  Cout >= 64 with >= 16 K blocks runs the warpgroup-MMA kernel, the rest the mma.sync kernel.
-Covered: row counts that are not a multiple of the tile, a device-side row count below the host one, each output
-alone, every Cout with Cin up to 128, the float64 oracle, and bit-reproducibility."""
+Covered: row counts that are not a multiple of the tile, a device-side row count below the host one, a neighbour
+table wider than the row count, each output alone, every Cout with Cin up to 128, the float64 oracle, and
+bit-reproducibility."""
 import pytest
 import torch
 
@@ -28,13 +29,16 @@ def _pack(w):
     return pk
 
 
-def _forward(fs, ce, pk, nbr, n_in, cout, scale, shift, residual, relu, n_dev=None, want_out=True, want_split=True):
-    """-> (fp32 rows or None, split image or None); rows not produced keep the NaN / 0xff fill"""
-    kv, n_out = nbr.shape
+def _forward(fs, ce, pk, nbr, n_in, cout, scale, shift, residual, relu, n_dev=None, want_out=True, want_split=True,
+             n_out=None):
+    """-> (fp32 rows or None, split image or None); rows not produced keep the NaN / 0xff fill.  nbr is
+    [kv, nbr_stride]; n_out (default nbr_stride) may be smaller, as in the encoder's cap-wide tables."""
+    kv, stride = nbr.shape
+    n_out = stride if n_out is None else n_out
     out = torch.full((n_out, cout), float("nan"), device=fs.device) if want_out else None
     osp = torch.full((n_out, cout * 4), 255, dtype=torch.uint8, device=fs.device) if want_split else None
     _C.check(_C.lib().bevb200_spconv_forward_split(
-        _C.ptr(fs), _C.ptr(pk), _C.ptr(nbr), n_out, n_in, n_out, _C.ptr(n_dev), ce, cout, kv, _C.ptr(scale),
+        _C.ptr(fs), _C.ptr(pk), _C.ptr(nbr), stride, n_in, n_out, _C.ptr(n_dev), ce, cout, kv, _C.ptr(scale),
         _C.ptr(shift), _C.ptr(residual), int(relu), _C.ptr(out), _C.ptr(osp), _C.current_stream(fs.device)),
         "forward_split")
     return out, osp
@@ -109,3 +113,25 @@ def test_each_output_alone_and_bit_reproducible(cout, cuda):
     gold = _oracle(f, w, nbr, scale, shift, res, False)
     err = (both_out.double() - gold).abs().max().item() / gold.abs().max().item()
     assert err <= 1e-4
+
+
+# a neighbour table wider than n_out (nbr_stride = the level's row cap, as bevb200_encoder_forward lays it out): the
+# columns past n_out hold in-range rows that must not be read
+@pytest.mark.parametrize("cin,cout,kv", [(16, 16, 27), (32, 32, 27), (16, 64, 27), (64, 64, 27), (32, 128, 27),
+                                         (128, 128, 3)])
+def test_forward_nbr_stride_wider_than_rows(cin, cout, kv, cuda):
+    n_in, n_out, stride = 1500, 1000, 1337
+    f, w, nbr, scale, shift, res = _case(cin, cout, n_in, n_out, kv, 31 * cin + cout, cuda)
+    wide = torch.randint(0, n_in, (kv, stride), device=cuda, dtype=torch.int32,
+                         generator=torch.Generator(device=cuda).manual_seed(cout))
+    wide[:, :n_out] = nbr
+    fs, ce = _split_rows(f)
+    pk = _pack(w)
+    out, osp = _forward(fs, ce, pk, wide, n_in, cout, scale, shift, res, True, n_out=n_out)
+    gold = _oracle(f, w, nbr, scale, shift, res, True)
+    torch.cuda.synchronize()
+    err = (out.double() - gold).abs().max().item() / gold.abs().max().item()
+    print(f"cin {cin} cout {cout} kvol {kv}: nbr_stride {stride} > n_out {n_out}, max rel err vs float64 {err:.2e}")
+    assert err <= 1e-4
+    dec = _decode_split(osp, cout)
+    assert ((dec - out).abs() <= out.abs() * 2.0 ** -16).all()
