@@ -217,8 +217,10 @@ __global__ void __launch_bounds__(256)
 // coalesced 16-byte-per-lane store.  An interval that crosses a warp-range boundary leaves its
 // pieces in `partial` (2 slots per range: head = continuation from the previous range, tail =
 // continues into the next) and the fix-up kernel adds them in range order: fixed summation
-// order, bit-reproducible, no float atomics.  Requires the intervals to tile [0, n) in order,
-// which is how QuickCumsumCuda (bev_pool.py:41-46) builds them; the host checks nothing else.
+// order, bit-reproducible, no float atomics.  Intervals must ascend and must not overlap.  With
+// `lengths` (MODE 0, the drop-in op) interval i covers rows [starts[i], starts[i] + lengths[i]) and
+// rows outside every interval are skipped, as in the reference kernel; MODE 1 / 2 read tables of
+// bevb200_bev_pool_prepare_*, which tile [0, n), so an interval there runs up to the next start.
 constexpr int kStageRows = 32;
 constexpr int kPoolStages = 3;
 
@@ -258,7 +260,8 @@ __global__ void __launch_bounds__(256)
                            const int32_t *__restrict__ perm, const float *__restrict__ depth, LiftDims lift,
                            const int32_t *__restrict__ starts, const int32_t *__restrict__ cells,
                            int n, int n_intervals, int rows_per_warp, int zfill, int total_cells,
-                           float4 *__restrict__ out, float4 *__restrict__ partial) {
+                           float4 *__restrict__ out, float4 *__restrict__ partial,
+                           const int32_t *__restrict__ lengths /* MODE 0 only */) {
   constexpr int QPL = (Q + 31) / 32;              // float4 columns per lane
   constexpr uint32_t kRowBytes = Q * 16;
   constexpr bool PERM = MODE == 1 || MODE == 2;   // cp.async gather with commit groups
@@ -335,6 +338,7 @@ __global__ void __launch_bounds__(256)
   for (int u = 0; u < QPL; ++u) acc[u] = make_float4(0.f, 0.f, 0.f, 0.f);
   bool open = false, head = false;   // an interval is being accumulated / it began before R0
   int cur_cell = -1;
+  int open_end = 0;                  // MODE 0: one past the last row of the open interval
   int ibase;
   {
     int i0 = find_interval(starts, n_intervals, R0);
@@ -342,7 +346,14 @@ __global__ void __launch_bounds__(256)
       ibase = i0;
     } else {
       ibase = i0 + 1;
-      if (i0 >= 0) { open = true; head = true; }
+      if (i0 >= 0) {
+        if constexpr (MODE == 0) {
+          open_end = (int)min((long long)__ldg(starts + i0) + __ldg(lengths + i0), (long long)n);
+          if (open_end > R0) { open = true; head = true; }
+        } else {
+          open = true; head = true;
+        }
+      }
     }
   }
   auto flush = [&](bool final_piece_continues) {
@@ -375,11 +386,13 @@ __global__ void __launch_bounds__(256)
   int st_n = ibase + lane < n_intervals ? __ldg(starts + ibase + lane) : 0x7fffffff;
   int cell_n = ibase + lane < n_intervals ? __ldg(cells + ibase + lane) : -1;
   int pc_n = ibase > 0 ? __ldg(cells + ibase - 1) : -1;
+  int len_n = 0;
+  if constexpr (MODE == 0) len_n = ibase + lane < n_intervals ? __ldg(lengths + ibase + lane) : 0;
   for (int it = 0; it < n_stages; ++it) {
     const int s = it % kPoolStages;
     const int r0s = R0 + it * kStageRows;
     const int nrows = min(kStageRows, R1 - r0s);
-    const int st = st_n, cellv = cell_n, prev_cell_base = pc_n;
+    const int st = st_n, cellv = cell_n, prev_cell_base = pc_n, lenv = len_n;
     const bool in_stage = st < r0s + nrows;      // st >= r0s by construction of ibase
     const uint32_t mask = __reduce_or_sync(0xffffffffu, in_stage ? (1u << (st - r0s)) : 0u);
     const int ib_cur = ibase;
@@ -388,6 +401,7 @@ __global__ void __launch_bounds__(256)
       st_n = ibase + lane < n_intervals ? __ldg(starts + ibase + lane) : 0x7fffffff;
       cell_n = ibase + lane < n_intervals ? __ldg(cells + ibase + lane) : -1;
       pc_n = ibase > 0 ? __ldg(cells + ibase - 1) : -1;
+      if constexpr (MODE == 0) len_n = ibase + lane < n_intervals ? __ldg(lengths + ibase + lane) : 0;
     }
     if constexpr (PERM) {
       asm volatile("cp.async.wait_group %0;" ::"n"(kPoolStages - 1) : "memory");
@@ -408,11 +422,22 @@ __global__ void __launch_bounds__(256)
           if (cur_cell > prevc + 1) zero_cells(prevc + 1, cur_cell);
           if (ib_cur + iv == n_intervals - 1 && cur_cell + 1 < total_cells) zero_cells(cur_cell + 1, total_cells);
         }
+        if constexpr (MODE == 0)
+          open_end = (int)min((long long)(r0s + row) + __shfl_sync(0xffffffffu, lenv, iv), (long long)n);
         ++iv;
         open = true;
       }
       const uint32_t rest = m >> 1;
-      const int run = min(nrows - row, rest ? __ffs(rest) : 32);
+      int run = min(nrows - row, rest ? __ffs(rest) : 32);
+      if constexpr (MODE == 0) {
+        // rows from open_end up to the next start lie outside every interval: skip them
+        const int left = open ? open_end - (r0s + row) : 0;
+        if (left <= 0) {
+          row += run;
+          continue;
+        }
+        run = min(run, left);
+      }
       int rr = row;
       for (; rr + 4 <= row + run; rr += 4) {
 #pragma unroll
@@ -459,7 +484,8 @@ __global__ void __launch_bounds__(256)
     commit();
   }
   // does the open interval continue into the next warp range?
-  const bool continues = R1 < n && !(ibase < n_intervals && __ldg(starts + ibase) == R1);
+  bool continues = R1 < n && !(ibase < n_intervals && __ldg(starts + ibase) == R1);
+  if constexpr (MODE == 0) continues = continues && open_end > R1;
   flush(continues);
 }
 
@@ -470,7 +496,8 @@ __global__ void bevpool_fwd_tma_fixup_kernel(const int32_t *__restrict__ starts,
                                              const int32_t *__restrict__ cells, int n,
                                              int n_intervals, int rows_per_warp, int n_ranges,
                                              float4 *__restrict__ out,
-                                             const float4 *__restrict__ partial) {
+                                             const float4 *__restrict__ partial,
+                                             const int32_t *__restrict__ lengths /* MODE 0 only */) {
   const int lane = lane_id();
   const int wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
   for (int j = wid; j < n_ranges; j += nw) {
@@ -479,7 +506,8 @@ __global__ void bevpool_fwd_tma_fixup_kernel(const int32_t *__restrict__ starts,
     const int iv = find_interval(starts, n_intervals, (int)R1 - 1);
     if (iv < 0) continue;
     const int s = __ldg(starts + iv);
-    const int e = iv + 1 < n_intervals ? __ldg(starts + iv + 1) : n;   // intervals tile [0, n)
+    const int e = lengths ? (int)min((long long)s + __ldg(lengths + iv), (long long)n)
+                          : (iv + 1 < n_intervals ? __ldg(starts + iv + 1) : n);   // tables that tile [0, n)
     if (s < R0 || e <= R1) continue;               // not the owner, or it ends inside the range
     const int cell = __ldg(cells + iv);
     if (cell < 0) continue;
@@ -671,9 +699,11 @@ static int launch_fwd(const float *x, const int32_t *perm, const int32_t *geom,
 
 template <int Q>
 static int launch_fwd_tma(const float *x, const int32_t *perm, const int32_t *geom,
-                          const int32_t *starts, int n, int c, int n_intervals, PoolDims dm, float *out,
-                          void *ws, int zfill, cudaStream_t st, const float *depth = nullptr,
-                          LiftDims lift = LiftDims{1, 1}) {
+                          const int32_t *starts, const int32_t *lengths, int n, int c, int n_intervals,
+                          PoolDims dm, float *out, void *ws, int zfill, cudaStream_t st,
+                          const float *depth = nullptr, LiftDims lift = LiftDims{1, 1}) {
+  // MODE 1 / 2 tables tile [0, n): their interval ends are the next starts
+  const int32_t *mode0_lengths = (depth == nullptr && perm == nullptr) ? lengths : nullptr;
   size_t nchunks = ((size_t)n + kChunkRows - 1) / kChunkRows;
   if (nchunks < (size_t)kTmaMaxRanges) nchunks = kTmaMaxRanges;
   float *partial = (float *)ws;
@@ -696,14 +726,14 @@ static int launch_fwd_tma(const float *x, const int32_t *perm, const int32_t *ge
                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));      \
     BEVB200_LAUNCH((bevpool_fwd_tma_kernel<Q, MODE>), grid, warps * 32, smem, st, (const float4 *)x,       \
                    perm, depth, lift, starts, cells, n, n_intervals, rpw, zfill,  \
-                   dm.b * dm.d * dm.h * dm.w, (float4 *)out, (float4 *)partial);                     \
+                   dm.b * dm.d * dm.h * dm.w, (float4 *)out, (float4 *)partial, mode0_lengths);      \
   } while (0)
   if (depth) BEVB200_POOL_TMA_LAUNCH(2);
   else if (perm) BEVB200_POOL_TMA_LAUNCH(1);
   else BEVB200_POOL_TMA_LAUNCH(0);
 #undef BEVB200_POOL_TMA_LAUNCH
   BEVB200_LAUNCH((bevpool_fwd_tma_fixup_kernel<Q>), (n_ranges * 32 + 255) / 256, 256, 0, st, starts, cells, n,
-                 n_intervals, rpw, n_ranges, (float4 *)out, (const float4 *)partial);
+                 n_intervals, rpw, n_ranges, (float4 *)out, (const float4 *)partial, mode0_lengths);
   return BEVB200_OK;
 }
 
@@ -754,26 +784,29 @@ static int pool_forward(int b, int d, int h, int w, int n, int c, int n_interval
   // zero-fills the empty cells itself; every other case pre-zeroes the grid
   bool tuned = false;
   switch (c) { case 16: case 32: case 64: case 80: case 96: case 128: case 160: case 256: tuned = true; }
-  const bool aligned16 = ((uintptr_t)x % 16 == 0) && ((uintptr_t)out % 16 == 0);
-  const int zfill = (perm != nullptr && b * d == 1 && n > 0 && n_intervals > 0 && tuned && aligned16 &&
-                     g_pool_variant == 0 && trust_tables) ? 1 : 0;
+  const bool aligned = ((uintptr_t)x % 16 == 0) && ((uintptr_t)out % 16 == 0);
+  const bool work = n > 0 && n_intervals > 0;
+  // every argument is checked before `out` is written: a refused call leaves it untouched
+  if (work) {
+    BEVB200_REQUIRE(x && geom && starts && lengths, "null input");
+    if (tuned && aligned && (ws == nullptr || ws_bytes < pool_partial_bytes(n, c))) {
+      snprintf(g_last_error, sizeof(g_last_error), "bev_pool: workspace too small (%zu < %zu)", ws_bytes,
+               pool_partial_bytes(n, c));
+      return BEVB200_EWORKSPACE;
+    }
+  }
+  const int zfill = (perm != nullptr && b * d == 1 && work && tuned && aligned && g_pool_variant == 0 &&
+                     trust_tables) ? 1 : 0;
   if (!zfill) BEVB200_CUDA(cudaMemsetAsync(out, 0, out_bytes, st));
-  if (n == 0 || n_intervals == 0) return BEVB200_OK;
-  BEVB200_REQUIRE(x && geom && starts && lengths, "null input");
+  if (!work) return BEVB200_OK;
   PoolDims dm{b, d, h, w};
   int rc = BEVB200_OK;
-  bool aligned = ((uintptr_t)x % 16 == 0) && ((uintptr_t)out % 16 == 0);
 #define CALL_FWD(Q, G)                                                                         \
   do {                                                                                         \
-    if (ws_bytes < pool_partial_bytes(n, c) || ws == nullptr) {                                \
-      snprintf(g_last_error, sizeof(g_last_error), "bev_pool: workspace too small (%zu < %zu)", \
-               ws_bytes, pool_partial_bytes(n, c));                                            \
-      return BEVB200_EWORKSPACE;                                                               \
-    }                                                                                          \
     if (g_pool_variant == 1)                                                                   \
       rc = launch_fwd<Q, G>(x, perm, geom, starts, lengths, n, n_intervals, dm, out, (float *)ws, st); \
     else                                                                                       \
-      rc = launch_fwd_tma<Q>(x, perm, geom, starts, n, c, n_intervals, dm, out, ws, zfill, st);  \
+      rc = launch_fwd_tma<Q>(x, perm, geom, starts, lengths, n, c, n_intervals, dm, out, ws, zfill, st); \
   } while (0)
 #define CALL_FWD_GENERIC()                                                                     \
   do {                                                                                         \
@@ -1072,8 +1105,8 @@ int bevb200_bev_pool_lift(int b, int d, int h, int w, int n, int c, int n_interv
   }
   PoolDims dm{b, d, h, w};
   LiftDims lift{depth_bins, pixels_per_camera};
-#define CALL_LIFT(Q, G) return launch_fwd_tma<Q>(ctx, perm, geom_feats, interval_starts, n, c, n_intervals, dm, \
-                                                 out, workspace, zfill, st, depth, lift)
+#define CALL_LIFT(Q, G) return launch_fwd_tma<Q>(ctx, perm, geom_feats, interval_starts, nullptr, n, c, n_intervals, \
+                                                 dm, out, workspace, zfill, st, depth, lift)
   BEVB200_POOL_DISPATCH(c, CALL_LIFT, BEVB200_REQUIRE(false, "bev_pool_lift: channel count not in {16,32,64,80,96,128,160,256}"));
 #undef CALL_LIFT
   return BEVB200_OK;

@@ -579,7 +579,8 @@ int bevb200_bev_pool_lift_columns(int b, int d, int h, int w, int n, int c, int 
   BEVB200_REQUIRE(c % 4 == 0 && c <= 256, "channel count must be a multiple of 4, <= 256");
   BEVB200_REQUIRE((long long)b * d * h * w < (1ll << 31), "grid has too many cells");
   cudaStream_t st = (cudaStream_t)stream;
-  const int zfill = (b * d == 1 && n > 0 && n_intervals > 0) ? 1 : 0;
+  // with no segment the cells kernel does not run, so nothing would zero-fill the grid
+  const int zfill = (b * d == 1 && n > 0 && n_intervals > 0 && n_segments > 0) ? 1 : 0;
   if (!zfill) BEVB200_CUDA(cudaMemsetAsync(out, 0, (size_t)b * d * h * w * c * sizeof(float), st));
   if (n == 0 || n_intervals == 0 || n_segments == 0) return BEVB200_OK;
   BEVB200_REQUIRE(depth && ctx && geom_feats && interval_starts && col_begin && seg_key && seg_mask && seg_slot &&

@@ -57,13 +57,19 @@ BEVB200_API void bevb200_reset_launch_count(void);
  * (bev_pool_cuda.cu:86-90, called from bev_pool_forward bev_pool_cpu.cpp:22-47).
  *   x               [n, c] fp32, rows sorted by rank (the op's contract)
  *   geom_feats      [n, 4] int32 (x, y, z, b) of each sorted row
- *   interval_starts [n_intervals], interval_lengths [n_intervals] int32
+ *   interval_starts [n_intervals], interval_lengths [n_intervals] int32; interval i is
+ *                   rows [starts[i], starts[i] + lengths[i]) of x, and the cell of its
+ *                   first row receives their sum.  Intervals ascend and do not overlap,
+ *                   but need not tile [0, n): rows outside every interval contribute
+ *                   nothing.  A row whose geom_feats lies outside the grid heads no cell.
  *   out             [b, d, h, w, c] fp32; EVERY element is written (cells without an
  *                   interval get 0), so the caller need not pre-zero it
  * Differences from the reference launcher: runs on `stream` (the reference uses the
  * legacy default stream, bev_pool_cuda.cu:88); sums each interval with a fixed
  * chunked order (deterministic run to run).
- * workspace: bevb200_bev_pool_workspace_bytes(n, c). */
+ * workspace: bevb200_bev_pool_workspace_bytes(n, c); a smaller one gives
+ * BEVB200_EWORKSPACE.  A call refused with BEVB200_EINVAL or BEVB200_EWORKSPACE leaves
+ * `out` untouched. */
 BEVB200_API size_t bevb200_bev_pool_workspace_bytes(int n, int c);
 BEVB200_API int bevb200_bev_pool(int b, int d, int h, int w, int n, int c, int n_intervals,
                      const float *x, const int32_t *geom_feats,
