@@ -99,7 +99,8 @@ __device__ __forceinline__ float nan_to_num(float v) {
 
 struct __align__(16) RfnWarpSmem {
   uint8_t act[2 * kRfnPlane];  // split image [hi | lo][16 rows][kRfnPitch B]; the last layer's fp32 rows
-  int row[16], out[16], cxy[16];
+  int row[16], out[16];
+  int2 cxy[16];
 };
 
 // One layer on the warp's 16 rows: D[16, N] = A[16, K] W^T in BF16x3 (lo*W_hi + hi*W_lo + hi*W_hi, fp32
@@ -165,7 +166,7 @@ __device__ __forceinline__ void rfn_layer_n(int n, RfnWarpSmem &s, int ksteps, c
   }
 }
 
-// Row table entry: {row index into `rows` (F floats each), output pillar index, cx << 16 | cy, 0}.
+// Row table entry: {row index into `rows` (F floats each), output pillar index, cx, cy}.
 // out[pillar * ps + c * cs] (rows form: [M, C], ps = C, cs = 1; canvas: ps = 1, cs = nx * ny).  The shape and
 // geometry stay in parameter space (__grid_constant__): indexing them by layer needs no local copy.
 __global__ void __launch_bounds__(kRfnWarps * 32)
@@ -190,7 +191,7 @@ __global__ void __launch_bounds__(kRfnWarps * 32)
       const int4 e = j < total ? table[j] : make_int4(0, -1, 0, 0);
       s.row[lane] = e.x;
       s.out[lane] = e.y;
-      s.cxy[lane] = e.z;
+      s.cxy[lane] = make_int2(e.z, e.w);
     }
     __syncwarp();
     // decorate the 16 rows into the split image; lane = column (point rows are 4 * F bytes, not 16-byte
@@ -199,7 +200,7 @@ __global__ void __launch_bounds__(kRfnWarps * 32)
     for (int r = 0; r < 16; ++r) {
       const bool ok = s.out[r] >= 0;
       const float *p = rows + (long long)s.row[r] * F;
-      const int cxy = s.cxy[r];
+      const int2 cxy = s.cxy[r];
       for (int k = lane; k < k0; k += 32) {
         float v = 0.f;
         if (ok) {
@@ -212,7 +213,7 @@ __global__ void __launch_bounds__(kRfnWarps * 32)
             }
           } else if (k < F + 2) {
             // coors * v + offset, two roundings as in the reference (no contraction into an FMA)
-            const float c = k == F ? (float)(cxy >> 16) : (float)(int16_t)(cxy & 0xffff);
+            const float c = (float)(k == F ? cxy.x : cxy.y);
             const float ctr = __fadd_rn(__fmul_rn(c, k == F ? g.vx : g.vy), k == F ? g.x_off : g.y_off);
             v = __fsub_rn(p[k - F], ctr);
           }
@@ -258,7 +259,7 @@ __global__ void __launch_bounds__(kRfnWarps * 32)
 // atomic, every pillar's rows land consecutively, and pillars with n < P fold the virtual row into out.
 // `row0` is the pillar's first row index (rows form) or, with `lists`, the slot-list base (fused form).
 __device__ __forceinline__ void rfn_fill_table(int lane, int cnt, bool virt, int row0, const int32_t *lists,
-                                               int out_idx, int cxy, int4 *__restrict__ table,
+                                               int out_idx, int cx, int cy, int4 *__restrict__ table,
                                                uint32_t *__restrict__ total_rows, const float *__restrict__ vrow,
                                                int C, float *__restrict__ out, long long ps, long long cs) {
   int incl = cnt;
@@ -276,9 +277,9 @@ __device__ __forceinline__ void rfn_fill_table(int lane, int cnt, bool virt, int
   for (int p = 0; p < 32; ++p) {
     const int pc = __shfl_sync(0xffffffffu, cnt, p), pf = __shfl_sync(0xffffffffu, first, p);
     const int pr = __shfl_sync(0xffffffffu, row0, p), po = __shfl_sync(0xffffffffu, out_idx, p);
-    const int pxy = __shfl_sync(0xffffffffu, cxy, p);
+    const int px = __shfl_sync(0xffffffffu, cx, p), py = __shfl_sync(0xffffffffu, cy, p);
     const bool pv = __shfl_sync(0xffffffffu, (int)virt, p) != 0;
-    if (lane < pc) table[pf + lane] = make_int4(lists ? lists[pr + lane] : pr + lane, po, pxy, 0);
+    if (lane < pc) table[pf + lane] = make_int4(lists ? lists[pr + lane] : pr + lane, po, px, py);
     if (pv)
       for (int c = lane; c < C; c += 32) {
         const int b = __float_as_int(vrow[c]);
@@ -297,15 +298,16 @@ __global__ void radar_rows_table_kernel(const int32_t *__restrict__ num_points, 
   const int stride = gridDim.x * blockDim.x;
   for (int v0 = blockIdx.x * blockDim.x + (threadIdx.x & ~31); v0 < m; v0 += stride) {
     const int v = v0 + lane;
-    int cnt = 0, cxy = 0;
+    int cnt = 0, cx = 0, cy = 0;
     bool virt = false;
     if (v < m) {
       const int n = num_points[v];
       cnt = min(max(n, 0), P);
       virt = n < P;
-      cxy = (coords4[4ll * v + 1] << 16) | (coords4[4ll * v + 2] & 0xffff);
+      cx = coords4[4ll * v + 1];
+      cy = coords4[4ll * v + 2];
     }
-    rfn_fill_table(lane, cnt, virt, v * P, nullptr, v, cxy, table, total_rows, vrow, C, out, C, 1);
+    rfn_fill_table(lane, cnt, virt, v * P, nullptr, v, cx, cy, table, total_rows, vrow, C, out, C, 1);
   }
 }
 
@@ -327,18 +329,16 @@ __global__ void radar_points_table_kernel(const float *__restrict__ points, int 
     const uint32_t bits = first_bits[wd];
     const uint32_t vid = word_prefix[wd] + __popc(bits & ((1u << lane) - 1u));
     const long long i = wd * 32 + lane;
-    int cnt = 0, cxy = 0, row0 = 0, cell = 0;
+    int cnt = 0, c[3] = {0, 0, 0}, row0 = 0, cell = 0;
     if (((bits >> lane) & 1u) && vid < (uint32_t)max_voxels && i < n_points) {
       const int pv = point_pvid[i];
       cnt = min(counts[pv], P);
-      int c[3];
       point_coords(points + i * F, vp, c);
-      cxy = (c[0] << 16) | (c[1] & 0xffff);
       cell = c[0] * vp.grid[1] + c[1];
       row0 = pv * P;
     }
-    rfn_fill_table(lane, cnt, cnt > 0 && cnt < P, row0, lists, cell, cxy, table, total_rows, vrow, C, canvas, 1,
-                   plane);
+    rfn_fill_table(lane, cnt, cnt > 0 && cnt < P, row0, lists, cell, c[0], c[1], table, total_rows, vrow, C, canvas,
+                   1, plane);
   }
 }
 
@@ -494,7 +494,6 @@ int bevb200_hard_voxelize_radar(const float *points, int num_points, int num_fea
   BEVB200_REQUIRE(make_params(voxel_size_host, coors_range_host, &vp) == 0, "bad voxel grid");
   BEVB200_RADAR_UNSUPPORTED(vp.grid[2] == 1, "radar pillars need a voxel grid one cell high");
   BEVB200_REQUIRE(vp.grid[0] == nx && vp.grid[1] == ny, "canvas shape differs from the voxel grid");
-  BEVB200_REQUIRE(nx <= 32767 && ny <= 32767, "grid too large");
   cudaStream_t st = (cudaStream_t)stream;
   const int n = num_points;
   if (n == 0) {

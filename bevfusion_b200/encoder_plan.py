@@ -7,7 +7,7 @@ import ctypes
 import torch
 
 from . import _C
-from .sparse_block import SparseBasicBlock, bn_scale_shift
+from .sparse_block import SparseBasicBlock, bn_fold_key, bn_scale_shift
 
 
 class _ConvDesc(ctypes.Structure):
@@ -100,12 +100,11 @@ class EncoderPlan:
 
     # -- parameters: packed once, re-packed when a weight / BN tensor changes -------------------
     def _sync_params(self, dev):
-        tensors = []
+        key = (str(dev),)
         for conv, bn, _, _ in self.chain:
-            tensors += [conv.weight, conv.bias]
+            key += tuple((t.data_ptr(), t._version) for t in (conv.weight, conv.bias) if t is not None)
             if bn is not None:
-                tensors += [bn.weight, bn.bias, bn.running_mean, bn.running_var]
-        key = (str(dev),) + tuple((t.data_ptr(), t._version) for t in tensors if t is not None)
+                key += bn_fold_key(bn)
         if key == self._param_key:
             return
         L = _C.lib()

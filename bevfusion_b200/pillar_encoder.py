@@ -18,7 +18,7 @@ from torch.autograd import Function
 from torch.nn import functional as F
 
 from . import _C
-from .sparse_block import bn_scale_shift, build_norm_layer
+from .sparse_block import bn_fold_key, bn_scale_shift, build_norm_layer
 from .spconv.ops import sparse_to_dense
 from .voxelize import Voxelization, _floats
 
@@ -104,10 +104,8 @@ class PillarFeatureNet(nn.Module):
     def packed_weights(self):
         """Native weight image (folded BN), rebuilt only when a parameter or statistic changes."""
         l1, l2 = self.pfn_layers
-        tensors = [l1.linear.weight, l2.linear.weight]
-        for bn in (l1.norm, l2.norm):
-            tensors += [t for t in (bn.weight, bn.bias, bn.running_mean, bn.running_var) if t is not None]
-        key = tuple((t.data_ptr(), t._version) for t in tensors)
+        key = tuple((w.data_ptr(), w._version) for w in (l1.linear.weight, l2.linear.weight))
+        key += bn_fold_key(l1.norm) + bn_fold_key(l2.norm)
         if self._packed_cache is not None and self._packed_cache[0] == key:
             return self._packed_cache[1]
         dev = l1.linear.weight.device

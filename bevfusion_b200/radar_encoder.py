@@ -24,7 +24,7 @@ from torch.nn import functional as F
 
 from . import _C
 from .pillar_encoder import PointPillarsScatter, get_paddings_indicator
-from .sparse_block import bn_scale_shift, build_norm_layer
+from .sparse_block import bn_fold_key, bn_scale_shift, build_norm_layer
 from .voxelize import Voxelization, _floats
 
 __all__ = ["RFNLayer", "RadarFeatureNet", "RadarEncoder"]
@@ -101,12 +101,9 @@ class RadarFeatureNet(nn.Module):
     def packed_weights(self):
         """Native weight image (bf16 hi | lo fragments, folded BN, the virtual row), rebuilt only when
         a parameter or statistic changes."""
-        tensors = []
+        key = ()
         for l in self.rfn_layers:
-            tensors.append(l.linear.weight)
-            tensors += [t for t in (l.norm.weight, l.norm.bias, l.norm.running_mean, l.norm.running_var)
-                        if t is not None]
-        key = tuple((t.data_ptr(), t._version) for t in tensors)
+            key += ((l.linear.weight.data_ptr(), l.linear.weight._version),) + bn_fold_key(l.norm)
         if self._packed_cache is not None and self._packed_cache[0] == key:
             return self._packed_cache[1]
         w0 = self.rfn_layers[0].linear.weight

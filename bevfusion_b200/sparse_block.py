@@ -30,11 +30,21 @@ def build_norm_layer(cfg, num_features, postfix=""):
     return "bn" + str(postfix), layer
 
 
+def bn_fold_key(bn):
+    """Cache key of the folded (scale, shift) of a BatchNorm: (data_ptr, _version) of every tensor that
+    defines it.  A train-mode forward updates running_mean / running_var in place without bumping their
+    version counters (the BN kernels' schemas do not mark them as mutated), but it does increment
+    num_batches_tracked, so that counter is part of the key.  In-place writes through `.data` (e.g.
+    `bn.running_mean.data.copy_(x)`) bypass the version counter and are not tracked; assigning a new
+    tensor, or writing in place under torch.no_grad(), is."""
+    tensors = (bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.num_batches_tracked)
+    return tuple((t.data_ptr(), t._version) for t in tensors if t is not None)
+
+
 def bn_scale_shift(bn):
     """Fold an eval-mode BatchNorm1d into per-channel (scale, shift); cached on the module until
-    one of its parameters / buffers changes."""
-    tensors = [t for t in (bn.weight, bn.bias, bn.running_mean, bn.running_var) if t is not None]
-    key = tuple((t.data_ptr(), t._version) for t in tensors)
+    one of its parameters / buffers changes (bn_fold_key)."""
+    key = bn_fold_key(bn)
     cached = getattr(bn, "_b200_fold", None)
     if cached is not None and cached[0] == key:
         return cached[1]

@@ -70,6 +70,27 @@ def test_create_rejects_bad_chains():
     assert b"two previous convs" in L.bevb200_last_error()
 
 
+def test_bn_fold_follows_train_mode_statistics():
+    """A train-mode BN forward moves running_mean / running_var in place; the cached fold (bn_scale_shift, and the
+    caches keyed on bn_fold_key) must see it even though no optimizer step touched a parameter."""
+    import torch
+    from bevfusion_b200.sparse_block import _bn_scale_shift, bn_fold_key, bn_scale_shift
+    g = torch.Generator().manual_seed(0)
+    bn = torch.nn.BatchNorm1d(16, eps=1e-3, momentum=0.01).eval()
+    s0, t0 = (v.clone() for v in bn_scale_shift(bn))
+    key = bn_fold_key(bn)
+    bn.train()
+    with torch.no_grad():
+        bn(torch.randn(256, 16, generator=g) * 3.0 + 2.0)
+    bn.eval()
+    assert bn_fold_key(bn) != key
+    s1, t1 = bn_scale_shift(bn)
+    es, et = _bn_scale_shift(bn)
+    assert torch.equal(s1, es) and torch.equal(t1, et)
+    assert not torch.equal(s1, s0) and not torch.equal(t1, t0)
+    assert bn_scale_shift(bn)[0] is s1                             # unchanged statistics: the cached fold
+
+
 def test_unsupported_orders_fall_back():
     enc = SparseEncoder(5, [64, 64, 9], order=("norm", "act", "conv"))
     assert not supported(enc)

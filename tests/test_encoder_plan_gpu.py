@@ -10,7 +10,8 @@
     ops.get_rulebook tables: residuals from one and two convs back and on the last conv, an all-SubM chain and a
     strided first conv.  (A residual from further back is refused by bevb200_encoder_create:
     test_encoder_plan_cpu.py.)
-  * The packed parameters follow the module: after a training step and after load_state_dict."""
+  * The packed parameters follow the module: after a training step, after load_state_dict, and after train-mode
+    forwards that move only the BN statistics (also through the per-conv loop)."""
 import copy
 import ctypes
 
@@ -96,12 +97,15 @@ def odd_coors(shape, B, n, seed, empty=1):
 
 
 def twin_of(m):
-    """eval-mode float64 copy of m (without its native plan, which owns a C handle)"""
+    """eval-mode float64 copy of m (without its native plan, which owns a C handle, nor its rulebook side streams)"""
     plan, m._plan = m._plan, None
+    streams = m.__dict__.pop("_rulebook_streams", None)
     try:
         t = copy.deepcopy(m)
     finally:
         m._plan = plan
+        if streams is not None:
+            m._rulebook_streams = streams
     return t.double().eval()
 
 
@@ -184,6 +188,32 @@ def test_plan_follows_parameter_updates(cuda):
 
     m.load_state_dict(voxelnet(shape, seed=10).state_dict())
     check_plan(m, feats, coors, B, "after load_state_dict")
+
+
+@pytest.mark.parametrize("path", ["loop", "plan"])
+def test_bn_refold_after_train_mode_forward(cuda, path):
+    """eval forward, train-mode forwards under no_grad (BN recalibration: the statistics move, no parameter does), eval
+    again: the per-conv loop (bn_scale_shift) and the native plan (its packed parameters) follow the new statistics."""
+    shape, B = [64, 56, 41], 2
+    m = voxelnet(shape, seed=12).to(cuda)
+    m.native_plan = path == "plan"
+    coors = torch.from_numpy(random_coors([64, 56, 40], B, 4000, seed=13)).to(cuda)
+    feats = torch.randn(coors.shape[0], 5, device=cuda, generator=torch.Generator(device=cuda).manual_seed(14))
+    m.eval()
+    with torch.no_grad():
+        before = m(feats, coors, B).clone()
+        m.train()
+        for _ in range(3):
+            m(feats, coors, B)
+        m.eval()
+        got = m(feats, coors, B)
+    assert bool(m._plan) == (path == "plan")
+    want, _, _ = encoder_forward(twin_of(m), feats.double(), coors, B)
+    moved = float((want - before.double()).abs().max() / want.abs().max())
+    err = float((got.double() - want).abs().max() / want.abs().max())
+    print("%s: the train-mode forwards moved the output by %.2e, rel err %.2e" % (path, moved, err))
+    assert moved > 1e-3, "the statistics moved too little for a stale fold to show"
+    assert err <= 1e-4, "%s: rel err %.3e after the statistics moved" % (path, err)
 
 
 # ---------------------------------------------------------------------------------------------------- raw C ABI
