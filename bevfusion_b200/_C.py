@@ -71,6 +71,10 @@ _SIGNATURES = {
     "bevb200_hard_voxelize_radar_workspace_bytes": (c_size_t, [c_int, c_int]),
     "bevb200_hard_voxelize_radar": (c_int, [_P, c_int, c_int, _P, _P, c_int, c_int, c_int, _P] + [c_float] * 4
                                     + [_P, _P, _P, _P, c_int, c_int, _P, _P, c_size_t, _P]),
+    "bevb200_boxes_iou_bev": (c_int, [_P, c_int, _P, c_int, _P, _P]),
+    "bevb200_boxes_overlap_bev": (c_int, [_P, c_int, _P, c_int, _P, _P]),
+    "bevb200_nms_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "bevb200_nms": (c_int, [_P, _P, c_int, c_int, c_int, ctypes.c_double, c_int, _P, _P, _P, _P, c_size_t, _P]),
     "bevb200_rulebook_workspace_bytes": (c_size_t, [c_int, c_int, _P]),
     "bevb200_rulebook_prepare": (c_int, [_P, c_int, c_int] + [_P] * 6 + [c_int, _P, _P, c_size_t, _P]),
     "bevb200_rulebook_fill": (c_int, [_P, c_int, c_int] + [_P] * 6 + [c_int, c_int, _P, _P, _P,

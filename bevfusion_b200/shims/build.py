@@ -1,5 +1,5 @@
-"""Build the three drop-in pybind modules (`bev_pool_ext`, `voxel_layer`, `sparse_conv_ext`: the names the
-reference's python wrappers import, mmdet3d/ops/{bev_pool,voxel,spconv}) in-tree, linked against
+"""Build the four drop-in pybind modules (`bev_pool_ext`, `voxel_layer`, `sparse_conv_ext`, `iou3d_cuda`: the
+names the reference's python wrappers import, mmdet3d/ops/{bev_pool,voxel,spconv,iou3d}) in-tree, linked against
 libbevfusion_b200.so.  Plain C++ (no .cu): every call forwards to the C ABI."""
 import os
 import sys
@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 LIB_DIR = os.path.join(os.path.dirname(HERE), "lib")
 OUT_DIR = os.path.join(LIB_DIR, "shims")
-MODULES = ("bev_pool_ext", "voxel_layer", "sparse_conv_ext")
+MODULES = ("bev_pool_ext", "voxel_layer", "sparse_conv_ext", "iou3d_cuda")
 
 
 def so_path(name):

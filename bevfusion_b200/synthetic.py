@@ -193,3 +193,56 @@ def radar_cloud(seed=0, radars=5, sweeps=6, per_sweep=110, clusters=4, cluster_p
                           one_hot(rng.integers(0, 18, n), 18),
                           (pdh[:, None] > np.arange(7)[None, :]).astype(np.float64)], 1).astype(np.float32)
     return pts[rng.permutation(n)]
+
+
+# CenterHead tasks of the nuScenes configs (centerhead/default.yaml: tasks) with typical (w, l, h) in metres
+CENTERHEAD_TASKS = [
+    [("car", (1.95, 4.6, 1.7))],
+    [("truck", (2.5, 6.9, 2.8)), ("construction_vehicle", (2.9, 6.4, 3.2))],
+    [("bus", (2.9, 11.5, 3.5)), ("trailer", (2.9, 12.0, 3.9))],
+    [("barrier", (2.5, 0.5, 1.0))],
+    [("motorcycle", (0.8, 2.1, 1.5)), ("bicycle", (0.6, 1.8, 1.3))],
+    [("pedestrian", (0.7, 0.7, 1.8)), ("traffic_cone", (0.3, 0.3, 1.1))],
+]
+# the box post-processing part of test_cfg (centerhead/default.yaml, lssfpn/camera+radar/default.yaml)
+CENTERHEAD_TEST_CFG = dict(post_center_limit_range=[-61.2, -61.2, -10.0, 61.2, 61.2, 10.0], max_per_img=500,
+                           min_radius=[4, 12, 10, 1, 0.85, 0.175], score_threshold=0.1, pre_max_size=1000,
+                           post_max_size=83, nms_thr=0.2)
+CENTERHEAD_RADAR_NMS_TYPE = ["circle", "rotate", "rotate", "circle", "rotate", "rotate"]
+CENTERHEAD_RADAR_NMS_SCALE = [[1.0], [1.0, 1.0], [1.0, 1.0], [1.0], [1.0, 1.0], [2.5, 4.0]]
+
+
+def centerhead_detections(seed=0, batch=1, max_num=500):
+    """What CenterPointBBoxCoder.decode hands to the NMS step, per task and sample: a list over the six
+    tasks of a list over samples of dict(bboxes [n, 9] fp32 (x, y, z, w, l, h, yaw, vx, vy), scores [n]
+    fp32, labels [n] int64).  30-80 objects per (task, sample), each seen as 4-10 jittered candidates
+    (n capped at max_num, the coder's max_num), centres within +-61 m, yaw in [-pi, pi), scores distinct,
+    in random order and spread over (0.02, 0.97), so that some fall below the 0.1 score threshold."""
+    rng = np.random.default_rng(seed)
+    out = []
+    for classes in CENTERHEAD_TASKS:
+        task = []
+        for _ in range(batch):
+            rows, labels = [], []
+            for _ in range(int(rng.integers(30, 81))):
+                lab = int(rng.integers(len(classes)))
+                w, l, h = np.array(classes[lab][1]) * rng.uniform(0.85, 1.15, 3)
+                x, y = rng.uniform(-61.0, 61.0, 2)
+                z, yaw = rng.uniform(-2.0, 1.0), rng.uniform(-math.pi, math.pi)
+                vx, vy = rng.normal(0, 3, 2)
+                for _ in range(int(rng.integers(4, 11))):
+                    jit = rng.normal(0, 1, 9) * [0.15 * w, 0.15 * l, 0.1, 0.05 * w, 0.05 * l, 0.05 * h, 0.15,
+                                                 0.3, 0.3]
+                    rows.append(np.array([x, y, z, w, l, h, yaw, vx, vy]) + jit)
+                    labels.append(lab)
+            n = min(len(rows), max_num)
+            pick = rng.permutation(len(rows))[:n]
+            b = np.array(rows)[pick]
+            b[:, :2] = b[:, :2].clip(-61.0, 61.0)
+            b[:, 6] = (b[:, 6] + math.pi) % (2 * math.pi) - math.pi
+            scores = (rng.permutation(n) + rng.uniform(0.05, 0.95, n)) / n * 0.95 + 0.02
+            task.append(dict(bboxes=torch.from_numpy(b.astype(np.float32)),
+                             scores=torch.from_numpy(scores.astype(np.float32)),
+                             labels=torch.from_numpy(np.array(labels)[pick].astype(np.int64))))
+        out.append(task)
+    return out

@@ -380,6 +380,50 @@ BEVB200_API int bevb200_hard_voxelize_radar(const float *points, int num_points,
                                             int ny, int32_t *voxel_num, void *workspace, size_t workspace_bytes,
                                             void *stream);
 
+/* ---- Rotated BEV IoU and NMS (mmdet3d/ops/iou3d/src/{iou3d.cpp,iou3d_kernel.cu},
+ *      core/post_processing/box3d_nms.py:180-219 circle_nms) ----------------------------------------
+ * Boxes are [x1, y1, x2, y2, ry] fp32 (xywhr2xyxyr form): the axis-aligned extent turned by ry about its
+ * centre, x' = (x-cx) cos r + (y-cy) sin r + cx, y' = -(x-cx) sin r + (y-cy) cos r + cy
+ * (iou3d_kernel.cu:116-124).  overlap = area of the convex intersection polygon (strict edge crossings,
+ * corners inside the other box within 1e-5); iou = overlap / max(sa + sb - overlap, 1e-8) with sa, sb the
+ * unrotated extents' areas (:249-256).  A box with a NaN coordinate overlaps nothing (IoU 0).  fp32: the
+ * value differs from the reference's own fp32 arithmetic in the last bits (DESIGN.md section 4.13). */
+
+/* boxes_overlap_bev_gpu / boxes_iou_bev_gpu (iou3d.cpp:48-94): a [na, 5], b [nb, 5] fp32 ->
+ * out [na, nb] fp32 row-major, every element written.  na <= 1,048,560, else BEVB200_EINVAL. */
+BEVB200_API int bevb200_boxes_iou_bev(const float *a, int na, const float *b, int nb, float *out, void *stream);
+BEVB200_API int bevb200_boxes_overlap_bev(const float *a, int na, const float *b, int nb, float *out,
+                                          void *stream);
+
+/* Greedy NMS over S independent segments (one (task, sample) box list each), replacing nms_gpu /
+ * nms_normal_gpu (iou3d.cpp:96-210, host loop :132-145) and circle_nms, in two launches and without
+ * host synchronisation or allocation:
+ *   boxes      [S, nmax, D] fp32, each segment sorted by descending score; D = 5 ([x1, y1, x2, y2, ry])
+ *              for ROTATE and NORMAL, D = 2 (centre x, y) for CIRCLE
+ *   counts     [S] int32 device, boxes of segment s are rows [0, counts[s]) (clamped to [0, nmax]);
+ *              nullable: every segment holds nmax
+ *   mode       ROTATE: pair (i, j) suppressed when rotated iou > (float)thresh (iou3d_kernel.cu:300);
+ *              NORMAL: the axis-aligned iou of :335-343 (ry ignored) > (float)thresh;
+ *              CIRCLE: fp32 dx*dx + dy*dy <= thresh compared in double (box3d_nms.py:213-216; thresh is
+ *              the config's min_radius, compared with the squared distance as the reference does)
+ *   order      [S, nmax] int64 device, nullable: keep holds order[s, i] instead of the sorted position i
+ *   keep       [S, post_max] int64 device: kept boxes in score order, the first keep_count[s] entries of
+ *              the greedy keep list, the rest -1.  keep_count [S] int32 device = min(kept, post_max).
+ * The result equals the reference's host loop bit for bit for the same suppression mask.  An empty
+ * segment gives keep_count 0.  nmax <= BEVB200_NMS_MAX_BOXES (the suppression bitmap lives in shared
+ * memory) and S <= BEVB200_NMS_MAX_SEGMENTS, else BEVB200_EUNSUPPORTED.  Workspace (the pair mask,
+ * S * nmax * ceil(nmax / 64) * 8 bytes): bevb200_nms_workspace_bytes(S, nmax), 0 for unsupported sizes;
+ * a smaller one gives BEVB200_EWORKSPACE. */
+#define BEVB200_NMS_ROTATE 0
+#define BEVB200_NMS_NORMAL 1
+#define BEVB200_NMS_CIRCLE 2
+#define BEVB200_NMS_MAX_BOXES 65536
+#define BEVB200_NMS_MAX_SEGMENTS 65535
+BEVB200_API size_t bevb200_nms_workspace_bytes(int S, int nmax);
+BEVB200_API int bevb200_nms(const float *boxes, const int32_t *counts, int S, int nmax, int mode, double thresh,
+                            int post_max, const int64_t *order, int64_t *keep, int32_t *keep_count,
+                            void *workspace, size_t workspace_bytes, void *stream);
+
 /* ---- LiDAR depth images for the depth-aware camera lift ------------------------------------
  * BaseDepthTransform.forward's per-sample loop (mmdet3d/models/vtransforms/base.py:279-329):
  * undo the lidar augmentation, project every point into every camera with lidar2image, clamp z to
