@@ -23,23 +23,9 @@
 #include <vector>
 
 #include "rulebook.cuh"
+#include "spconv.cuh"
 
 namespace bevb200 {
-
-int spconv_v6_cin_eff(int c_in);
-bool spconv_v6_shape_ok(int c_in, int c_out, int kvol);
-size_t spconv_v6_packed_bytes(int c_in, int c_out, int kvol);
-int spconv_v6_pack_weights(const float *weight, int c_in, int c_out, int kvol, void *packed, cudaStream_t st);
-int spconv_v6_split_rows(const float *features, int n_cap, const int32_t *n_dev, int c_in, void *split,
-                         cudaStream_t st);
-int spconv_v6_forward_ex(const void *features_split, const void *packed, const int32_t *nbr, long long nbr_stride,
-                         int n_in, int n_out, const int32_t *n_out_dev, int c_in, int c_out, int kvol,
-                         const float *scale, const float *shift, const float *residual, const void *residual_split,
-                         int relu, float *out, void *out_split, cudaStream_t st);
-int spconv_v6_forward(const void *features_split, const void *packed, const int32_t *nbr, long long nbr_stride,
-                      int n_in, int n_out, const int32_t *n_out_dev, int c_in, int c_out, int kvol,
-                      const float *scale, const float *shift, const float *residual, int relu, float *out,
-                      void *out_split, cudaStream_t st);
 
 __global__ void enc_set_count_kernel(int32_t *dst, int value) { *dst = value; }
 
@@ -385,7 +371,7 @@ int bevb200_encoder_forward(bevb200_encoder_t *e, const void *params, const floa
   if (forked) BEVB200_CUDA(cudaEventRecord(e->events[1 + nr], ss));
 
   // ------------------------------ features (stream st) -------------------------------------
-  int rc = spconv_v6_split_rows(voxel_features, caps[0], n_voxels_dev, e->in_channels, w.split[0][0], st);
+  int rc = spconv_v6_split_rows(voxel_features, caps[0], n_voxels_dev, e->in_channels, e->c0_eff, w.split[0][0], st);
   if (rc) return rc;
   std::vector<int> split_turn(nl, 0), f32_turn(nl, 0);
   split_turn[0] = 1;
@@ -418,11 +404,11 @@ int bevb200_encoder_forward(bevb200_encoder_t *e, const void *params, const floa
     const float *res = cv.d.residual_from >= 0 ? f32_of[cv.d.residual_from] : nullptr;
     const uint8_t *res_split = (cv.d.residual_from >= 0 && res == nullptr) ? split_of[cv.d.residual_from] : nullptr;
     BEVB200_REQUIRE(cv.d.residual_from < 0 || res || res_split, "residual source has no rows");
-    rc = spconv_v6_forward_ex(cur_split, pbase + cv.packed_off, w.nbr[cv.rulebook], (long long)caps[lo], caps[cv.level_in],
-                              caps[lo], w.counts[lo], cv.c_in_eff, cv.d.c_out, cv.kvol,
-                              cv.has_scale ? (const float *)(pbase + cv.scale_off) : nullptr,
-                              cv.has_shift ? (const float *)(pbase + cv.shift_off) : nullptr, res, res_split, cv.d.relu,
-                              of32, osplit, st);
+    rc = spconv_v6_forward(cur_split, pbase + cv.packed_off, w.nbr[cv.rulebook], (long long)caps[lo], caps[cv.level_in],
+                           caps[lo], w.counts[lo], cv.c_in_eff, cv.d.c_out, cv.kvol,
+                           cv.has_scale ? (const float *)(pbase + cv.scale_off) : nullptr,
+                           cv.has_shift ? (const float *)(pbase + cv.shift_off) : nullptr, res, res_split, cv.d.relu,
+                           of32, osplit, st);
     if (rc) return rc;
     split_of[i] = osplit;
     cur_split = osplit;

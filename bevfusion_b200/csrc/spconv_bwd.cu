@@ -11,30 +11,9 @@
 //     partial; a second kernel adds the partials of every element in ascending chunk order.  The
 //     result is bit-reproducible run to run (the reference's cuBLAS GEMM per offset is too; the
 //     round-1 version with fp32 atomicAdd was not).
-#include "common.cuh"
+#include "spconv.cuh"
 
 namespace bevb200 {
-
-int spconv_forward_simt(const float *features, const float *weight, const int32_t *nbr, int n_in,
-                        int n_out, int c_in, int c_out, int kvol, const float *scale,
-                        const float *shift, const float *residual, int relu, float *out,
-                        cudaStream_t st);
-bool spconv_wgrad_tc_ok(int c_in, int c_out, int kvol);
-const void *spconv_wgrad_tc_grad_image(const void *workspace, int n_in, int c_in);
-bool spconv_tc_runs_on_split_images(int c_in, int c_out, int kvol, int precision);
-size_t spconv_v6_packed_bytes(int c_in, int c_out, int kvol);
-int spconv_v6_pack_weights(const float *weight, int c_in, int c_out, int kvol, void *packed, cudaStream_t st);
-int spconv_v6_forward(const void *features_split, const void *packed, const int32_t *nbr, long long nbr_stride,
-                      int n_in, int n_out, const int32_t *n_out_dev, int c_in, int c_out, int kvol,
-                      const float *scale, const float *shift, const float *residual, int relu, float *out,
-                      void *out_split, cudaStream_t st);
-size_t spconv_wgrad_tc_workspace_bytes(int n_in, int n_out, int c_in, int c_out, int kvol);
-int spconv_wgrad_tc(const float *features, const float *out_grad, const int32_t *nbr, int n_in, int n_out,
-                    int c_in, int c_out, int kvol, float *weight_grad, void *workspace, cudaStream_t st);
-int spconv_forward_tc(const float *features, const float *weight, const float *packed,
-                      const int32_t *nbr, int n_in, int n_out, int c_in, int c_out, int kvol,
-                      const float *scale, const float *shift, const float *residual, int relu,
-                      int precision, float *out, cudaStream_t st);
 
 __global__ void nbr_transpose_kernel(const int32_t *__restrict__ nbr, int kvol, int n_out, int n_in,
                                      int32_t *__restrict__ nbr_t) {
@@ -193,6 +172,11 @@ __global__ void spconv_wgrad_reduce_kernel(const float *__restrict__ partial, lo
   }
 }
 
+int spconv_wgrad_reduce(const float *partial, long long elems, int n_chunks, float *weight_grad, cudaStream_t st) {
+  BEVB200_LAUNCH(spconv_wgrad_reduce_kernel, grid_for(elems, 256), 256, 0, st, partial, elems, n_chunks, weight_grad);
+  return BEVB200_OK;
+}
+
 }  // namespace bevb200
 
 using namespace bevb200;
@@ -255,23 +239,20 @@ int bevb200_spconv_backward(const float *features, const float *weight, const fl
                         (uintptr_t)out_grad % 16 == 0;
   char *tc_ws = (char *)workspace + align_up(wbytes);
   // One split of out_grad serves both gradients when the filter gradient's out-grad image is the generation-6 row
-  // image (c_out = 32 / 64 / 128) and the input gradient runs on generation 6: dW first, then dIn gathers from it.
+  // image (c_out = 32 / 64 / 128) and the input gradient runs on split images: dW first, then dIn gathers from it.
   if (tc_wgrad && (c_out == 32 || c_out == 64 || c_out == 128) &&
-      spconv_tc_runs_on_split_images(c_out, c_in, kernel_volume, precision) && (uintptr_t)input_grad % 16 == 0) {
+      spconv_forward_path(precision, c_out, c_in, kernel_volume, false, out_grad, input_grad, nullptr) ==
+          FwdPath::kSplit) {
     rc = spconv_wgrad_tc(features, out_grad, nbr, n_in, n_out, c_in, c_out, kernel_volume, weight_grad, tc_ws, st);
     if (rc) return rc;
     void *packed = tc_ws + spconv_wgrad_tc_workspace_bytes(n_in, n_out, c_in, c_out, kernel_volume);
     rc = spconv_v6_pack_weights(wt, c_out, c_in, kernel_volume, packed, st);
     if (rc) return rc;
     return spconv_v6_forward(spconv_wgrad_tc_grad_image(tc_ws, n_in, c_in), packed, nbr_t, n_in, n_out, n_in, nullptr, c_out,
-                             c_in, kernel_volume, nullptr, nullptr, nullptr, 0, input_grad, nullptr, st);
+                             c_in, kernel_volume, nullptr, nullptr, nullptr, nullptr, 0, input_grad, nullptr, st);
   }
-  if (precision == BEVB200_PREC_FP32)
-    rc = spconv_forward_simt(out_grad, wt, nbr_t, n_out, n_in, c_out, c_in, kernel_volume, nullptr,
-                             nullptr, nullptr, 0, input_grad, st);
-  else
-    rc = spconv_forward_tc(out_grad, wt, nullptr, nbr_t, n_out, n_in, c_out, c_in, kernel_volume, nullptr,
-                           nullptr, nullptr, 0, precision, input_grad, st);
+  rc = spconv_forward(out_grad, wt, nullptr, nbr_t, n_out, n_in, c_out, c_in, kernel_volume, nullptr, nullptr, nullptr,
+                      0, precision, input_grad, st);
   if (rc) return rc;
   // dW on the tensor cores (spconv_wgrad_tc.cu) for the tensor-core precisions and channel counts 32 / 64 / 128 ...
   if (tc_wgrad)
@@ -312,9 +293,7 @@ int bevb200_spconv_backward(const float *features, const float *weight, const fl
                    c_in, c_out, partial);
   }
 #undef WG2
-  const long long elems = (long long)kernel_volume * c_in * c_out;
-  BEVB200_LAUNCH(spconv_wgrad_reduce_kernel, grid_for(elems, 256), 256, 0, st, partial, elems, n_chunks, weight_grad);
-  return BEVB200_OK;
+  return spconv_wgrad_reduce(partial, (long long)kernel_volume * c_in * c_out, n_chunks, weight_grad, st);
 }
 
 }  // extern "C"

@@ -10,8 +10,8 @@
 // is applied before the single store of each output row.
 //
 // This file is the fp32-FFMA variant (bit-for-bit fp32 products, fp32 accumulation); the
-// tensor-core variants live in spconv_tc.cu and spconv_v6.cu.
-#include "common.cuh"
+// tensor-core variants live in spconv_v6.cu, and spconv_fwd.cu picks between them.
+#include "spconv.cuh"
 
 namespace bevb200 {
 
@@ -163,73 +163,3 @@ int spconv_forward_simt(const float *features, const float *weight, const int32_
 }
 
 }  // namespace bevb200
-
-using namespace bevb200;
-
-namespace bevb200 {
-int spconv_forward_tc(const float *features, const float *weight, const float *packed,
-                      const int32_t *nbr, int n_in, int n_out, int c_in, int c_out, int kvol,
-                      const float *scale, const float *shift, const float *residual, int relu,
-                      int precision, float *out, cudaStream_t st);
-size_t spconv_packed_bytes(int c_in, int c_out, int kvol, int precision);
-int spconv_padded_channels(int c_in, int precision);
-int spconv_pack_weights(const float *weight, int c_in, int c_out, int kvol, int precision,
-                        float *packed, cudaStream_t st);
-}
-
-extern "C" {
-
-int bevb200_spconv_forward(const float *features, const float *weight, const int32_t *nbr,
-                           int n_in, int n_out, int c_in, int c_out, int kernel_volume,
-                           const float *scale, const float *shift, const float *residual,
-                           int relu, int precision, float *out, void *stream) {
-  BEVB200_REQUIRE(n_in >= 0 && n_out >= 0 && c_in > 0 && c_out > 0 && kernel_volume > 0,
-                  "bad sizes");
-  if (n_out == 0) return BEVB200_OK;
-  BEVB200_REQUIRE(weight && nbr && out, "null argument");
-  BEVB200_REQUIRE(features != nullptr || n_in == 0, "null features");
-  cudaStream_t st = (cudaStream_t)stream;
-  if (precision == BEVB200_PREC_FP32)
-    return spconv_forward_simt(features, weight, nbr, n_in, n_out, c_in, c_out, kernel_volume,
-                               scale, shift, residual, relu, out, st);
-  if (precision == BEVB200_PREC_TF32X3 || precision == BEVB200_PREC_TF32 || precision == BEVB200_PREC_BF16X3)
-    return spconv_forward_tc(features, weight, nullptr, nbr, n_in, n_out, c_in, c_out, kernel_volume,
-                             scale, shift, residual, relu, precision, out, st);
-  BEVB200_REQUIRE(false, "unknown precision mode");
-}
-
-int bevb200_spconv_padded_channels(int c_in, int precision) {
-  return spconv_padded_channels(c_in, precision);
-}
-
-size_t bevb200_spconv_packed_weight_bytes(int c_in, int c_out, int kernel_volume, int precision) {
-  if (precision != BEVB200_PREC_TF32X3 && precision != BEVB200_PREC_TF32 && precision != BEVB200_PREC_BF16X3) return 0;
-  return spconv_packed_bytes(c_in, c_out, kernel_volume, precision);
-}
-
-int bevb200_spconv_pack_weights(const float *weight, int c_in, int c_out, int kernel_volume,
-                                int precision, float *packed, void *stream) {
-  BEVB200_REQUIRE(weight && packed, "null argument");
-  BEVB200_REQUIRE(bevb200_spconv_packed_weight_bytes(c_in, c_out, kernel_volume, precision) > 0,
-                  "shape / precision has no packed form");
-  return spconv_pack_weights(weight, c_in, c_out, kernel_volume, precision, packed,
-                             (cudaStream_t)stream);
-}
-
-int bevb200_spconv_forward_packed(const float *features, const float *packed_weight,
-                                  const int32_t *nbr, int n_in, int n_out, int c_in, int c_out,
-                                  int kernel_volume, const float *scale, const float *shift,
-                                  const float *residual, int relu, int precision, float *out,
-                                  void *stream) {
-  BEVB200_REQUIRE(n_in >= 0 && n_out >= 0 && c_in > 0 && c_out > 0 && kernel_volume > 0,
-                  "bad sizes");
-  if (n_out == 0) return BEVB200_OK;
-  BEVB200_REQUIRE(packed_weight && nbr && out, "null argument");
-  BEVB200_REQUIRE(bevb200_spconv_packed_weight_bytes(c_in, c_out, kernel_volume, precision) > 0,
-                  "shape / precision has no packed form");
-  return spconv_forward_tc(features, nullptr, packed_weight, nbr, n_in, n_out, c_in, c_out,
-                           kernel_volume, scale, shift, residual, relu, precision, out,
-                           (cudaStream_t)stream);
-}
-
-}  // extern "C"

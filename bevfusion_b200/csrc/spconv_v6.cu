@@ -20,9 +20,7 @@
 // rows and / or the split image) runs once through a shared-memory transpose.  The number of output rows may be
 // read from device memory (n_out_dev), so a strided conv needs no host round trip and the whole encoder can be
 // captured in a CUDA graph.
-#include <stdlib.h>
-
-#include "common.cuh"
+#include "spconv.cuh"
 #include "tc_ptx.cuh"
 
 namespace bevb200 {
@@ -580,48 +578,42 @@ int spconv_v6_pack_weights(const float *weight, int c_in, int c_out, int kvol, v
   return BEVB200_OK;
 }
 
-int spconv_v6_split_rows(const float *features, int n_cap, const int32_t *n_dev, int c_in, void *split,
+// c_eff: 16 .. 128 for the forward kernels; the filter-gradient kernel wants whole 128-byte slabs (spconv_wgrad_tc.cu)
+int spconv_v6_split_rows(const float *features, int n_cap, const int32_t *n_dev, int c_in, int c_eff, void *split,
                          cudaStream_t st) {
-  const int ce = spconv_v6_cin_eff(c_in);
-  if (n_cap <= 0) return BEVB200_OK;
-  BEVB200_LAUNCH(spconv_v6_split_rows_kernel, grid_for((long long)n_cap * (ce / 8), 256), 256, 0, st, features,
-                 n_cap, n_dev, c_in, ce, (uint8_t *)split);
-  return BEVB200_OK;
-}
-
-// split image with an explicit padded channel count (multiple of 16, >= c_in): the filter-gradient kernel wants
-// whole 128-byte slabs (spconv_wgrad_tc.cu)
-int spconv_v6_split_rows_padded(const float *features, int n, int c_in, int c_eff, void *split, cudaStream_t st) {
   BEVB200_REQUIRE(c_eff >= c_in && c_eff % 16 == 0 && c_in >= 1, "bad padded channel count");
-  if (n <= 0) return BEVB200_OK;
-  BEVB200_LAUNCH(spconv_v6_split_rows_kernel, grid_for((long long)n * (c_eff / 8), 256), 256, 0, st, features, n,
-                 (const int32_t *)nullptr, c_in, c_eff, (uint8_t *)split);
+  if (n_cap <= 0) return BEVB200_OK;
+  BEVB200_LAUNCH(spconv_v6_split_rows_kernel, grid_for((long long)n_cap * (c_eff / 8), 256), 256, 0, st, features,
+                 n_cap, n_dev, c_in, c_eff, (uint8_t *)split);
   return BEVB200_OK;
 }
 
-template <int MODE, int COUT>
-static int v6_launch_one(const V6Params &p, cudaStream_t st) {
-  using Sh = V6Shape<MODE, COUT>;
-  const int n_tiles = (p.n_out + kV6TileM - 1) / kV6TileM;
-  int grid = 2 * kNumSMs;
-  if (grid > n_tiles) grid = n_tiles;
-  BEVB200_CUDA(cudaFuncSetAttribute(spconv_v6_kernel<MODE, COUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, Sh::kSmem));
-  // programmatic stream serialisation: the kernel's launch overlaps the tail of the previous kernel in the stream
-  // (21 back-to-back convs per frame)
+// Both forward kernels launch with programmatic stream serialisation: the launch overlaps the tail of the previous
+// kernel in the stream (21 back-to-back convs per frame), and the kernel waits for its results (griddepcontrol.wait).
+static int v6_launch_kernel(void (*kernel)(V6Params), int grid, int threads, int smem, const V6Params &p,
+                            cudaStream_t st) {
+  BEVB200_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3((unsigned)grid);
-  cfg.blockDim = dim3((unsigned)kV6Threads);
-  cfg.dynamicSmemBytes = Sh::kSmem;
+  cfg.blockDim = dim3((unsigned)threads);
+  cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  BEVB200_CUDA(cudaLaunchKernelEx(&cfg, spconv_v6_kernel<MODE, COUT>, p));
+  BEVB200_CUDA(cudaLaunchKernelEx(&cfg, kernel, p));
   ++g_launch_count;
   return BEVB200_OK;
+}
+
+template <int MODE, int COUT>
+static int v6_launch_one(const V6Params &p, cudaStream_t st) {
+  const int n_tiles = (p.n_out + kV6TileM - 1) / kV6TileM;
+  return v6_launch_kernel(spconv_v6_kernel<MODE, COUT>, n_tiles < 2 * kNumSMs ? n_tiles : 2 * kNumSMs, kV6Threads,
+                          V6Shape<MODE, COUT>::kSmem, p, st);
 }
 
 template <int MODE>
@@ -639,21 +631,7 @@ template <int COUT>
 static int wg_launch_one(const V6Params &p, cudaStream_t st) {
   using Sh = WgShape<COUT>;
   const int n_tiles = (p.n_out + Sh::kTileM - 1) / Sh::kTileM;
-  BEVB200_CUDA(cudaFuncSetAttribute(spconv_wg_kernel<COUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, Sh::kSmem));
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3((unsigned)(n_tiles < kNumSMs ? n_tiles : kNumSMs));
-  cfg.blockDim = dim3((unsigned)kWgThreads);
-  cfg.dynamicSmemBytes = Sh::kSmem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  BEVB200_CUDA(cudaLaunchKernelEx(&cfg, spconv_wg_kernel<COUT>, p));
-  ++g_launch_count;
-  return BEVB200_OK;
+  return v6_launch_kernel(spconv_wg_kernel<COUT>, n_tiles < kNumSMs ? n_tiles : kNumSMs, kWgThreads, Sh::kSmem, p, st);
 }
 
 static int wg_launch(const V6Params &p, cudaStream_t st) {
@@ -681,23 +659,10 @@ static void v6_common(V6Params &p, const void *rows, const void *packed, const i
   while ((1 << p.cin_shift) < c_in) ++p.cin_shift;
 }
 
-// features_split: split image with c_in (multiple of 16, <= 128) channels per row.
-int spconv_v6_forward_ex(const void *features_split, const void *packed, const int32_t *nbr, long long nbr_stride,
-                         int n_in, int n_out, const int32_t *n_out_dev, int c_in, int c_out, int kvol,
-                         const float *scale, const float *shift, const float *residual, const void *residual_split,
-                         int relu, float *out, void *out_split, cudaStream_t st);
 int spconv_v6_forward(const void *features_split, const void *packed, const int32_t *nbr, long long nbr_stride,
-                      int n_in, int n_out, const int32_t *n_out_dev, int c_in, int c_out, int kvol,
-                      const float *scale, const float *shift, const float *residual, int relu, float *out,
+                      int n_in, int n_out, const int32_t *n_out_dev, int c_in, int c_out, int kvol, const float *scale,
+                      const float *shift, const float *residual, const void *residual_split, int relu, float *out,
                       void *out_split, cudaStream_t st) {
-  return spconv_v6_forward_ex(features_split, packed, nbr, nbr_stride, n_in, n_out, n_out_dev, c_in, c_out, kvol, scale,
-                              shift, residual, nullptr, relu, out, out_split, st);
-}
-// residual_split: the residual rows as a split image instead of fp32 rows (at most one of the two)
-int spconv_v6_forward_ex(const void *features_split, const void *packed, const int32_t *nbr, long long nbr_stride,
-                         int n_in, int n_out, const int32_t *n_out_dev, int c_in, int c_out, int kvol,
-                         const float *scale, const float *shift, const float *residual, const void *residual_split,
-                         int relu, float *out, void *out_split, cudaStream_t st) {
   BEVB200_REQUIRE(!(residual && residual_split), "residual given twice");
   BEVB200_REQUIRE(residual_split == nullptr || (uintptr_t)residual_split % 16 == 0, "residual image must be 16-byte aligned");
   BEVB200_REQUIRE(c_in == spconv_v6_cin_eff(c_in) && spconv_v6_shape_ok(c_in, c_out, kvol), "shape has no tensor-core form");
@@ -719,7 +684,7 @@ int spconv_v6_forward_ex(const void *features_split, const void *packed, const i
 }
 
 // TF32 (tf32x3 = false) / 3xTF32 forward on zero-padded fp32 rows [n_in][c_in] (c_in a power of two, 8 .. 128) and
-// the tf32 weight image of spconv_tc.cu ([K block][hi (| lo)][Cout][32 fp32], chunk-swizzled like the bf16 images)
+// the tf32 weight image of spconv_fwd.cu ([K block][hi (| lo)][Cout][32 fp32], chunk-swizzled like the bf16 images)
 int spconv_v6_forward_tf32(const float *rows, const void *packed, const int32_t *nbr, int n_in, int n_out, int c_in,
                            int c_out, int kvol, bool tf32x3, const float *scale, const float *shift,
                            const float *residual, int relu, float *out, cudaStream_t st) {
@@ -744,7 +709,7 @@ int bevb200_spconv_split_rows(const float *features, int n, const int32_t *n_dev
   BEVB200_REQUIRE(n >= 0 && c_in >= 1 && spconv_v6_cin_eff(c_in) != 0, "bad sizes");
   if (n == 0) return BEVB200_OK;
   BEVB200_REQUIRE(features && split && (uintptr_t)split % 16 == 0, "null / unaligned argument");
-  return spconv_v6_split_rows(features, n, n_dev, c_in, split, (cudaStream_t)stream);
+  return spconv_v6_split_rows(features, n, n_dev, c_in, spconv_v6_cin_eff(c_in), split, (cudaStream_t)stream);
 }
 
 size_t bevb200_spconv_split_weight_bytes(int c_in, int c_out, int kernel_volume) {
@@ -765,7 +730,7 @@ int bevb200_spconv_forward_split(const void *features_split, const void *packed_
   BEVB200_REQUIRE(n_in >= 0 && n_out >= 0 && nbr_stride >= n_out, "bad sizes");
   BEVB200_REQUIRE(out != nullptr || out_split != nullptr, "no output requested");
   return spconv_v6_forward(features_split, packed_weight, nbr, nbr_stride, n_in, n_out, n_out_dev, c_in, c_out,
-                           kernel_volume, scale, shift, residual, relu, out, out_split, (cudaStream_t)stream);
+                           kernel_volume, scale, shift, residual, nullptr, relu, out, out_split, (cudaStream_t)stream);
 }
 
 }  // extern "C"

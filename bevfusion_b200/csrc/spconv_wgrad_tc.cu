@@ -17,12 +17,10 @@
 //   * multiplies hi.hi + hi.lo + lo.hi per 16-row k step (the lo.lo term is below the fp32 rounding of the sum).
 #include <stdlib.h>
 
-#include "common.cuh"
+#include "spconv.cuh"
 #include "tc_ptx.cuh"
 
 namespace bevb200 {
-
-int spconv_v6_split_rows_padded(const float *features, int n, int c_in, int c_eff, void *split, cudaStream_t st);
 
 constexpr int kWgtThreads = 256;
 constexpr int kWgtRows = 32;           // reduction rows per stage
@@ -164,16 +162,6 @@ __global__ void __launch_bounds__(kWgtThreads, 1) spconv_wgrad_tc_kernel(const W
   }
 }
 
-// dW[e] = sum over chunks (ascending) of partial[chunk][e]
-__global__ void spconv_wgrad_tc_reduce_kernel(const float *__restrict__ partial, long long elems, int n_chunks,
-                                              float *__restrict__ w_grad) {
-  for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < elems; e += (long long)gridDim.x * blockDim.x) {
-    float s = 0.f;
-    for (int ch = 0; ch < n_chunks; ++ch) s += partial[(long long)ch * elems + e];
-    w_grad[e] = s;
-  }
-}
-
 bool spconv_wgrad_tc_ok(int c_in, int c_out, int kvol) {
   static const bool enabled = [] {
     const char *e = getenv("BEVB200_WGRAD_TC");
@@ -241,8 +229,8 @@ int spconv_wgrad_tc(const float *features, const float *out_grad, const int32_t 
   uint8_t *fsplit = (uint8_t *)workspace;
   uint8_t *gsplit = fsplit + align_up((size_t)n_in * ci_eff * 4);
   float *partial = (float *)(gsplit + align_up((size_t)n_out * co_eff * 4));
-  int rc = spconv_v6_split_rows_padded(features, n_in, c_in, ci_eff, fsplit, st);
-  if (!rc) rc = spconv_v6_split_rows_padded(out_grad, n_out, c_out, co_eff, gsplit, st);
+  int rc = spconv_v6_split_rows(features, n_in, nullptr, c_in, ci_eff, fsplit, st);
+  if (!rc) rc = spconv_v6_split_rows(out_grad, n_out, nullptr, c_out, co_eff, gsplit, st);
   if (rc) return rc;
   WgtParams p;
   memset(&p, 0, sizeof(p));
@@ -256,9 +244,7 @@ int spconv_wgrad_tc(const float *features, const float *out_grad, const int32_t 
   else if (ci_eff == 64) rc = wgt_launch_co<64>(p, co_eff, st);
   else rc = wgt_launch_co<128>(p, co_eff, st);
   if (rc) return rc;
-  const long long elems = (long long)kvol * c_in * c_out;
-  BEVB200_LAUNCH(spconv_wgrad_tc_reduce_kernel, grid_for(elems, 256), 256, 0, st, partial, elems, p.n_chunks, weight_grad);
-  return BEVB200_OK;
+  return spconv_wgrad_reduce(partial, (long long)kvol * c_in * c_out, p.n_chunks, weight_grad, st);
 }
 
 }  // namespace bevb200
