@@ -75,6 +75,10 @@ _SIGNATURES = {
     "bevb200_boxes_overlap_bev": (c_int, [_P, c_int, _P, c_int, _P, _P]),
     "bevb200_nms_workspace_bytes": (c_size_t, [c_int, c_int]),
     "bevb200_nms": (c_int, [_P, _P, c_int, c_int, c_int, ctypes.c_double, c_int, _P, _P, _P, _P, c_size_t, _P]),
+    "bevb200_head_targets_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "bevb200_head_targets": (c_int, [_P, _P, _P, c_int, c_int, c_int, _P, c_int, _P, c_int] + [c_float] * 4
+                             + [c_int] * 3 + [ctypes.c_double] + [c_int] * 4 + [_P] * 6 + [c_size_t, _P]),
+    "bevb200_draw_heatmap_gaussian": (c_int, [_P] + [c_int] * 5 + [c_float, _P]),
     "bevb200_rulebook_workspace_bytes": (c_size_t, [c_int, c_int, _P]),
     "bevb200_rulebook_prepare": (c_int, [_P, c_int, c_int] + [_P] * 6 + [c_int, _P, _P, c_size_t, _P]),
     "bevb200_rulebook_fill": (c_int, [_P, c_int, c_int] + [_P] * 6 + [c_int, c_int, _P, _P, _P,

@@ -212,6 +212,28 @@ CENTERHEAD_RADAR_NMS_TYPE = ["circle", "rotate", "rotate", "circle", "rotate", "
 CENTERHEAD_RADAR_NMS_SCALE = [[1.0], [1.0, 1.0], [1.0, 1.0], [1.0], [1.0, 1.0], [2.5, 4.0]]
 
 
+def gt_boxes(seed=0, batch=1, min_boxes=40, max_boxes=120, extent=54.0):
+    """nuScenes-shaped ground truth for the head training targets: (boxes, labels), lists over samples of
+    [n, 9] fp32 LiDARInstance3DBoxes tensors (x, y, z_bottom, dx, dy, dz, yaw, vx, vy) and [n] int64 labels
+    0..9 (the classes of CENTERHEAD_TASKS in task order), n in [min_boxes, max_boxes].  Sizes are the class's
+    (w, l, h) jittered by +-15 %, centres uniform over +-extent m (so some lie off a +-51.2 m map), yaw in
+    [-pi, pi), velocities N(0, 3) m/s (0 for barriers and cones)."""
+    rng = np.random.default_rng(seed)
+    sizes = [s for classes in CENTERHEAD_TASKS for _, s in classes]
+    static = {5, 9}                                      # barrier, traffic_cone
+    boxes, labels = [], []
+    for _ in range(batch):
+        n = int(rng.integers(min_boxes, max_boxes + 1))
+        lab = rng.integers(0, len(sizes), n)
+        whl = np.array([sizes[l] for l in lab]) * rng.uniform(0.85, 1.15, (n, 3))
+        vel = rng.normal(0.0, 3.0, (n, 2)) * (~np.isin(lab, list(static)))[:, None]
+        b = np.concatenate([rng.uniform(-extent, extent, (n, 2)), rng.uniform(-2.5, 0.5, (n, 1)), whl,
+                            rng.uniform(-math.pi, math.pi, (n, 1)), vel], 1)
+        boxes.append(torch.from_numpy(b.astype(np.float32)))
+        labels.append(torch.from_numpy(lab.astype(np.int64)))
+    return boxes, labels
+
+
 def centerhead_detections(seed=0, batch=1, max_num=500):
     """What CenterPointBBoxCoder.decode hands to the NMS step, per task and sample: a list over the six
     tasks of a list over samples of dict(bboxes [n, 9] fp32 (x, y, z, w, l, h, yaw, vx, vy), scores [n]

@@ -424,6 +424,59 @@ BEVB200_API int bevb200_nms(const float *boxes, const int32_t *counts, int S, in
                             int post_max, const int64_t *order, int64_t *keep, int32_t *keep_count,
                             void *workspace, size_t workspace_bytes, void *stream);
 
+/* ---- Heatmap training targets of CenterHead and TransFusionHead (centerpoint.py:432-582
+ *      get_targets_single, the heatmap block of transfusion.py:526-573, core/utils/gaussian.py) ------------
+ * Three launches (zero, assign, draw), no host synchronisation, no allocation; CUDA-graph capturable.
+ *   boxes       [B, nmax, box_dim] fp32 device, LiDARInstance3DBoxes.tensor rows (x, y, z_bottom, dx, dy, dz, yaw
+ *               [, vx, vy]); box_dim 7 or 9
+ *   labels      [B, nmax] int32 device; counts [B] int32 device (sample b is rows [0, counts[b]), clamped to
+ *               [0, nmax]; nullable: every sample holds nmax)
+ *   label_table_host  [num_labels, 2] int32 host: (task, channel within the task) of each label, task -1 for a
+ *               label of no task; task_classes_host [num_tasks] int32 host: classes per task (ncls_t)
+ *   pc_x, pc_y, vs_x, vs_y  point_cloud_range[0:2] and voxel_size[0:2] as fp32; fmap_x = grid_size[0] // osf,
+ *               fmap_y = grid_size[1] // osf
+ * Per object, in fp32 with one rounding per op: width = dx / vs_x / osf, length = dy / vs_y / osf; drawn only if
+ * width > 0 and length > 0; r = gaussian_radius((length, width), gaussian_overlap) op for op (gaussian.py:55-84),
+ * radius = max(min_radius, int(r)); coor = (x - pc) / vs / osf, (cx, cy) = coor truncated toward zero.  The
+ * gaussian exp(-(dx^2 + dy^2) / (2 sigma^2)), sigma = (2 radius + 1) / 6, is evaluated in double, set to 0 below
+ * DBL_EPSILON and rounded to fp32, over the window rows cx +- radius, columns cy +- radius of a [fmap_y, fmap_x]
+ * plane, clipped to the plane (the reference draws center_int[[1, 0]]), and maxed into the heatmap.
+ * mode CENTERHEAD: objects are assigned to their task's slots by class in task order, then by index
+ *               (centerpoint.py:463-486); slots >= max_objs are dropped and not drawn; a centre with cx outside
+ *               [0, fmap_x) or cy outside [0, fmap_y) is skipped.  Labels of no task are dropped, as the reference's
+ *               task masks drop them.  Outputs, task-major: heatmap [T][B, ncls_t, fmap_y, fmap_x],
+ *               anno_box [T][B, max_objs, box_dim == 9 ? 10 : 8] fp32 ((coor - c)[2], z + dz / 2, log(dims) if
+ *               norm_bbox else dims, sin(yaw), cos(yaw)[, vx, vy]), ind int64 [T][B, max_objs] = cx * fmap_y + cy,
+ *               mask uint8 [T][B, max_objs]; every slot is written (zeros for empty slots).
+ * mode TRANSFUSION: num_tasks 1, no max_objs cap, no range test (a centre up to radius cells off the map draws its
+ *               in-map part); heatmap [B, ncls, fmap_y, fmap_x]; anno_box, ind, mask unused (nullable).
+ * status [1] int32 device: objects with width, length > 0 skipped because int(r) is undefined (r not finite or
+ * >= 2^30, where the reference raises) or, in TRANSFUSION mode, because the label is of no task (the reference
+ * would wrap a negative label or raise).  An object whose centre is not finite is skipped without a count.
+ * nmax <= BEVB200_HEAD_TARGETS_MAX_BOXES, else BEVB200_EUNSUPPORTED; num_tasks <= BEVB200_HEAD_TARGETS_MAX_TASKS,
+ * num_labels <= BEVB200_HEAD_TARGETS_MAX_LABELS.  Workspace (one draw record per object, 16 * B * nmax bytes):
+ * bevb200_head_targets_workspace_bytes(B, nmax), 0 for unsupported sizes; a smaller one gives
+ * BEVB200_EWORKSPACE. */
+#define BEVB200_HEAD_TARGETS_CENTERHEAD 0
+#define BEVB200_HEAD_TARGETS_TRANSFUSION 1
+#define BEVB200_HEAD_TARGETS_MAX_BOXES 4096
+#define BEVB200_HEAD_TARGETS_MAX_TASKS 32
+#define BEVB200_HEAD_TARGETS_MAX_LABELS 256
+BEVB200_API size_t bevb200_head_targets_workspace_bytes(int B, int nmax);
+BEVB200_API int bevb200_head_targets(const float *boxes, const int32_t *labels, const int32_t *counts, int B,
+                                     int nmax, int box_dim, const int32_t *label_table_host, int num_labels,
+                                     const int32_t *task_classes_host, int num_tasks, float pc_x, float pc_y,
+                                     float vs_x, float vs_y, int out_size_factor, int fmap_x, int fmap_y,
+                                     double gaussian_overlap, int min_radius, int mode, int max_objs, int norm_bbox,
+                                     float *heatmap, float *anno_box, int64_t *ind, uint8_t *mask, int32_t *status,
+                                     void *workspace, size_t workspace_bytes, void *stream);
+/* draw_heatmap_gaussian(heatmap, (x, y), radius, k) (gaussian.py:24-52) on one [height, width] fp32 plane, through
+ * the draw kernel of bevb200_head_targets with one record: column x, row y.  Every cell of the window clipped to the
+ * plane becomes torch.max(cell, k * gaussian) (any k; zeros of the gaussian included; NaN propagates).
+ * 0 <= radius < 2^30, else BEVB200_EINVAL. */
+BEVB200_API int bevb200_draw_heatmap_gaussian(float *heatmap, int height, int width, int x, int y, int radius,
+                                              float k, void *stream);
+
 /* ---- LiDAR depth images for the depth-aware camera lift ------------------------------------
  * BaseDepthTransform.forward's per-sample loop (mmdet3d/models/vtransforms/base.py:279-329):
  * undo the lidar augmentation, project every point into every camera with lidar2image, clamp z to
