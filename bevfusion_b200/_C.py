@@ -79,6 +79,11 @@ _SIGNATURES = {
     "bevb200_head_targets": (c_int, [_P, _P, _P, c_int, c_int, c_int, _P, c_int, _P, c_int] + [c_float] * 4
                              + [c_int] * 3 + [ctypes.c_double] + [c_int] * 4 + [_P] * 6 + [c_size_t, _P]),
     "bevb200_draw_heatmap_gaussian": (c_int, [_P] + [c_int] * 5 + [c_float, _P]),
+    "bevb200_lsap_workspace_bytes": (c_size_t, [c_int] * 3),
+    "bevb200_lsap": (c_int, [_P] * 3 + [c_int] * 3 + [_P] * 5 + [c_size_t, _P]),
+    "bevb200_transfusion_assign_workspace_bytes": (c_size_t, [c_int] * 4),
+    "bevb200_transfusion_assign": (c_int, [_P] * 6 + [c_int] * 4 + [_P] * 3 + [c_int] * 2 + [ctypes.c_double] * 4
+                                   + [c_int] * 2 + [ctypes.c_double] * 10 + [_P] * 13 + [c_size_t, _P]),
     "bevb200_rulebook_workspace_bytes": (c_size_t, [c_int, c_int, _P]),
     "bevb200_rulebook_prepare": (c_int, [_P, c_int, c_int] + [_P] * 6 + [c_int, _P, _P, c_size_t, _P]),
     "bevb200_rulebook_fill": (c_int, [_P, c_int, c_int] + [_P] * 6 + [c_int, c_int, _P, _P, _P,

@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIB_DIR, "libbevfusion_b200.so")
-SOURCES = ["common.cu", "bevpool.cu", "bevpool_lift.cu", "voxelize.cu", "pillars.cu", "radar.cu", "scatter.cu", "depthmap.cu", "rulebook.cu", "spconv_fwd.cu", "spconv_simt.cu", "spconv_v6.cu", "encoder.cu", "spconv_bwd.cu", "spconv_wgrad_tc.cu", "box_nms.cu", "head_targets.cu"]
+SOURCES = ["common.cu", "bevpool.cu", "bevpool_lift.cu", "voxelize.cu", "pillars.cu", "radar.cu", "scatter.cu", "depthmap.cu", "rulebook.cu", "spconv_fwd.cu", "spconv_simt.cu", "spconv_v6.cu", "encoder.cu", "spconv_bwd.cu", "spconv_wgrad_tc.cu", "box_nms.cu", "head_targets.cu", "transfusion_assign.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr",

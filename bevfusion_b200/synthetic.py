@@ -234,6 +234,64 @@ def gt_boxes(seed=0, batch=1, min_boxes=40, max_boxes=120, extent=54.0):
     return boxes, labels
 
 
+TRANSFUSION_CODER = dict(pc_range=[-51.2, -51.2], voxel_size=[0.1, 0.1], out_size_factor=8, code_size=10)
+TRANSFUSION_TRAIN_CFG = dict(point_cloud_range=[-51.2, -51.2, -5.0, 51.2, 51.2, 3.0], grid_size=[1024, 1024, 1],
+                             voxel_size=[0.1, 0.1, 0.2], out_size_factor=8, gaussian_overlap=0.1, min_radius=2,
+                             pos_weight=-1,
+                             assigner=dict(type="HungarianAssigner3D",
+                                           iou_calculator=dict(type="BboxOverlaps3D", coordinate="lidar"),
+                                           cls_cost=dict(type="FocalLossCost", gamma=2.0, alpha=0.25, weight=0.15),
+                                           reg_cost=dict(type="BBoxBEVL1Cost", weight=0.25),
+                                           iou_cost=dict(type="IoU3DCost", weight=0.25)))
+
+
+def transfusion_predictions(seed, batch, gt, num_proposals=200, num_classes=10, layers=1):
+    """Raw TransFusionHead predictions for the training-target assignment, shaped as the head emits them (the
+    transfusion/default.yaml coder: pc_range -51.2, voxel 0.1, out_size_factor 8): dict(heatmap [B, K, N] logits,
+    center [B, 2, N] feature cells, height [B, 1, N] gravity-centre z, dim [B, 3, N] log sizes, rot [B, 2, N]
+    (sin, cos), vel [B, 2, N]) fp32 CPU tensors, N = layers * num_proposals.  gt = (boxes, labels) as gt_boxes
+    gives them.  In each layer about half the proposals are jittered copies of gts (their logit raised at the
+    gt's label) and the rest random; a few proposals are exact copies of others, so the cost has ties."""
+    rng = np.random.default_rng(seed)
+    boxes, labels = gt
+    P, K, N = num_proposals, num_classes, layers * num_proposals
+    cell = TRANSFUSION_CODER["out_size_factor"] * TRANSFUSION_CODER["voxel_size"][0]
+    out = {k: np.zeros((batch, r, N), np.float32) for k, r in
+           (("heatmap", K), ("center", 2), ("height", 1), ("dim", 3), ("rot", 2), ("vel", 2))}
+    for b in range(batch):
+        g = boxes[b].numpy().astype(np.float64) if len(boxes[b]) else np.zeros((0, 9))
+        lab = labels[b].numpy()
+        for l in range(layers):
+            cols = slice(l * P, (l + 1) * P)
+            heat = rng.normal(-2.0, 1.0, (K, P))
+            xy = rng.uniform(-51.2, 51.2, (P, 2))
+            z = rng.uniform(-2.0, 1.0, P)
+            d = np.log(rng.uniform(0.3, 6.0, (P, 3)))
+            yaw = rng.uniform(-np.pi, np.pi, P)
+            vel = rng.normal(0.0, 2.0, (P, 2))
+            n_copy = min(len(g), P // 2)
+            if n_copy:
+                pick = rng.choice(len(g), n_copy, replace=False)
+                dst = rng.choice(P, n_copy, replace=False)
+                src = g[pick]
+                xy[dst] = src[:, :2] + rng.normal(0.0, 0.3, (n_copy, 2))
+                z[dst] = src[:, 2] + src[:, 5] * 0.5 + rng.normal(0.0, 0.1, n_copy)
+                d[dst] = np.log(src[:, 3:6]) + rng.normal(0.0, 0.08, (n_copy, 3))
+                yaw[dst] = src[:, 6] + rng.normal(0.0, 0.15, n_copy)
+                vel[dst] = src[:, 7:9] + rng.normal(0.0, 0.3, (n_copy, 2))
+                heat[lab[pick], dst] += rng.uniform(1.0, 4.0, n_copy)
+            out["heatmap"][b, :, cols] = heat
+            out["center"][b, :, cols] = ((xy - np.array(TRANSFUSION_CODER["pc_range"])) / cell).T
+            out["height"][b, 0, cols] = z
+            out["dim"][b, :, cols] = d.T
+            out["rot"][b, :, cols] = np.stack([np.sin(yaw), np.cos(yaw)]) * rng.uniform(0.8, 1.2, P)
+            out["vel"][b, :, cols] = vel.T
+            dup = rng.choice(P, 8, replace=False) + l * P            # exact duplicate proposals: cost ties
+            for key in out:
+                out[key][b, :, dup[4:]] = out[key][b, :, dup[:4]]
+    return {k: torch.from_numpy(v) for k, v in out.items()}
+
+
 def centerhead_detections(seed=0, batch=1, max_num=500):
     """What CenterPointBBoxCoder.decode hands to the NMS step, per task and sample: a list over the six
     tasks of a list over samples of dict(bboxes [n, 9] fp32 (x, y, z, w, l, h, yaw, vx, vy), scores [n]

@@ -477,6 +477,81 @@ BEVB200_API int bevb200_head_targets(const float *boxes, const int32_t *labels, 
 BEVB200_API int bevb200_draw_heatmap_gaussian(float *heatmap, int height, int width, int x, int y, int radius,
                                               float k, void *stream);
 
+/* ---- Exact linear sum assignment and the TransFusion training-target assignment (transfusion.py:408-525
+ *      get_targets_single, core/bbox/assigners/hungarian_assigner.py, scipy.optimize.linear_sum_assignment) ----
+ * The solver is scipy's rectangular_lsap.cpp (shortest augmenting paths, Crouse 2016) restated in double with
+ * the same column selection and tie breaks: for the same fp32 matrix it returns scipy's assignment bit for bit,
+ * ties included.  A segment is one independent matrix; it is transposed when it has fewer columns than rows, as
+ * scipy does.  One CTA per segment; no host synchronisation, no allocation, CUDA-graph capturable.
+ * Per-segment status bits (nonzero: the segment has no matches; scipy / the reference would raise):
+ *   BEVB200_ASSIGN_INVALID_COST  a cost entry is NaN or -inf
+ *   BEVB200_ASSIGN_BAD_LABEL     (transfusion_assign) a gt label outside [0, K); its cost column is NaN
+ *   BEVB200_ASSIGN_INFEASIBLE    +inf entries leave no complete assignment
+ * Limits: at most BEVB200_ASSIGN_MAX rows and columns per segment, BEVB200_ASSIGN_MAX_SEGMENTS segments and
+ * BEVB200_ASSIGN_MAX_CLASSES classes, else BEVB200_EUNSUPPORTED. */
+#define BEVB200_ASSIGN_MAX 4096
+#define BEVB200_ASSIGN_MAX_SEGMENTS 65535
+#define BEVB200_ASSIGN_MAX_CLASSES 256
+#define BEVB200_ASSIGN_INVALID_COST 1
+#define BEVB200_ASSIGN_BAD_LABEL 2
+#define BEVB200_ASSIGN_INFEASIBLE 4
+
+/* linear_sum_assignment of S matrices at once:
+ *   cost        [S, R, C] fp32 device; segment s is its top-left row_counts[s] x col_counts[s] block (counts int32
+ *               device, clamped to [0, R] / [0, C]; nullable: R / C)
+ *   col4row     [S, R] int32 device: the column matched to each row, -1 for none (padding rows included)
+ *   row4col     [S, C] int32 device, nullable: the row matched to each column, -1 for none
+ *   status      [S] int32 device, nullable: the status bits above
+ *   steps       [S] int32 device, nullable: the solver's Dijkstra steps (columns settled) per segment
+ * The solver keeps its state in shared memory: the workspace query returns 0, and workspace may be null. */
+BEVB200_API size_t bevb200_lsap_workspace_bytes(int S, int R, int C);
+BEVB200_API int bevb200_lsap(const float *cost, const int32_t *row_counts, const int32_t *col_counts, int S, int R,
+                             int C, int32_t *col4row, int32_t *row4col, int32_t *status, int32_t *steps,
+                             void *workspace, size_t workspace_bytes, void *stream);
+
+/* TransFusionHead.get_targets (everything but the heatmap) for B samples and L decoder layers of P proposals
+ * (N = L * P) in three launches (cost, solver, targets).  Segment s = b * L + l is layer l of sample b.
+ *   heatmap     [B, K, N] fp32 logits; center [B, 2, N] (feature cells), height [B, 1, N] (gravity-centre z),
+ *               dim [B, 3, N] (log sizes), rot [B, 2, N] (sin, cos): the head's raw predictions, decoded as
+ *               TransFusionBBoxCoder.decode does (cx = center * osf * vs + pc, dims = exp, z = height - dz / 2,
+ *               yaw = atan2).  decoded [B, N, box_dim] fp32, nullable: boxes already decoded (center, height,
+ *               dim, rot are then unused)
+ *   gt_boxes    [B, nmax, box_dim] fp32 (x, y, z_bottom, dx, dy, dz, yaw[, vx, vy]); gt_labels [B, nmax] int32;
+ *               gt_counts [B] int32 device (clamped to [0, nmax]; nullable: nmax)
+ *   coder_*     TransFusionBBoxCoder pc_range[0:2], voxel_size[0:2] and out_size_factor; code_size 8 or 10 (10
+ *               needs box_dim 9); pc_x0, pc_y0, pc_x1, pc_y1: train_cfg.point_cloud_range[0, 1, 3, 4]
+ *   cls_weight, alpha, gamma, reg_weight, iou_weight: FocalLossCost, BBoxBEVL1Cost, IoU3DCost; pos_weight:
+ *               train_cfg.pos_weight
+ * Cost per (proposal, gt), fp32 with one rounding per op in the reference's order: focal class cost of the gt's
+ * label (p = sigmoid, (pos - neg) * w) + L1 of the xy normalised by the range, times reg_weight + (-iou3d) *
+ * iou_weight, iou3d = rotated BEV overlap (as bevb200_boxes_overlap_bev) * height overlap / clamp(va + vb - ov,
+ * 1e-8).  The assignment is scipy's on that matrix.  Outputs, all written:
+ *   labels        [B, N] int64: the matched gt's label, K when unmatched
+ *   label_weights [B, N] int64: 1; positives (int64)pos_weight when pos_weight > 0
+ *   bbox_targets  [B, N, code_size] fp32: TransFusionBBoxCoder.encode of the matched gt ((x - pc) * the fp32
+ *                 reciprocal of (float)(osf * vs), z + dz / 2, log dims, sin, cos[, vx, vy]), 0 when unmatched
+ *   bbox_weights  [B, N, code_size] fp32: 1 on matched rows; ious [B, N] fp32: clamp(iou3d, 0, 1) on matches
+ *   num_pos [B] int32, mean_iou [B] fp32 = sum(ious of the positives) / max(num_pos, 1); status [B] int32: the
+ *                 status bits of the sample's segments ORed
+ *   gt_inds [B, N] int64, nullable: matched gt + 1, 0 when unmatched; max_overlaps [B, N] fp32, nullable: the
+ *                 unclamped iou3d of matches, 0 elsewhere (HungarianAssigner3D's AssignResult)
+ *   cost_out      [B * L, P, nmax] fp32, nullable: the cost matrix, proposal-major; entries of absent gts are
+ *                 not written
+ *   steps         [B * L] int32, nullable: the solver's steps per segment
+ * A sample with no gt gets all-negative targets (the reference raises).  Workspace:
+ * bevb200_transfusion_assign_workspace_bytes(B, L, P, nmax) (4 * B * L * (P * nmax + P + 1) bytes, aligned), 0
+ * for unsupported sizes; a smaller one gives BEVB200_EWORKSPACE. */
+BEVB200_API size_t bevb200_transfusion_assign_workspace_bytes(int B, int L, int P, int nmax);
+BEVB200_API int bevb200_transfusion_assign(
+    const float *heatmap, const float *center, const float *height, const float *dim, const float *rot,
+    const float *decoded, int B, int L, int P, int K, const float *gt_boxes, const int32_t *gt_labels,
+    const int32_t *gt_counts, int nmax, int box_dim, double coder_pc_x, double coder_pc_y, double coder_vs_x,
+    double coder_vs_y, int coder_out_size_factor, int code_size, double pc_x0, double pc_y0, double pc_x1,
+    double pc_y1, double cls_weight, double alpha, double gamma, double reg_weight, double iou_weight,
+    double pos_weight, int64_t *labels, int64_t *label_weights, float *bbox_targets, float *bbox_weights,
+    float *ious, int32_t *num_pos, float *mean_iou, int32_t *status, int64_t *gt_inds, float *max_overlaps,
+    float *cost_out, int32_t *steps, void *workspace, size_t workspace_bytes, void *stream);
+
 /* ---- LiDAR depth images for the depth-aware camera lift ------------------------------------
  * BaseDepthTransform.forward's per-sample loop (mmdet3d/models/vtransforms/base.py:279-329):
  * undo the lidar augmentation, project every point into every camera with lidar2image, clamp z to
