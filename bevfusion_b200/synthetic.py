@@ -292,6 +292,37 @@ def transfusion_predictions(seed, batch, gt, num_proposals=200, num_classes=10, 
     return {k: torch.from_numpy(v) for k, v in out.items()}
 
 
+def transfusion_heatmap(seed, batch, num_classes=10, height=128, width=128, dtype=torch.float32, gt=None,
+                        extent=54.0):
+    """Dense TransFusion heatmap logits [B, C, H, W] on the CPU, shaped like a trained head's output: a smooth
+    background near logit -5 (sigmoid about 0.007; iid N(0, 1) noise blurred over 3 x 3 cells, so that a few per cent
+    of the cells are local maxima) plus one Gaussian blob per object at its label's channel, centred on the object's
+    cell, with a peak logit raise of 3 to 9 and a sigma of half the object's footprint in cells (at least 0.7).
+    gt = (boxes, labels) as gt_boxes gives them (default gt_boxes(seed, batch)); a centre maps to
+    column (x + extent) / (2 extent) * W and row (y + extent) / (2 extent) * H, and objects off the map are skipped.
+    Labels at or above num_classes are skipped.  Computed in float64, returned in `dtype`."""
+    rng = np.random.default_rng(seed)
+    boxes, labels = gt if gt is not None else gt_boxes(seed=seed, batch=batch)
+    noise = rng.standard_normal((batch, num_classes, height + 2, width + 2))
+    base = sum(noise[:, :, dy:dy + height, dx:dx + width] for dy in range(3) for dx in range(3)) / 3.0
+    heat = base * 0.5 - 5.0
+    rows, cols = np.arange(height)[:, None], np.arange(width)[None, :]
+    for b in range(batch):
+        g = boxes[b].numpy().astype(np.float64)
+        lab = labels[b].numpy()
+        for i in range(len(g)):
+            if lab[i] >= num_classes:
+                continue
+            cx = (g[i, 0] + extent) / (2 * extent) * width
+            cy = (g[i, 1] + extent) / (2 * extent) * height
+            if not (0 <= cx < width and 0 <= cy < height):
+                continue
+            sigma = max(0.7, 0.5 * max(g[i, 3] / (2 * extent) * width, g[i, 4] / (2 * extent) * height))
+            amp = rng.uniform(3.0, 9.0)
+            heat[b, lab[i]] += amp * np.exp(-((cols - cx) ** 2 + (rows - cy) ** 2) / (2 * sigma * sigma))
+    return torch.from_numpy(heat).to(dtype).contiguous()
+
+
 def centerhead_detections(seed=0, batch=1, max_num=500):
     """What CenterPointBBoxCoder.decode hands to the NMS step, per task and sample: a list over the six
     tasks of a list over samples of dict(bboxes [n, 9] fp32 (x, y, z, w, l, h, yaw, vx, vy), scores [n]

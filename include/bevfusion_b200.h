@@ -552,6 +552,39 @@ BEVB200_API int bevb200_transfusion_assign(
     float *ious, int32_t *num_pos, float *mean_iou, int32_t *status, int64_t *gt_inds, float *max_overlaps,
     float *cost_out, int32_t *steps, void *workspace, size_t workspace_bytes, void *stream);
 
+/* ---- TransFusion query proposals (TransFusionHead.forward_single, transfusion.py:237-281 and :322-325) ----------
+ * The query initialisation of the head for B samples in two launches (peak, select), no host synchronisation, no
+ * allocation; CUDA-graph capturable and the same bit for bit on every run.
+ *   heatmap     [B, C, H, W] device, the dense heatmap logits; dtype BEVB200_PROPOSALS_F32 or _F16
+ *   kernel_size k, the nms_kernel_size: odd, 3 <= k <= BEVB200_PROPOSALS_MAX_KERNEL, k <= H and k <= W; p = k / 2
+ *   exempt0, exempt1  classes whose peak test is against themselves (nuScenes 8, 9; Waymo 1, 2), -1 for none
+ * With s = sigmoid(x) as torch computes it on CUDA (1 / (1 + expf(-x)) in fp32, IEEE division, rounded to fp16 for
+ * fp16 input), local_max = the k x k window maximum (NaN propagates, as max_pool2d) on cells at least p from every
+ * edge and 0 in the border band, or s itself for an exempt class, the masked plane is m = s * (s == local_max): a
+ * border cell is 0, a NaN stays NaN.  Over the C * H * W values of m per sample, flat index c * H * W + h * W + w,
+ * the first K = num_proposals in descending value (NaN above everything) with ties by ascending flat index, i.e.
+ * argsort(descending=True, stable=True)[:K], give:
+ *   labels               [B, K] int64 device: flat / (H * W)  (the reference's query_labels)
+ *   index                [B, K] int64 device: flat % (H * W)
+ *   query_heatmap_score  [B, C, K] device in the heatmap's dtype: m[b, :, index], every class at each selected cell
+ * Every output element is written.  BEVB200_EINVAL: a size < 1, an even k or k = 1, H or W < k, an exempt class
+ * outside [-1, C), K < 1 or K > C * H * W, a null pointer.  BEVB200_EUNSUPPORTED: another dtype, or B, C, C * H * W,
+ * K or k above the limits below.  Workspace (each tile of 1024 cells gets 1024 8-byte key slots and a count):
+ * bevb200_transfusion_proposals_workspace_bytes(B, C, H, W) = align256(8 * B * T * 1024) + align256(4 * B * T),
+ * T = ceil(C * H * W / 1024); 0 for unsupported sizes; a smaller one gives BEVB200_EWORKSPACE. */
+#define BEVB200_PROPOSALS_F32 0
+#define BEVB200_PROPOSALS_F16 1
+#define BEVB200_PROPOSALS_MAX_BATCH 65535
+#define BEVB200_PROPOSALS_MAX_CLASSES 64
+#define BEVB200_PROPOSALS_MAX_CELLS (1 << 24)   /* C * H * W per sample */
+#define BEVB200_PROPOSALS_MAX_K 4096
+#define BEVB200_PROPOSALS_MAX_KERNEL 15
+BEVB200_API size_t bevb200_transfusion_proposals_workspace_bytes(int B, int C, int H, int W);
+BEVB200_API int bevb200_transfusion_proposals(const void *heatmap, int dtype, int B, int C, int H, int W,
+                                              int num_proposals, int kernel_size, int exempt0, int exempt1,
+                                              int64_t *labels, int64_t *index, void *query_heatmap_score,
+                                              void *workspace, size_t workspace_bytes, void *stream);
+
 /* ---- LiDAR depth images for the depth-aware camera lift ------------------------------------
  * BaseDepthTransform.forward's per-sample loop (mmdet3d/models/vtransforms/base.py:279-329):
  * undo the lidar augmentation, project every point into every camera with lidar2image, clamp z to
