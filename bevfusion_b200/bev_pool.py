@@ -149,6 +149,16 @@ def gen_dx_bx(xbound, ybound, zbound):
     return dx, bx, nx
 
 
+def _grid_host(dx, bx, nx, B):
+    """Host arrays of the quantisation grid -- fp32 lower = bx - dx/2 (base.py:149, evaluated in fp32), fp32 dx,
+    int32 nx -- and the pooled dims (B, nz, nx, ny)."""
+    lower = bx.float().cpu() - dx.float().cpu() / 2.0
+    lower_h = _C.host_array(ctypes.c_float, [float(v) for v in lower])
+    dx_h = _C.host_array(ctypes.c_float, [float(v) for v in dx.float().cpu()])
+    nx_h = _C.host_array(ctypes.c_int32, [int(v) for v in nx])
+    return lower_h, dx_h, nx_h, (int(B), int(nx[2]), int(nx[0]), int(nx[1]))
+
+
 def prepare_from_geometry(geom_xyz, dx, bx, nx, B):
     """quantise + filter + rank + sort + intervals of lidar-frame frustum points
     (base.py:149-169 then bev_pool.py:87-94, :41-46), all on the device."""
@@ -156,11 +166,7 @@ def prepare_from_geometry(geom_xyz, dx, bx, nx, B):
     g = geom_xyz.reshape(-1, 3)
     n_total = g.shape[0]
     assert n_total % B == 0
-    lower = (bx.float().cpu() - dx.float().cpu() / 2.0)  # base.py:149, evaluated in fp32
-    lower_h = _C.host_array(ctypes.c_float, [float(v) for v in lower])
-    dx_h = _C.host_array(ctypes.c_float, [float(v) for v in dx.float().cpu()])
-    nx_h = _C.host_array(ctypes.c_int32, [int(v) for v in nx])
-    dims = (int(B), int(nx[2]), int(nx[0]), int(nx[1]))
+    lower_h, dx_h, nx_h, dims = _grid_host(dx, bx, nx, B)
     with torch.cuda.device(g.device):
         return _finish_tables(n_total, g.device, dims, lambda r, p, gm, s, l, c, ws:
                               _C.lib().bevb200_bev_pool_prepare_geom(
@@ -194,11 +200,7 @@ def prepare_from_cameras(frustum, camera2lidar_rots, camera2lidar_trans, intrins
     fr = frustum.reshape(-1, 3).contiguous()
     n_fr = fr.shape[0]
     n_total = n_fr * B * N
-    lower = (bx.float().cpu() - dx.float().cpu() / 2.0)
-    lower_h = _C.host_array(ctypes.c_float, [float(v) for v in lower])
-    dx_h = _C.host_array(ctypes.c_float, [float(v) for v in dx.float().cpu()])
-    nx_h = _C.host_array(ctypes.c_int32, [int(v) for v in nx])
-    dims = (int(B), int(nx[2]), int(nx[0]), int(nx[1]))
+    lower_h, dx_h, nx_h, dims = _grid_host(dx, bx, nx, B)
     with torch.cuda.device(dev):
         geom = torch.empty((n_total, 3), **f32) if return_geometry else None
         tables = _finish_tables(n_total, dev, dims, lambda r, p, gm, s, l, c, ws:

@@ -5,43 +5,23 @@
 // mmdet3d/ops/bev_pool/bev_pool.py:38-98, mmdet3d/models/vtransforms/base.py:141-176.
 //
 // Design (HBM-bound, ~0.64 GB per launch at the C2 workload):
-//   * the sorted row stream is cut into CHUNK_ROWS-row chunks; one warp owns one chunk, so
-//     work per warp is uniform no matter how skewed the interval lengths are (1 .. >1000)
-//   * an interval belongs to the chunk that holds its first row and is reduced by that warp
-//     alone, except intervals longer than 2*CHUNK_ROWS which are cut at chunk boundaries into
-//     pieces; pieces land in a small partial buffer and a second tiny kernel adds them in
-//     fixed order -> results are bit-reproducible run to run (no float atomics)
-//   * rows are read with 16-byte streaming loads (ld.global.nc.L1::no_allocate.v4), G rows x
-//     C/4 quads = T*32 float4 per warp step, two steps in flight (>= 2*T*512 B per warp)
-//   * the per-lane partial sums are folded through shared memory once per interval and the
-//     finished row is stored with one coalesced 16-byte-per-lane store
+//   * forward: every warp owns a contiguous range of the sorted row stream and stages it through
+//     its own shared-memory ring (section "forward" below), so work per warp is uniform no matter
+//     how skewed the interval lengths are (1 .. >1000); intervals that cross a range boundary
+//     leave pieces in a small partial buffer that a second tiny kernel adds in fixed order ->
+//     results are bit-reproducible run to run (no float atomics)
+//   * backward: one warp per 128-row chunk broadcasts each interval's out_grad row with 16-byte
+//     streaming stores
 //   * `perm` variants read rows of the ORIGINAL feature tensor through the sorted->original
 //     map, which removes x[kept] / feats[indices] (2 x 0.6 GB of copies) from the frame
 #include <cub/device/device_radix_sort.cuh>
 
-#include <stdlib.h>
-
-#include "common.cuh"
+#include "bevpool.cuh"
 
 namespace bevb200 {
 
-constexpr int kChunkRows = 128;            // rows of the sorted stream owned by one warp
-constexpr int kLongRows = 2 * kChunkRows;  // intervals longer than this are cut into pieces
-constexpr int kPoolWarps = 8;              // warps per CTA
-
-struct PoolDims {
-  int b, d, h, w;
-};
-
-__device__ __forceinline__ long long cell_of(const int32_t *__restrict__ geom_feats, int row,
-                                             const PoolDims dm) {
-  // flat index into out[b][d][h][w] from (x, y, z, b) = geom_feats[row] (bev_pool_cuda.cu:34-36)
-  int4 g = *reinterpret_cast<const int4 *>(geom_feats + 4ll * row);
-  if ((unsigned)g.x >= (unsigned)dm.h || (unsigned)g.y >= (unsigned)dm.w ||
-      (unsigned)g.z >= (unsigned)dm.d || (unsigned)g.w >= (unsigned)dm.b)
-    return -1;
-  return (((long long)g.w * dm.d + g.z) * dm.h + g.x) * dm.w + g.y;
-}
+constexpr int kChunkRows = 128;            // backward: rows of the sorted stream owned by one warp
+constexpr int kPoolWarps = 8;              // backward: warps per CTA
 
 // last index i in [0, n) with starts[i] <= row, or -1
 __device__ __forceinline__ int find_interval(const int32_t *__restrict__ starts, int n, int row) {
@@ -54,158 +34,7 @@ __device__ __forceinline__ int find_interval(const int32_t *__restrict__ starts,
 }
 
 // ---------------------------------------------------------------------------------------
-// forward
-// ---------------------------------------------------------------------------------------
-// Q = C/4 float4 per row, G rows per warp step, T = G*Q/32 float4 per lane per step.
-template <int Q, int G>
-struct PoolCfg {
-  static constexpr int T = G * Q / 32;
-  static_assert(G * Q % 32 == 0, "a warp step must be a whole number of float4 per lane");
-  static_assert(32 % G == 0, "G must divide the 32-row perm block");
-};
-
-template <int Q, int G>
-__device__ __forceinline__ void reduce_piece(const float4 *__restrict__ x,
-                                             const int32_t *__restrict__ perm, int s, int e,
-                                             float4 *__restrict__ dst, float4 *sm /*[G*Q]*/) {
-  constexpr int T = PoolCfg<Q, G>::T;
-  const int lane = lane_id();
-  int rig[T], qq[T];
-#pragma unroll
-  for (int t = 0; t < T; ++t) {
-    int f = lane + 32 * t;
-    rig[t] = f / Q;
-    qq[t] = f % Q;
-  }
-  float4 acc[T];
-#pragma unroll
-  for (int t = 0; t < T; ++t) acc[t] = make_float4(0.f, 0.f, 0.f, 0.f);
-
-  for (int r0 = s; r0 < e; r0 += 32) {
-    // source rows of this 32-row block, one per lane
-    int row = r0 + lane;
-    int src = row < e ? (perm ? __ldg(perm + row) : row) : 0;
-    const int nrows = min(32, e - r0);
-#pragma unroll 1
-    for (int g0 = 0; g0 < nrows; g0 += 2 * G) {
-      float4 va[T], vb[T];
-#pragma unroll
-      for (int t = 0; t < T; ++t) {
-        int ra = g0 + rig[t];
-        int sa = __shfl_sync(0xffffffffu, src, ra & 31);
-        va[t] = ra < nrows ? ldg_stream_f4(x + (long long)sa * Q + qq[t])
-                           : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-      if (2 * G <= 32) {
-#pragma unroll
-        for (int t = 0; t < T; ++t) {
-          int rb = g0 + G + rig[t];
-          int sb = __shfl_sync(0xffffffffu, src, rb & 31);
-          vb[t] = rb < nrows ? ldg_stream_f4(x + (long long)sb * Q + qq[t])
-                             : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-      }
-#pragma unroll
-      for (int t = 0; t < T; ++t) {
-        acc[t].x += va[t].x; acc[t].y += va[t].y; acc[t].z += va[t].z; acc[t].w += va[t].w;
-      }
-      if (2 * G <= 32) {
-#pragma unroll
-        for (int t = 0; t < T; ++t) {
-          acc[t].x += vb[t].x; acc[t].y += vb[t].y; acc[t].z += vb[t].z; acc[t].w += vb[t].w;
-        }
-      }
-    }
-  }
-  // fold the G row-slots of every quad (fixed order) and store the finished row
-  __syncwarp();
-#pragma unroll
-  for (int t = 0; t < T; ++t) sm[lane + 32 * t] = acc[t];
-  __syncwarp();
-  for (int q = lane; q < Q; q += 32) {
-    float4 r = sm[q];
-#pragma unroll
-    for (int g = 1; g < G; ++g) {
-      float4 v = sm[g * Q + q];
-      r.x += v.x; r.y += v.y; r.z += v.z; r.w += v.w;
-    }
-    dst[q] = r;
-  }
-  __syncwarp();
-}
-
-template <int Q, int G>
-__global__ void __launch_bounds__(kPoolWarps * 32)
-    bevpool_fwd_kernel(const float4 *__restrict__ x, const int32_t *__restrict__ perm,
-                       const int32_t *__restrict__ geom_feats,
-                       const int32_t *__restrict__ starts, const int32_t *__restrict__ lengths,
-                       int n, int n_intervals, PoolDims dm, float4 *__restrict__ out,
-                       float4 *__restrict__ partial) {
-  __shared__ float4 sm_all[kPoolWarps][G * Q];
-  float4 *sm = sm_all[threadIdx.x >> 5];
-  const int nchunks = (n + kChunkRows - 1) / kChunkRows;
-  const int warps_total = gridDim.x * kPoolWarps;
-  for (int j = blockIdx.x * kPoolWarps + (threadIdx.x >> 5); j < nchunks; j += warps_total) {
-    const int c0 = j * kChunkRows, c1 = min(n, c0 + kChunkRows);
-    int i = find_interval(starts, n_intervals, c0);
-    // (a) a long interval that began before this chunk and reaches into it
-    if (i >= 0) {
-      int s = __ldg(starts + i), L = __ldg(lengths + i);
-      if (s < c0 && L > kLongRows && s + L > c0)
-        reduce_piece<Q, G>(x, perm, c0, min(s + L, c1), partial + (2ll * j) * Q, sm);
-      if (s < c0) ++i;
-    } else {
-      i = 0;
-    }
-    // (b) intervals whose first row lies in this chunk
-    for (; i < n_intervals; ++i) {
-      int s = __ldg(starts + i);
-      if (s >= c1) break;
-      int L = __ldg(lengths + i);
-      if (L <= 0) continue;
-      int e = min(s + L, n);
-      if (L > kLongRows) {
-        reduce_piece<Q, G>(x, perm, s, min(e, c1), partial + (2ll * j + 1) * Q, sm);
-      } else {
-        long long cell = cell_of(geom_feats, s, dm);
-        if (cell >= 0) reduce_piece<Q, G>(x, perm, s, e, out + cell * Q, sm);
-      }
-    }
-  }
-}
-
-// adds the pieces of every long interval in chunk order (one warp per interval)
-template <int Q>
-__global__ void __launch_bounds__(256)
-    bevpool_fwd_fixup_kernel(const int32_t *__restrict__ geom_feats,
-                             const int32_t *__restrict__ starts,
-                             const int32_t *__restrict__ lengths, int n, int n_intervals,
-                             PoolDims dm, float4 *__restrict__ out,
-                             const float4 *__restrict__ partial) {
-  const int lane = lane_id();
-  const int warps_total = gridDim.x * (blockDim.x >> 5);
-  for (int i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); i < n_intervals;
-       i += warps_total) {
-    int L = __ldg(lengths + i);
-    if (L <= kLongRows) continue;
-    int s = __ldg(starts + i);
-    int e = min(s + L, n);
-    long long cell = cell_of(geom_feats, s, dm);
-    if (cell < 0 || e <= s) continue;
-    int jf = s / kChunkRows, jl = (e - 1) / kChunkRows;
-    for (int q = lane; q < Q; q += 32) {
-      float4 r = partial[(2ll * jf + 1) * Q + q];
-      for (int j = jf + 1; j <= jl; ++j) {
-        float4 v = partial[(2ll * j) * Q + q];
-        r.x += v.x; r.y += v.y; r.z += v.z; r.w += v.w;
-      }
-      out[cell * Q + q] = r;
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------------------
-// forward, v2: TMA-staged streaming reduction (the default for the tuned channel widths)
+// forward: TMA-staged streaming reduction (the tuned channel widths)
 // ---------------------------------------------------------------------------------------
 // Every warp owns a contiguous range of the sorted row stream and runs its own
 // cp.async.bulk -> shared memory ring (32 rows per stage, mbarrier complete_tx), so the bytes in
@@ -241,11 +70,8 @@ __device__ __forceinline__ void pool_mbar_wait(uint32_t bar, uint32_t parity) {
 __global__ void pool_interval_cells_kernel(const int32_t *__restrict__ geom_feats,
                                            const int32_t *__restrict__ starts, int n, int n_intervals,
                                            PoolDims dm, int32_t *__restrict__ cells) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_intervals; i += gridDim.x * blockDim.x) {
-    int s = starts[i];
-    long long c = (s >= 0 && s < n) ? cell_of(geom_feats, s, dm) : -1;
-    cells[i] = (int32_t)c;  // host guarantees b*d*h*w < 2^31
-  }
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_intervals; i += gridDim.x * blockDim.x)
+    cells[i] = interval_cell(geom_feats, starts[i], n, dm);
 }
 
 // MODE 0: rows already sorted (one TMA bulk copy per stage); MODE 1: rows gathered through perm;
@@ -576,6 +402,16 @@ __global__ void bevpool_fwd_generic_kernel(const float *__restrict__ x,
 // ---------------------------------------------------------------------------------------
 // backward: x_grad[row, :] = out_grad[cell(interval(row)), :]
 // ---------------------------------------------------------------------------------------
+// Q = C/4 float4 per row, G rows per warp step, T = G*Q/32 float4 per lane per step.
+template <int Q, int G>
+struct PoolCfg {
+  static constexpr int T = G * Q / 32;
+  static_assert(G * Q % 32 == 0, "a warp step must be a whole number of float4 per lane");
+  static_assert(32 % G == 0, "G must divide the 32-row perm block");
+};
+// G of each tuned width: 3 to 5 float4 per lane per step
+constexpr int bwd_rows_per_step(int q) { return q <= 4 ? 32 : q <= 8 ? 16 : q <= 20 ? 8 : q <= 40 ? 4 : 2; }
+
 template <int Q, int G>
 __global__ void __launch_bounds__(kPoolWarps * 32)
     bevpool_bwd_kernel(const float4 *__restrict__ out_grad, const int32_t *__restrict__ perm,
@@ -676,40 +512,34 @@ __global__ void bevpool_bwd_generic_kernel(const float *__restrict__ out_grad,
 // host dispatch
 // ---------------------------------------------------------------------------------------
 constexpr int kTmaMaxRanges = kNumSMs * 8;   // warp ranges of the TMA-staged kernel (<= 8 warps per SM)
-static size_t pool_partial_bytes(int n, int c) {
-  size_t nchunks = ((size_t)n + kChunkRows - 1) / kChunkRows;
-  if (nchunks < (size_t)kTmaMaxRanges) nchunks = kTmaMaxRanges;
-  // partial rows (2 per chunk / warp range) + one int32 cell id per interval (<= n of them)
-  return align_up(2 * nchunks * (size_t)c * sizeof(float)) + align_up((size_t)n * sizeof(int32_t));
-}
 
-template <int Q, int G>
-static int launch_fwd(const float *x, const int32_t *perm, const int32_t *geom,
-                      const int32_t *starts, const int32_t *lengths, int n, int n_intervals,
-                      PoolDims dm, float *out, float *partial, cudaStream_t st) {
-  int nchunks = (n + kChunkRows - 1) / kChunkRows;
-  int grid = min((nchunks + kPoolWarps - 1) / kPoolWarps, kNumSMs * 4);
-  BEVB200_LAUNCH((bevpool_fwd_kernel<Q, G>), grid, kPoolWarps * 32, 0, st, (const float4 *)x, perm,
-                 geom, starts, lengths, n, n_intervals, dm, (float4 *)out, (float4 *)partial);
-  int fgrid = min((n_intervals + 7) / 8, kNumSMs * 4);
-  BEVB200_LAUNCH((bevpool_fwd_fixup_kernel<Q>), fgrid, 256, 0, st, geom, starts, lengths, n,
-                 n_intervals, dm, (float4 *)out, (const float4 *)partial);
-  return BEVB200_OK;
+// Workspace of the TMA-staged forward (pooling and the row lift): two partial rows per warp range, then one cell per
+// interval (<= n of them).  It holds max(ceil(n / kChunkRows), kTmaMaxRanges) ranges, more than the kernel uses;
+// bevb200_bev_pool_workspace_bytes reports this size.
+struct PoolTmaWs {
+  float *partial;
+  int32_t *cells;
+};
+static size_t pool_tma_layout(int n, int c, void *ws, PoolTmaWs *out) {
+  size_t ranges = ((size_t)n + kChunkRows - 1) / kChunkRows;
+  if (ranges < (size_t)kTmaMaxRanges) ranges = kTmaMaxRanges;
+  Arena a(ws, 0);
+  PoolTmaWs w;
+  w.partial = a.take<float>(2 * ranges * (size_t)c);
+  w.cells = a.take<int32_t>((size_t)n);
+  if (out) *out = w;
+  return a.off;
 }
 
 template <int Q>
 static int launch_fwd_tma(const float *x, const int32_t *perm, const int32_t *geom,
-                          const int32_t *starts, const int32_t *lengths, int n, int c, int n_intervals,
-                          PoolDims dm, float *out, void *ws, int zfill, cudaStream_t st,
+                          const int32_t *starts, const int32_t *lengths, int n, int n_intervals,
+                          PoolDims dm, float *out, const PoolTmaWs &ws, int zfill, cudaStream_t st,
                           const float *depth = nullptr, LiftDims lift = LiftDims{1, 1}) {
   // MODE 1 / 2 tables tile [0, n): their interval ends are the next starts
   const int32_t *mode0_lengths = (depth == nullptr && perm == nullptr) ? lengths : nullptr;
-  size_t nchunks = ((size_t)n + kChunkRows - 1) / kChunkRows;
-  if (nchunks < (size_t)kTmaMaxRanges) nchunks = kTmaMaxRanges;
-  float *partial = (float *)ws;
-  int32_t *cells = (int32_t *)((char *)ws + align_up(2 * nchunks * (size_t)c * sizeof(float)));
   BEVB200_LAUNCH(pool_interval_cells_kernel, grid_for(n_intervals, 256), 256, 0, st, geom, starts, n,
-                 n_intervals, dm, cells);
+                 n_intervals, dm, ws.cells);
   const size_t stage_bytes = (size_t)kStageRows * Q * 16 + (depth ? 128 : 0);
   int warps = (int)((200 * 1024) / (kPoolStages * stage_bytes));
   if (warps > 8) warps = 8;
@@ -720,50 +550,28 @@ static int launch_fwd_tma(const float *x, const int32_t *perm, const int32_t *ge
   rpw = (rpw + kStageRows - 1) / kStageRows * kStageRows;
   const int n_ranges = (n + rpw - 1) / rpw;
   const int grid = (n_ranges + warps - 1) / warps;
-#define BEVB200_POOL_TMA_LAUNCH(MODE)                                                             \
-  do {                                                                                              \
-    BEVB200_CUDA(cudaFuncSetAttribute(bevpool_fwd_tma_kernel<Q, MODE>,                              \
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));      \
-    BEVB200_LAUNCH((bevpool_fwd_tma_kernel<Q, MODE>), grid, warps * 32, smem, st, (const float4 *)x,       \
-                   perm, depth, lift, starts, cells, n, n_intervals, rpw, zfill,  \
-                   dm.b * dm.d * dm.h * dm.w, (float4 *)out, (float4 *)partial, mode0_lengths);      \
-  } while (0)
-  if (depth) BEVB200_POOL_TMA_LAUNCH(2);
-  else if (perm) BEVB200_POOL_TMA_LAUNCH(1);
-  else BEVB200_POOL_TMA_LAUNCH(0);
-#undef BEVB200_POOL_TMA_LAUNCH
-  BEVB200_LAUNCH((bevpool_fwd_tma_fixup_kernel<Q>), (n_ranges * 32 + 255) / 256, 256, 0, st, starts, cells, n,
-                 n_intervals, rpw, n_ranges, (float4 *)out, (const float4 *)partial, mode0_lengths);
+  const auto kernel = depth  ? &bevpool_fwd_tma_kernel<Q, 2>
+                      : perm ? &bevpool_fwd_tma_kernel<Q, 1>
+                             : &bevpool_fwd_tma_kernel<Q, 0>;
+  BEVB200_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  BEVB200_LAUNCH(kernel, grid, warps * 32, smem, st, (const float4 *)x, perm, depth, lift, starts, ws.cells, n,
+                 n_intervals, rpw, zfill, dm.b * dm.d * dm.h * dm.w, (float4 *)out, (float4 *)ws.partial,
+                 mode0_lengths);
+  BEVB200_LAUNCH((bevpool_fwd_tma_fixup_kernel<Q>), (n_ranges * 32 + 255) / 256, 256, 0, st, starts, ws.cells, n,
+                 n_intervals, rpw, n_ranges, (float4 *)out, (const float4 *)ws.partial, mode0_lengths);
   return BEVB200_OK;
 }
 
-template <int Q, int G>
+template <int Q>
 static int launch_bwd(const float *og, const int32_t *perm, const int32_t *geom,
                       const int32_t *starts, const int32_t *lengths, int n, int n_total,
                       int n_intervals, PoolDims dm, float *xg, cudaStream_t st) {
   int nchunks = (n_total + kChunkRows - 1) / kChunkRows;
   int grid = min((nchunks + kPoolWarps - 1) / kPoolWarps, kNumSMs * 4);
-  BEVB200_LAUNCH((bevpool_bwd_kernel<Q, G>), grid, kPoolWarps * 32, 0, st, (const float4 *)og, perm,
-                 geom, starts, lengths, n, n_total, n_intervals, dm, (float4 *)xg);
+  BEVB200_LAUNCH((bevpool_bwd_kernel<Q, bwd_rows_per_step(Q)>), grid, kPoolWarps * 32, 0, st, (const float4 *)og,
+                 perm, geom, starts, lengths, n, n_total, n_intervals, dm, (float4 *)xg);
   return BEVB200_OK;
 }
-
-#define BEVB200_POOL_DISPATCH(C, CALL, FALLBACK) \
-  switch (C) {                                   \
-    case 16: CALL(4, 32); break;                 \
-    case 32: CALL(8, 16); break;                 \
-    case 64: CALL(16, 8); break;                 \
-    case 80: CALL(20, 8); break;                 \
-    case 96: CALL(24, 4); break;                 \
-    case 128: CALL(32, 4); break;                \
-    case 160: CALL(40, 4); break;                \
-    case 256: CALL(64, 2); break;                \
-    default: FALLBACK; break;                    \
-  }
-
-// 0 = TMA-staged streaming kernel (default), 1 = register-gather kernel (v1).  Selected by the
-// environment variable BEVB200_POOL_VARIANT at first use (kept for A/B measurements).
-static int g_pool_variant = -1;
 
 static int pool_forward(int b, int d, int h, int w, int n, int c, int n_intervals, const float *x,
                         const int32_t *perm, const int32_t *geom, const int32_t *starts,
@@ -774,53 +582,32 @@ static int pool_forward(int b, int d, int h, int w, int n, int c, int n_interval
   BEVB200_REQUIRE(out != nullptr, "null out");
   BEVB200_REQUIRE((long long)b * d * h * w * c < (1ll << 40), "output too large");
   BEVB200_REQUIRE((long long)b * d * h * w < (1ll << 31), "grid has too many cells");
-  if (g_pool_variant < 0) {
-    const char *e = getenv("BEVB200_POOL_VARIANT");
-    g_pool_variant = (e && e[0] == '1') ? 1 : 0;
-  }
   cudaStream_t st = (cudaStream_t)stream;
   size_t out_bytes = (size_t)b * d * h * w * c * sizeof(float);
-  // plan tables (perm != null) with B*D == 1 are in ascending cell order: the pooling kernel
-  // zero-fills the empty cells itself; every other case pre-zeroes the grid
-  bool tuned = false;
-  switch (c) { case 16: case 32: case 64: case 80: case 96: case 128: case 160: case 256: tuned = true; }
-  const bool aligned = ((uintptr_t)x % 16 == 0) && ((uintptr_t)out % 16 == 0);
+  // the TMA-staged kernel takes the tuned widths on 16-byte aligned rows, the generic one everything else
+  const bool tma = TunedWidths::has(c) && ((uintptr_t)x % 16 == 0) && ((uintptr_t)out % 16 == 0);
   const bool work = n > 0 && n_intervals > 0;
   // every argument is checked before `out` is written: a refused call leaves it untouched
+  PoolTmaWs tws;
   if (work) {
     BEVB200_REQUIRE(x && geom && starts && lengths, "null input");
-    if (tuned && aligned && (ws == nullptr || ws_bytes < pool_partial_bytes(n, c))) {
-      snprintf(g_last_error, sizeof(g_last_error), "bev_pool: workspace too small (%zu < %zu)", ws_bytes,
-               pool_partial_bytes(n, c));
-      return BEVB200_EWORKSPACE;
-    }
+    if (tma)
+      if (const int rc = workspace_check("bev_pool", ws, ws_bytes, pool_tma_layout(n, c, ws, &tws))) return rc;
   }
-  const int zfill = (perm != nullptr && b * d == 1 && work && tuned && aligned && g_pool_variant == 0 &&
-                     trust_tables) ? 1 : 0;
+  // plan tables (perm != null) with B*D == 1 are in ascending cell order: the pooling kernel
+  // zero-fills the empty cells itself; every other case pre-zeroes the grid
+  const int zfill = (perm != nullptr && b * d == 1 && work && tma && trust_tables) ? 1 : 0;
   if (!zfill) BEVB200_CUDA(cudaMemsetAsync(out, 0, out_bytes, st));
   if (!work) return BEVB200_OK;
   PoolDims dm{b, d, h, w};
-  int rc = BEVB200_OK;
-#define CALL_FWD(Q, G)                                                                         \
-  do {                                                                                         \
-    if (g_pool_variant == 1)                                                                   \
-      rc = launch_fwd<Q, G>(x, perm, geom, starts, lengths, n, n_intervals, dm, out, (float *)ws, st); \
-    else                                                                                       \
-      rc = launch_fwd_tma<Q>(x, perm, geom, starts, lengths, n, c, n_intervals, dm, out, ws, zfill, st); \
-  } while (0)
-#define CALL_FWD_GENERIC()                                                                     \
-  do {                                                                                         \
-    BEVB200_LAUNCH(bevpool_fwd_generic_kernel, grid_for((long long)n_intervals * c, 256), 256, 0, \
-                   st, x, perm, geom, starts, lengths, n, c, n_intervals, dm, out);            \
-  } while (0)
-  if (!aligned) {
-    CALL_FWD_GENERIC();
-  } else {
-    BEVB200_POOL_DISPATCH(c, CALL_FWD, CALL_FWD_GENERIC());
+  if (!tma) {
+    BEVB200_LAUNCH(bevpool_fwd_generic_kernel, grid_for((long long)n_intervals * c, 256), 256, 0, st, x, perm, geom,
+                   starts, lengths, n, c, n_intervals, dm, out);
+    return BEVB200_OK;
   }
-#undef CALL_FWD
-#undef CALL_FWD_GENERIC
-  return rc;
+  return TunedWidths::dispatch(c, [&](auto q) {
+    return launch_fwd_tma<decltype(q)::value>(x, perm, geom, starts, lengths, n, n_intervals, dm, out, tws, zfill, st);
+  });
 }
 
 static int pool_backward(int b, int d, int h, int w, int n, int n_total, int c, int n_intervals,
@@ -837,24 +624,15 @@ static int pool_backward(int b, int d, int h, int w, int n, int n_total, int c, 
   }
   BEVB200_REQUIRE(og && geom && starts && lengths, "null input");
   PoolDims dm{b, d, h, w};
-  int rc = BEVB200_OK;
-  bool aligned = ((uintptr_t)og % 16 == 0) && ((uintptr_t)xg % 16 == 0);
-#define CALL_BWD(Q, G) \
-  rc = launch_bwd<Q, G>(og, perm, geom, starts, lengths, n, n_total, n_intervals, dm, xg, st)
-#define CALL_BWD_GENERIC()                                                                     \
-  do {                                                                                         \
-    BEVB200_CUDA(cudaMemsetAsync(xg, 0, (size_t)n_total * c * sizeof(float), st));             \
-    BEVB200_LAUNCH(bevpool_bwd_generic_kernel, grid_for((long long)n_intervals * c, 256), 256, 0, \
-                   st, og, perm, geom, starts, lengths, n, c, n_intervals, dm, xg);            \
-  } while (0)
-  if (!aligned) {
-    CALL_BWD_GENERIC();
-  } else {
-    BEVB200_POOL_DISPATCH(c, CALL_BWD, CALL_BWD_GENERIC());
+  if (!TunedWidths::has(c) || (uintptr_t)og % 16 != 0 || (uintptr_t)xg % 16 != 0) {
+    BEVB200_CUDA(cudaMemsetAsync(xg, 0, (size_t)n_total * c * sizeof(float), st));
+    BEVB200_LAUNCH(bevpool_bwd_generic_kernel, grid_for((long long)n_intervals * c, 256), 256, 0, st, og, perm, geom,
+                   starts, lengths, n, c, n_intervals, dm, xg);
+    return BEVB200_OK;
   }
-#undef CALL_BWD
-#undef CALL_BWD_GENERIC
-  return rc;
+  return TunedWidths::dispatch(c, [&](auto q) {
+    return launch_bwd<decltype(q)::value>(og, perm, geom, starts, lengths, n, n_total, n_intervals, dm, xg, st);
+  });
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1017,9 +795,37 @@ static size_t prepare_layout(int n, void *ws, size_t ws_bytes, PrepareWs *out) {
   return a.off;
 }
 
-static int prepare_finish(PrepareWs &w, int n, long long total_cells, int B, int D, int W,
-                          int32_t *ranks_sorted, int32_t *perm, int32_t *geom_sorted,
-                          int32_t *starts, int32_t *lengths, int32_t *counts, cudaStream_t st) {
+static QuantParams quant_params(const float *lower, const float *dx, const int32_t *nx, int B, int n_per_batch) {
+  QuantParams p;
+  for (int k = 0; k < 3; ++k) {
+    p.lower[k] = lower[k];
+    p.dx[k] = dx[k];
+    p.nx[k] = nx[k];
+  }
+  p.B = B;
+  p.n_per_batch = n_per_batch;
+  return p;
+}
+
+// What the three prepare entries share: the grid and output checks, the empty call, the workspace check, then the
+// entry's rank kernel -- rank(w, dropped_key) fills w.keys_a with each point's rank (dropped_key = B*D*H*W for a
+// filtered point) and w.vals_a with its index -- and the sort and interval passes.
+template <typename Rank>
+static int prepare_tables(const void *points, int n, int B, int D, int H, int W, int32_t *ranks_sorted, int32_t *perm,
+                          int32_t *geom_sorted, int32_t *starts, int32_t *lengths, int32_t *counts, void *ws,
+                          size_t ws_bytes, cudaStream_t st, Rank &&rank) {
+  BEVB200_REQUIRE(B > 0 && D > 0 && H > 0 && W > 0, "bad grid");
+  const long long total_cells = (long long)B * D * H * W;
+  BEVB200_REQUIRE(total_cells < 0xfffffff0ll, "grid too large for 32-bit ranks");
+  BEVB200_REQUIRE(counts != nullptr, "null counts");
+  if (n == 0) {
+    BEVB200_CUDA(cudaMemsetAsync(counts, 0, 2 * sizeof(int32_t), st));
+    return BEVB200_OK;
+  }
+  BEVB200_REQUIRE(points && ranks_sorted && perm && geom_sorted && starts && lengths, "null argument");
+  PrepareWs w;
+  if (const int rc = workspace_check("bev_pool_prepare", ws, ws_bytes, prepare_layout(n, ws, ws_bytes, &w))) return rc;
+  if (const int rc = rank(w, (uint32_t)total_cells)) return rc;
   int end_bit = 1;
   while ((1ll << end_bit) <= total_cells && end_bit < 32) ++end_bit;  // keys in [0, total_cells]
   size_t cub_bytes = w.cub_bytes;
@@ -1046,7 +852,7 @@ extern "C" {
 
 size_t bevb200_bev_pool_workspace_bytes(int n, int c) {
   if (n < 0 || c <= 0) return 0;
-  return pool_partial_bytes(n, c);
+  return pool_tma_layout(n, c, nullptr, nullptr);
 }
 
 int bevb200_bev_pool(int b, int d, int h, int w, int n, int c, int n_intervals, const float *x,
@@ -1093,23 +899,27 @@ int bevb200_bev_pool_lift(int b, int d, int h, int w, int n, int c, int n_interv
   BEVB200_REQUIRE(out != nullptr, "null out");
   BEVB200_REQUIRE(depth_bins > 0 && pixels_per_camera > 0, "bad lift dims");
   BEVB200_REQUIRE((long long)b * d * h * w < (1ll << 31), "grid has too many cells");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int zfill = (b * d == 1 && n > 0 && n_intervals > 0) ? 1 : 0;
-  if (!zfill) BEVB200_CUDA(cudaMemsetAsync(out, 0, (size_t)b * d * h * w * c * sizeof(float), st));
-  if (n == 0 || n_intervals == 0) return BEVB200_OK;
-  BEVB200_REQUIRE(depth && ctx && perm && geom_feats && interval_starts, "null input");
-  BEVB200_REQUIRE(((uintptr_t)ctx % 16 == 0) && ((uintptr_t)out % 16 == 0), "ctx / out must be 16-byte aligned");
-  if (workspace == nullptr || workspace_bytes < pool_partial_bytes(n, c)) {
-    snprintf(g_last_error, sizeof(g_last_error), "bev_pool_lift: workspace too small");
-    return BEVB200_EWORKSPACE;
+  const bool work = n > 0 && n_intervals > 0;
+  // every argument is checked before `out` is written: a refused call leaves it untouched
+  PoolTmaWs ws;
+  if (work) {
+    BEVB200_REQUIRE(depth && ctx && perm && geom_feats && interval_starts, "null input");
+    BEVB200_REQUIRE(((uintptr_t)ctx % 16 == 0) && ((uintptr_t)out % 16 == 0), "ctx / out must be 16-byte aligned");
+    if (const int rc = workspace_check("bev_pool_lift", workspace, workspace_bytes, pool_tma_layout(n, c, workspace, &ws)))
+      return rc;
+    BEVB200_REQUIRE(TunedWidths::has(c), "no tuned kernel for this channel count");
   }
+  cudaStream_t st = (cudaStream_t)stream;
+  // the tables tile [0, n) in ascending cell order: at B*D == 1 the kernel zero-fills the empty cells itself
+  const int zfill = (b * d == 1 && work) ? 1 : 0;
+  if (!zfill) BEVB200_CUDA(cudaMemsetAsync(out, 0, (size_t)b * d * h * w * c * sizeof(float), st));
+  if (!work) return BEVB200_OK;
   PoolDims dm{b, d, h, w};
   LiftDims lift{depth_bins, pixels_per_camera};
-#define CALL_LIFT(Q, G) return launch_fwd_tma<Q>(ctx, perm, geom_feats, interval_starts, nullptr, n, c, n_intervals, \
-                                                 dm, out, workspace, zfill, st, depth, lift)
-  BEVB200_POOL_DISPATCH(c, CALL_LIFT, BEVB200_REQUIRE(false, "bev_pool_lift: channel count not in {16,32,64,80,96,128,160,256}"));
-#undef CALL_LIFT
-  return BEVB200_OK;
+  return TunedWidths::dispatch(c, [&](auto q) {
+    return launch_fwd_tma<decltype(q)::value>(ctx, perm, geom_feats, interval_starts, nullptr, n, n_intervals, dm, out,
+                                              ws, zfill, st, depth, lift);
+  });
 }
 
 int bevb200_bev_channels_first(const float *in, float *out, int batch, int nz, int rows, int c,
@@ -1136,38 +946,18 @@ int bevb200_bev_pool_prepare_geom(const float *geom_xyz, int n_total, int n_per_
                                   int32_t *interval_lengths, int32_t *counts, void *workspace,
                                   size_t workspace_bytes, void *stream) {
   BEVB200_REQUIRE(n_total >= 0 && B > 0 && n_per_batch > 0, "bad sizes");
-  BEVB200_REQUIRE(lower_host && dx_host && nx_host && counts, "null argument");
+  BEVB200_REQUIRE(lower_host && dx_host && nx_host, "null argument");
   BEVB200_REQUIRE((long long)n_per_batch * B >= n_total, "n_per_batch * B < n_total");
-  long long total_cells = (long long)nx_host[0] * nx_host[1] * nx_host[2] * B;
-  BEVB200_REQUIRE(nx_host[0] > 0 && nx_host[1] > 0 && nx_host[2] > 0, "bad grid");
-  BEVB200_REQUIRE(total_cells < 0xfffffff0ll, "grid too large for 32-bit ranks");
   cudaStream_t st = (cudaStream_t)stream;
-  if (n_total == 0) {
-    BEVB200_CUDA(cudaMemsetAsync(counts, 0, 2 * sizeof(int32_t), st));
-    return BEVB200_OK;
-  }
-  BEVB200_REQUIRE(geom_xyz && ranks_sorted && perm && geom_sorted && interval_starts &&
-                      interval_lengths, "null argument");
-  PrepareWs w;
-  size_t need = prepare_layout(n_total, workspace, workspace_bytes, &w);
-  if (workspace == nullptr || workspace_bytes < need) {
-    snprintf(g_last_error, sizeof(g_last_error), "bev_pool_prepare: workspace too small (%zu < %zu)",
-             workspace_bytes, need);
-    return BEVB200_EWORKSPACE;
-  }
-  QuantParams p;
-  for (int k = 0; k < 3; ++k) {
-    p.lower[k] = lower_host[k];
-    p.dx[k] = dx_host[k];
-    p.nx[k] = nx_host[k];
-  }
-  p.B = B;
-  p.n_per_batch = n_per_batch;
-  BEVB200_LAUNCH(pool_rank_from_geom_kernel, grid_for(n_total, 256), 256, 0, st, geom_xyz, n_total,
-                 p, (uint32_t)total_cells, w.keys_a, w.vals_a);
+  const QuantParams p = quant_params(lower_host, dx_host, nx_host, B, n_per_batch);
   // (B, D, H, W) = (B, nz, nx, ny)
-  return prepare_finish(w, n_total, total_cells, B, nx_host[2], nx_host[1], ranks_sorted, perm,
-                        geom_sorted, interval_starts, interval_lengths, counts, st);
+  return prepare_tables(geom_xyz, n_total, B, nx_host[2], nx_host[0], nx_host[1], ranks_sorted, perm, geom_sorted,
+                        interval_starts, interval_lengths, counts, workspace, workspace_bytes, st,
+                        [&](PrepareWs &w, uint32_t dropped_key) {
+                          BEVB200_LAUNCH(pool_rank_from_geom_kernel, grid_for(n_total, 256), 256, 0, st, geom_xyz,
+                                         n_total, p, dropped_key, w.keys_a, w.vals_a);
+                          return BEVB200_OK;
+                        });
 }
 
 int bevb200_bev_pool_prepare_cameras(const float *frustum, int n_frustum, int cameras, int cams_per_batch,
@@ -1178,32 +968,18 @@ int bevb200_bev_pool_prepare_cameras(const float *frustum, int n_frustum, int ca
                                      void *workspace, size_t workspace_bytes, void *stream) {
   BEVB200_REQUIRE(n_frustum > 0 && cameras > 0 && cams_per_batch > 0 && B > 0 && cameras == B * cams_per_batch, "bad sizes");
   BEVB200_REQUIRE((long long)n_frustum * cameras < (1ll << 31), "too many frustum points");
-  BEVB200_REQUIRE(frustum && cam_params && lower_host && dx_host && nx_host && counts, "null argument");
+  BEVB200_REQUIRE(frustum && cam_params && lower_host && dx_host && nx_host, "null argument");
   const int n_total = n_frustum * cameras;
-  long long total_cells = (long long)nx_host[0] * nx_host[1] * nx_host[2] * B;
-  BEVB200_REQUIRE(nx_host[0] > 0 && nx_host[1] > 0 && nx_host[2] > 0, "bad grid");
-  BEVB200_REQUIRE(total_cells < 0xfffffff0ll, "grid too large for 32-bit ranks");
-  BEVB200_REQUIRE(ranks_sorted && perm && geom_sorted && interval_starts && interval_lengths, "null argument");
   cudaStream_t st = (cudaStream_t)stream;
-  PrepareWs w;
-  size_t need = prepare_layout(n_total, workspace, workspace_bytes, &w);
-  if (workspace == nullptr || workspace_bytes < need) {
-    snprintf(g_last_error, sizeof(g_last_error), "bev_pool_prepare: workspace too small (%zu < %zu)",
-             workspace_bytes, need);
-    return BEVB200_EWORKSPACE;
-  }
-  QuantParams p;
-  for (int k = 0; k < 3; ++k) {
-    p.lower[k] = lower_host[k];
-    p.dx[k] = dx_host[k];
-    p.nx[k] = nx_host[k];
-  }
-  p.B = B;
-  p.n_per_batch = n_frustum * cams_per_batch;
-  BEVB200_LAUNCH(pool_rank_from_cameras_kernel, grid_for(n_total, 256), 256, 0, st, frustum, n_frustum, cams_per_batch,
-                 cam_params, extra_params, n_total, p, (uint32_t)total_cells, w.keys_a, w.vals_a, geom_out);
-  return prepare_finish(w, n_total, total_cells, B, nx_host[2], nx_host[1], ranks_sorted, perm, geom_sorted,
-                        interval_starts, interval_lengths, counts, st);
+  const QuantParams p = quant_params(lower_host, dx_host, nx_host, B, n_frustum * cams_per_batch);
+  return prepare_tables(frustum, n_total, B, nx_host[2], nx_host[0], nx_host[1], ranks_sorted, perm, geom_sorted,
+                        interval_starts, interval_lengths, counts, workspace, workspace_bytes, st,
+                        [&](PrepareWs &w, uint32_t dropped_key) {
+                          BEVB200_LAUNCH(pool_rank_from_cameras_kernel, grid_for(n_total, 256), 256, 0, st, frustum,
+                                         n_frustum, cams_per_batch, cam_params, extra_params, n_total, p, dropped_key,
+                                         w.keys_a, w.vals_a, geom_out);
+                          return BEVB200_OK;
+                        });
 }
 
 int bevb200_bev_pool_prepare_coords(const int64_t *coords, int n, int B, int D, int H, int W,
@@ -1211,28 +987,14 @@ int bevb200_bev_pool_prepare_coords(const int64_t *coords, int n, int B, int D, 
                                     int32_t *interval_starts, int32_t *interval_lengths,
                                     int32_t *counts, void *workspace, size_t workspace_bytes,
                                     void *stream) {
-  BEVB200_REQUIRE(n >= 0 && B > 0 && D > 0 && H > 0 && W > 0, "bad sizes");
-  BEVB200_REQUIRE(counts != nullptr, "null counts");
-  long long total_cells = (long long)B * D * H * W;
-  BEVB200_REQUIRE(total_cells < 0xfffffff0ll, "grid too large for 32-bit ranks");
+  BEVB200_REQUIRE(n >= 0, "bad sizes");
   cudaStream_t st = (cudaStream_t)stream;
-  if (n == 0) {
-    BEVB200_CUDA(cudaMemsetAsync(counts, 0, 2 * sizeof(int32_t), st));
-    return BEVB200_OK;
-  }
-  BEVB200_REQUIRE(coords && ranks_sorted && perm && geom_sorted && interval_starts &&
-                      interval_lengths, "null argument");
-  PrepareWs w;
-  size_t need = prepare_layout(n, workspace, workspace_bytes, &w);
-  if (workspace == nullptr || workspace_bytes < need) {
-    snprintf(g_last_error, sizeof(g_last_error), "bev_pool_prepare: workspace too small (%zu < %zu)",
-             workspace_bytes, need);
-    return BEVB200_EWORKSPACE;
-  }
-  BEVB200_LAUNCH(pool_rank_from_coords_kernel, grid_for(n, 256), 256, 0, st,
-                 (const long long *)coords, n, B, D, H, W, (uint32_t)total_cells, w.keys_a, w.vals_a);
-  return prepare_finish(w, n, total_cells, B, D, W, ranks_sorted, perm, geom_sorted,
-                        interval_starts, interval_lengths, counts, st);
+  return prepare_tables(coords, n, B, D, H, W, ranks_sorted, perm, geom_sorted, interval_starts, interval_lengths,
+                        counts, workspace, workspace_bytes, st, [&](PrepareWs &w, uint32_t dropped_key) {
+                          BEVB200_LAUNCH(pool_rank_from_coords_kernel, grid_for(n, 256), 256, 0, st,
+                                         (const long long *)coords, n, B, D, H, W, dropped_key, w.keys_a, w.vals_a);
+                          return BEVB200_OK;
+                        });
 }
 
 }  // extern "C"

@@ -23,7 +23,7 @@
 // The backward (gradients of depth and ctx, section "backward" below) runs over the same segment tables.
 #include <cub/cub.cuh>
 
-#include "common.cuh"
+#include "bevpool.cuh"
 
 namespace bevb200 {
 
@@ -238,26 +238,6 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-struct PoolDimsL {
-  int b, d, h, w;
-};
-// cell of the sorted row s (the first row of an interval), -1 outside the grid
-__device__ __forceinline__ int32_t lift_cell_of(const int32_t *__restrict__ geom_feats, int s, int n, PoolDimsL dm) {
-  long long c = -1;
-  if (s >= 0 && s < n) {
-    const int4 g = *reinterpret_cast<const int4 *>(geom_feats + 4ll * s);   // (x, y, z, b): bev_pool_cuda.cu:32-36
-    if ((unsigned)g.x < (unsigned)dm.h && (unsigned)g.y < (unsigned)dm.w && (unsigned)g.z < (unsigned)dm.d &&
-        (unsigned)g.w < (unsigned)dm.b)
-      c = (((long long)g.w * dm.d + g.z) * dm.h + g.x) * dm.w + g.y;
-  }
-  return (int32_t)c;
-}
-__global__ void lift_interval_cells_kernel(const int32_t *__restrict__ geom_feats, const int32_t *__restrict__ starts,
-                                           int n, int n_intervals, PoolDimsL dm, int32_t *__restrict__ cells) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_intervals; i += gridDim.x * blockDim.x)
-    cells[i] = lift_cell_of(geom_feats, starts[i], n, dm);
-}
-
 // ---- backward ------------------------------------------------------------------------------------
 // With G = dL/dout and cell(p) the BEV cell of the kept frustum point p = (cam, d, h, w):
 //     ddepth[cam, d, h, w] = ctx[cam, h, w, :] . G[cell(p), :]        (0 for a filtered point)
@@ -268,9 +248,9 @@ __global__ void lift_interval_cells_kernel(const int32_t *__restrict__ geom_feat
 // cell of every segment (through its interval); -1 would mean "outside the grid" (cannot occur for prepared tables)
 __global__ void lift_seg_cells_kernel(const unsigned long long *__restrict__ seg_key, int n_seg,
                                       const int32_t *__restrict__ geom_feats, const int32_t *__restrict__ starts, int n,
-                                      PoolDimsL dm, int32_t *__restrict__ seg_cell) {
+                                      PoolDims dm, int32_t *__restrict__ seg_cell) {
   for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < n_seg; s += gridDim.x * blockDim.x)
-    seg_cell[s] = lift_cell_of(geom_feats, starts[(uint32_t)(seg_key[s] & 0xffffffffull)], n, dm);
+    seg_cell[s] = interval_cell(geom_feats, starts[(uint32_t)(seg_key[s] & 0xffffffffull)], n, dm);
 }
 
 // Shared memory of the column backward: fixed part + per staged segment.  Rows of ctx_s and g_s are padded to Q + 1
@@ -386,12 +366,12 @@ __global__ void __launch_bounds__(256)
 // ORIGINAL order (-1 for the filtered ones, which perm lists after the kept ones) ...
 __global__ void lift_point_cells_kernel(const int32_t *__restrict__ perm, const int32_t *__restrict__ geom_feats,
                                         const int32_t *__restrict__ starts, const int32_t *__restrict__ lengths,
-                                        int n, int n_total, int n_intervals, PoolDimsL dm,
+                                        int n, int n_total, int n_intervals, PoolDims dm,
                                         int32_t *__restrict__ point_cell) {
   const int lane = lane_id(), warps = (gridDim.x * blockDim.x) >> 5;
   for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n_intervals; i += warps) {   // warp per interval
     const int s0 = starts[i], len = lengths[i];
-    const int32_t c = lift_cell_of(geom_feats, s0, n, dm);
+    const int32_t c = interval_cell(geom_feats, s0, n, dm);
     for (int s = s0 + lane; s < s0 + len && s < n; s += 32) point_cell[perm[s]] = c;
   }
   for (int s = n + blockIdx.x * blockDim.x + threadIdx.x; s < n_total; s += gridDim.x * blockDim.x)
@@ -457,10 +437,6 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-static bool lift_channels_ok(int c) {
-  return c == 16 || c == 32 || c == 64 || c == 80 || c == 96 || c == 128 || c == 160 || c == 256;
-}
-
 struct LiftWs {
   int32_t *ival_of;
   unsigned long long *keys_a, *keys_b;
@@ -498,6 +474,32 @@ static size_t lift_prepare_layout(int n, void *ws, size_t ws_bytes, LiftWs *out)
   return a.off;
 }
 
+// Workspace of the column forward: one partial row per segment, then the cell of every interval
+struct LiftColumnsWs {
+  float *partial;
+  int32_t *cells;
+};
+static size_t lift_columns_layout(int n_segments, int n_intervals, int c, void *ws, LiftColumnsWs *out) {
+  Arena a(ws, 0);
+  LiftColumnsWs w;
+  w.partial = a.take<float>((size_t)n_segments * c);
+  w.cells = a.take<int32_t>((size_t)n_intervals);
+  if (out) *out = w;
+  return a.off;
+}
+
+// Workspace of both lift backwards: the cell of every segment (column form) or of every frustum point (pixel form),
+// room for at least one
+static size_t lift_bwd_layout(int items, void *ws, int32_t **cells) {
+  Arena a(ws, 0);
+  int32_t *p = a.take<int32_t>(items > 0 ? items : 1);
+  if (cells) *cells = p;
+  return a.off;
+}
+
+// the workspace queries of the column forward and both backwards report this much more than the calls require
+constexpr size_t kLiftQuerySlack = 256;
+
 }  // namespace bevb200
 
 using namespace bevb200;
@@ -528,11 +530,9 @@ int bevb200_bev_pool_lift_prepare(const int32_t *perm, const int32_t *interval_s
   }
   BEVB200_REQUIRE(perm && interval_starts, "null input");
   LiftWs w;
-  const size_t need = lift_prepare_layout(n_kept, workspace, workspace_bytes, &w);
-  if (workspace == nullptr || workspace_bytes < need) {
-    snprintf(g_last_error, sizeof(g_last_error), "bev_pool_lift_prepare: workspace too small (%zu < %zu)", workspace_bytes, need);
-    return BEVB200_EWORKSPACE;
-  }
+  if (const int rc = workspace_check("bev_pool_lift_prepare", workspace, workspace_bytes,
+                                     lift_prepare_layout(n_kept, workspace, workspace_bytes, &w)))
+    return rc;
   BEVB200_LAUNCH(lift_interval_ids_kernel, grid_for(n_intervals, 128), 128, 0, st, interval_starts, n_intervals, n_kept,
                  w.ival_of);
   BEVB200_LAUNCH(lift_keys_kernel, grid_for(n_kept, 256), 256, 0, st, perm, w.ival_of, n_kept, g, w.keys_a, w.vals_a);
@@ -578,61 +578,52 @@ int bevb200_bev_pool_lift_columns(int b, int d, int h, int w, int n, int c, int 
   BEVB200_REQUIRE(out != nullptr, "null out");
   BEVB200_REQUIRE(c % 4 == 0 && c <= 256, "channel count must be a multiple of 4, <= 256");
   BEVB200_REQUIRE((long long)b * d * h * w < (1ll << 31), "grid has too many cells");
-  cudaStream_t st = (cudaStream_t)stream;
   // with no segment the cells kernel does not run, so nothing would zero-fill the grid
-  const int zfill = (b * d == 1 && n > 0 && n_intervals > 0 && n_segments > 0) ? 1 : 0;
-  if (!zfill) BEVB200_CUDA(cudaMemsetAsync(out, 0, (size_t)b * d * h * w * c * sizeof(float), st));
-  if (n == 0 || n_intervals == 0 || n_segments == 0) return BEVB200_OK;
-  BEVB200_REQUIRE(depth && ctx && geom_feats && interval_starts && col_begin && seg_key && seg_mask && seg_slot &&
-                      interval_slot_begin, "null input");
-  BEVB200_REQUIRE(((uintptr_t)ctx % 16 == 0) && ((uintptr_t)out % 16 == 0), "ctx / out must be 16-byte aligned");
-  const size_t part_bytes = align_up((size_t)n_segments * c * sizeof(float));
-  const size_t need = part_bytes + align_up((size_t)n_intervals * sizeof(int32_t));
-  if (workspace == nullptr || workspace_bytes < need) {
-    snprintf(g_last_error, sizeof(g_last_error), "bev_pool_lift_columns: workspace too small (%zu < %zu)", workspace_bytes, need);
-    return BEVB200_EWORKSPACE;
-  }
-  float4 *partial = (float4 *)workspace;
-  int32_t *cells = (int32_t *)((char *)workspace + part_bytes);
-  PoolDimsL dm{b, d, h, w};
-  LiftGeom g{depth_bins, feature_h, feature_w, cameras * feature_w};
-  BEVB200_LAUNCH(lift_interval_cells_kernel, grid_for(n_intervals, 256), 256, 0, st, geom_feats, interval_starts, n,
-                 n_intervals, dm, cells);
+  const bool work = n > 0 && n_intervals > 0 && n_segments > 0;
   const size_t smem = (size_t)feature_h * c * sizeof(float) + (size_t)depth_bins * feature_h * sizeof(float) +
                       (size_t)depth_bins * sizeof(int);
-  BEVB200_REQUIRE(smem <= 200 * 1024, "image column does not fit in shared memory");
-  const int total_cells = b * d * h * w;
-#define LIFT_LAUNCH(Q)                                                                                               \
-  do {                                                                                                               \
-    BEVB200_CUDA(cudaFuncSetAttribute(lift_columns_kernel<Q>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    BEVB200_LAUNCH(lift_columns_kernel<Q>, g.ncols, 256, smem, st, depth, (const float4 *)ctx, g, col_begin,          \
-                   (const unsigned long long *)seg_key, (const unsigned long long *)seg_mask, seg_slot, partial);      \
-    BEVB200_LAUNCH(lift_cells_kernel<Q>, grid_for((long long)n_intervals * 32, 256, kNumSMs * 8), 256, 0, st,         \
-                   (const float4 *)partial, interval_slot_begin, cells, n_intervals, zfill, total_cells, (float4 *)out); \
-  } while (0)
-  switch (c) {
-    case 16: LIFT_LAUNCH(4); break;
-    case 32: LIFT_LAUNCH(8); break;
-    case 64: LIFT_LAUNCH(16); break;
-    case 80: LIFT_LAUNCH(20); break;
-    case 96: LIFT_LAUNCH(24); break;
-    case 128: LIFT_LAUNCH(32); break;
-    case 160: LIFT_LAUNCH(40); break;
-    case 256: LIFT_LAUNCH(64); break;
-    default: BEVB200_REQUIRE(false, "bev_pool_lift_columns: channel count not in {16,32,64,80,96,128,160,256}");
+  // every argument is checked before `out` is written: a refused call leaves it untouched
+  LiftColumnsWs ws;
+  if (work) {
+    BEVB200_REQUIRE(depth && ctx && geom_feats && interval_starts && col_begin && seg_key && seg_mask && seg_slot &&
+                        interval_slot_begin, "null input");
+    BEVB200_REQUIRE(((uintptr_t)ctx % 16 == 0) && ((uintptr_t)out % 16 == 0), "ctx / out must be 16-byte aligned");
+    if (const int rc = workspace_check("bev_pool_lift_columns", workspace, workspace_bytes,
+                                       lift_columns_layout(n_segments, n_intervals, c, workspace, &ws)))
+      return rc;
+    BEVB200_REQUIRE(smem <= 200 * 1024, "image column does not fit in shared memory");
+    BEVB200_REQUIRE(TunedWidths::has(c), "no tuned kernel for this channel count");
   }
-#undef LIFT_LAUNCH
-  return BEVB200_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int zfill = (b * d == 1 && work) ? 1 : 0;
+  if (!zfill) BEVB200_CUDA(cudaMemsetAsync(out, 0, (size_t)b * d * h * w * c * sizeof(float), st));
+  if (!work) return BEVB200_OK;
+  PoolDims dm{b, d, h, w};
+  LiftGeom g{depth_bins, feature_h, feature_w, cameras * feature_w};
+  BEVB200_LAUNCH(pool_interval_cells_kernel, grid_for(n_intervals, 256), 256, 0, st, geom_feats, interval_starts, n,
+                 n_intervals, dm, ws.cells);
+  const int total_cells = b * d * h * w;
+  return TunedWidths::dispatch(c, [&](auto q) {
+    constexpr int Q = decltype(q)::value;
+    BEVB200_CUDA(cudaFuncSetAttribute(lift_columns_kernel<Q>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    BEVB200_LAUNCH(lift_columns_kernel<Q>, g.ncols, 256, smem, st, depth, (const float4 *)ctx, g, col_begin,
+                   (const unsigned long long *)seg_key, (const unsigned long long *)seg_mask, seg_slot,
+                   (float4 *)ws.partial);
+    BEVB200_LAUNCH(lift_cells_kernel<Q>, grid_for((long long)n_intervals * 32, 256, kNumSMs * 8), 256, 0, st,
+                   (const float4 *)ws.partial, interval_slot_begin, ws.cells, n_intervals, zfill, total_cells,
+                   (float4 *)out);
+    return BEVB200_OK;
+  });
 }
 
 size_t bevb200_bev_pool_lift_columns_workspace_bytes(int n_segments, int n_intervals, int c) {
   if (n_segments < 0 || n_intervals < 0 || c <= 0) return 0;
-  return align_up((size_t)n_segments * c * sizeof(float)) + align_up((size_t)n_intervals * sizeof(int32_t)) + 256;
+  return lift_columns_layout(n_segments, n_intervals, c, nullptr, nullptr) + kLiftQuerySlack;
 }
 
 size_t bevb200_bev_pool_lift_columns_backward_workspace_bytes(int n_segments, int n_intervals, int c) {
-  if (n_segments < 0 || n_intervals < 0 || !lift_channels_ok(c)) return 0;
-  return align_up((size_t)(n_segments > 0 ? n_segments : 1) * sizeof(int32_t)) + 256;   // cell of every segment
+  if (n_segments < 0 || n_intervals < 0 || !TunedWidths::has(c)) return 0;
+  return lift_bwd_layout(n_segments, nullptr, nullptr) + kLiftQuerySlack;
 }
 
 int bevb200_bev_pool_lift_columns_backward(int b, int d, int h, int w, int n, int c, int n_intervals,
@@ -645,7 +636,7 @@ int bevb200_bev_pool_lift_columns_backward(int b, int d, int h, int w, int n, in
   BEVB200_REQUIRE(b > 0 && d > 0 && h > 0 && w > 0 && n >= 0 && n_intervals >= 0 && n_segments >= 0, "bad sizes");
   BEVB200_REQUIRE(cameras > 0 && depth_bins > 0 && feature_h > 0 && feature_w > 0, "bad lift dims");
   BEVB200_REQUIRE(feature_h <= 64, "feature height > 64: use bevb200_bev_pool_lift_backward");
-  BEVB200_REQUIRE(lift_channels_ok(c), "bev_pool_lift_columns_backward: channel count not in {16,32,64,80,96,128,160,256}");
+  BEVB200_REQUIRE(TunedWidths::has(c), "no tuned kernel for this channel count");
   BEVB200_REQUIRE((long long)b * d * h * w < (1ll << 31), "grid has too many cells");
   BEVB200_REQUIRE((long long)cameras * feature_w * depth_bins < (1ll << 31), "too many (column, depth) pairs");
   if (ddepth == nullptr && dctx == nullptr) return BEVB200_OK;
@@ -654,12 +645,10 @@ int bevb200_bev_pool_lift_columns_backward(int b, int d, int h, int w, int n, in
   BEVB200_REQUIRE(depth || !dctx, "dctx needs depth");
   BEVB200_REQUIRE(((uintptr_t)ctx % 16 == 0) && ((uintptr_t)dctx % 16 == 0) && ((uintptr_t)out_grad % 16 == 0),
                   "ctx / dctx / out_grad must be 16-byte aligned");
-  const size_t need = bevb200_bev_pool_lift_columns_backward_workspace_bytes(n_segments, n_intervals, c) - 256;
-  if (workspace == nullptr || workspace_bytes < need) {
-    snprintf(g_last_error, sizeof(g_last_error), "bev_pool_lift_columns_backward: workspace too small (%zu < %zu)",
-             workspace_bytes, need);
-    return BEVB200_EWORKSPACE;
-  }
+  int32_t *seg_cell;
+  if (const int rc = workspace_check("bev_pool_lift_columns_backward", workspace, workspace_bytes,
+                                     lift_bwd_layout(n_segments, workspace, &seg_cell)))
+    return rc;
   const int q = c / 4;
   const LiftBwdSmem sm = lift_bwd_smem(q, feature_h, depth_bins);
   // chunk size: all of a column's segments at once when that stays within ~100 KB (two CTAs per SM), else as many
@@ -672,36 +661,24 @@ int bevb200_bev_pool_lift_columns_backward(int b, int d, int h, int w, int n, in
   const size_t smem = sm.fixed + (size_t)smax * sm.per_seg;
   cudaStream_t st = (cudaStream_t)stream;
   LiftGeom g{depth_bins, feature_h, feature_w, cameras * feature_w};
-  int32_t *seg_cell = (int32_t *)workspace;
   if (n_segments > 0) {
-    PoolDimsL dm{b, d, h, w};
+    PoolDims dm{b, d, h, w};
     BEVB200_LAUNCH(lift_seg_cells_kernel, grid_for(n_segments, 256), 256, 0, st, (const unsigned long long *)seg_key,
                    n_segments, geom_feats, interval_starts, n, dm, seg_cell);
   }
-#define LIFT_BWD_LAUNCH(Q)                                                                                             \
-  do {                                                                                                                 \
-    BEVB200_CUDA(cudaFuncSetAttribute(lift_columns_bwd_kernel<Q>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    BEVB200_LAUNCH(lift_columns_bwd_kernel<Q>, g.ncols, 256, smem, st, (const float4 *)out_grad, depth,                \
-                   (const float4 *)ctx, g, col_begin, (const unsigned long long *)seg_key,                             \
-                   (const unsigned long long *)seg_mask, seg_cell, (int)smax, ddepth, (float4 *)dctx);                 \
-  } while (0)
-  switch (c) {
-    case 16: LIFT_BWD_LAUNCH(4); break;
-    case 32: LIFT_BWD_LAUNCH(8); break;
-    case 64: LIFT_BWD_LAUNCH(16); break;
-    case 80: LIFT_BWD_LAUNCH(20); break;
-    case 96: LIFT_BWD_LAUNCH(24); break;
-    case 128: LIFT_BWD_LAUNCH(32); break;
-    case 160: LIFT_BWD_LAUNCH(40); break;
-    case 256: LIFT_BWD_LAUNCH(64); break;
-  }
-#undef LIFT_BWD_LAUNCH
-  return BEVB200_OK;
+  return TunedWidths::dispatch(c, [&](auto q) {
+    constexpr int Q = decltype(q)::value;
+    BEVB200_CUDA(cudaFuncSetAttribute(lift_columns_bwd_kernel<Q>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    BEVB200_LAUNCH(lift_columns_bwd_kernel<Q>, g.ncols, 256, smem, st, (const float4 *)out_grad, depth,
+                   (const float4 *)ctx, g, col_begin, (const unsigned long long *)seg_key,
+                   (const unsigned long long *)seg_mask, seg_cell, (int)smax, ddepth, (float4 *)dctx);
+    return BEVB200_OK;
+  });
 }
 
 size_t bevb200_bev_pool_lift_backward_workspace_bytes(int n_total, int c) {
-  if (n_total < 0 || !lift_channels_ok(c)) return 0;
-  return align_up((size_t)(n_total > 0 ? n_total : 1) * sizeof(int32_t)) + 256;   // cell of every frustum point
+  if (n_total < 0 || !TunedWidths::has(c)) return 0;
+  return lift_bwd_layout(n_total, nullptr, nullptr) + kLiftQuerySlack;
 }
 
 int bevb200_bev_pool_lift_backward(int b, int d, int h, int w, int n, int n_total, int c, int n_intervals,
@@ -712,7 +689,7 @@ int bevb200_bev_pool_lift_backward(int b, int d, int h, int w, int n, int n_tota
   BEVB200_REQUIRE(b > 0 && d > 0 && h > 0 && w > 0 && n >= 0 && n_total >= n && n_intervals >= 0, "bad sizes");
   BEVB200_REQUIRE(depth_bins > 0 && pixels_per_camera > 0 && n_total % ((long long)depth_bins * pixels_per_camera) == 0,
                   "bad lift dims");
-  BEVB200_REQUIRE(lift_channels_ok(c), "bev_pool_lift_backward: channel count not in {16,32,64,80,96,128,160,256}");
+  BEVB200_REQUIRE(TunedWidths::has(c), "no tuned kernel for this channel count");
   BEVB200_REQUIRE((long long)b * d * h * w < (1ll << 31), "grid has too many cells");
   if (ddepth == nullptr && dctx == nullptr) return BEVB200_OK;
   BEVB200_REQUIRE(out_grad && perm && geom_feats && interval_starts && interval_lengths, "null input");
@@ -720,35 +697,22 @@ int bevb200_bev_pool_lift_backward(int b, int d, int h, int w, int n, int n_tota
   BEVB200_REQUIRE(depth || !dctx, "dctx needs depth");
   BEVB200_REQUIRE(((uintptr_t)ctx % 16 == 0) && ((uintptr_t)dctx % 16 == 0) && ((uintptr_t)out_grad % 16 == 0),
                   "ctx / dctx / out_grad must be 16-byte aligned");
-  const size_t need = bevb200_bev_pool_lift_backward_workspace_bytes(n_total, c) - 256;
-  if (workspace == nullptr || workspace_bytes < need) {
-    snprintf(g_last_error, sizeof(g_last_error), "bev_pool_lift_backward: workspace too small (%zu < %zu)",
-             workspace_bytes, need);
-    return BEVB200_EWORKSPACE;
-  }
+  int32_t *point_cell;
+  if (const int rc = workspace_check("bev_pool_lift_backward", workspace, workspace_bytes,
+                                     lift_bwd_layout(n_total, workspace, &point_cell)))
+    return rc;
   if (n_total == 0) return BEVB200_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  int32_t *point_cell = (int32_t *)workspace;
-  PoolDimsL dm{b, d, h, w};
+  PoolDims dm{b, d, h, w};
   BEVB200_LAUNCH(lift_point_cells_kernel, grid_for((long long)n_total, 256), 256, 0, st, perm, geom_feats,
                  interval_starts, interval_lengths, n, n_total, n_intervals, dm, point_cell);
   const int n_pixels = (int)(n_total / depth_bins);
   const int grid = grid_for((long long)n_pixels * 32, 256, kNumSMs * 16);
-#define LIFT_PIX_LAUNCH(Q)                                                                                             \
-  BEVB200_LAUNCH(lift_pixels_bwd_kernel<Q>, grid, 256, 0, st, (const float4 *)out_grad, depth, (const float4 *)ctx,   \
-                 point_cell, n_pixels, depth_bins, pixels_per_camera, ddepth, (float4 *)dctx)
-  switch (c) {
-    case 16: LIFT_PIX_LAUNCH(4); break;
-    case 32: LIFT_PIX_LAUNCH(8); break;
-    case 64: LIFT_PIX_LAUNCH(16); break;
-    case 80: LIFT_PIX_LAUNCH(20); break;
-    case 96: LIFT_PIX_LAUNCH(24); break;
-    case 128: LIFT_PIX_LAUNCH(32); break;
-    case 160: LIFT_PIX_LAUNCH(40); break;
-    case 256: LIFT_PIX_LAUNCH(64); break;
-  }
-#undef LIFT_PIX_LAUNCH
-  return BEVB200_OK;
+  return TunedWidths::dispatch(c, [&](auto q) {
+    BEVB200_LAUNCH(lift_pixels_bwd_kernel<decltype(q)::value>, grid, 256, 0, st, (const float4 *)out_grad, depth,
+                   (const float4 *)ctx, point_cell, n_pixels, depth_bins, pixels_per_camera, ddepth, (float4 *)dctx);
+    return BEVB200_OK;
+  });
 }
 
 }  // extern "C"

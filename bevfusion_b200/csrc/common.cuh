@@ -69,14 +69,6 @@ inline int grid_for(long long work_items, int block, int max_blocks = kNumSMs * 
 // ---- device helpers -------------------------------------------------------------------
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
 
-__device__ __forceinline__ float4 ldg_stream_f4(const float4 *p) {
-  // read-once streaming data: bypass L1 allocation
-  float4 v;
-  asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%4];"
-               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
-               : "l"(p));
-  return v;
-}
 __device__ __forceinline__ void stg_stream_f4(float4 *p, const float4 &v) {
   asm volatile("st.global.L1::no_allocate.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(v.x),
                "f"(v.y), "f"(v.z), "f"(v.w)

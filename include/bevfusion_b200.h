@@ -122,7 +122,9 @@ BEVB200_API int bevb200_bev_channels_first(const float *in, float *out, int batc
  *   original point index i -> pixel row (i / (depth_bins*pixels_per_camera)) * pixels_per_camera
  *                                       + i % pixels_per_camera
  * Tables as for bevb200_bev_pool_perm (from bevb200_bev_pool_prepare_geom).  Backward:
- * bevb200_bev_pool_lift_backward (any feature height) and bevb200_bev_pool_lift_columns_backward below. */
+ * bevb200_bev_pool_lift_backward (any feature height) and bevb200_bev_pool_lift_columns_backward below.
+ * workspace: bevb200_bev_pool_workspace_bytes(n, c).  A call refused with BEVB200_EINVAL or BEVB200_EWORKSPACE
+ * leaves `out` untouched. */
 BEVB200_API int bevb200_bev_pool_lift(int b, int d, int h, int w, int n, int c, int n_intervals,
                           const float *depth, const float *ctx, int depth_bins,
                           int pixels_per_camera, const int32_t *perm, const int32_t *geom_feats,
@@ -144,7 +146,8 @@ BEVB200_API int bevb200_bev_pool_lift(int b, int d, int h, int w, int n, int c, 
  *       Synchronises the stream once (it needs the segment count).
  *   bevb200_bev_pool_lift_columns   per frame: depth [cameras, depth_bins, feature_h, feature_w] fp32,
  *       ctx [cameras, feature_h, feature_w, c] fp32 -> out [b, d, h, w, c] (fully written).  n_segments as read
- *       back from the prepare call; workspace: bevb200_bev_pool_lift_columns_workspace_bytes(). */
+ *       back from the prepare call; workspace: bevb200_bev_pool_lift_columns_workspace_bytes().  A call refused
+ *       with BEVB200_EINVAL or BEVB200_EWORKSPACE leaves `out` untouched. */
 BEVB200_API size_t bevb200_bev_pool_lift_prepare_workspace_bytes(int n_kept);
 BEVB200_API int bevb200_bev_pool_lift_prepare(const int32_t *perm, const int32_t *interval_starts, int n_kept,
                                   int n_intervals, int cameras, int depth_bins, int feature_h, int feature_w,

@@ -6,8 +6,6 @@ Forward paths (bevpool.cu), each named by the branch it reaches and told apart b
   * tma1z   bevb200_bev_pool_perm, tuned C, B*D = 1: bevpool_fwd_tma_kernel<Q, 1>, empty cells zeroed by the warps
   * tma1m   bevb200_bev_pool_perm, tuned C, B*D > 1: the same kernel after a memset of the grid
   * generic either entry, C not tuned or x / out off 16-byte alignment: bevpool_fwd_generic_kernel
-  * v1      either entry under BEVB200_POOL_VARIANT=1 (read once per process, so in a subprocess):
-            bevpool_fwd_kernel + bevpool_fwd_fixup_kernel
 Backward: bevpool_bwd_kernel (tuned C) and bevpool_bwd_generic_kernel, through both entries.  Lift: the column form
 (bevpool_lift.cu) and the rows form (bevpool_fwd_tma_kernel<Q, 2>).
 
@@ -16,10 +14,6 @@ bit-identical; the Python wrappers must return the same bits.  Pooling must stay
 float64 sum of each cell's L rows, the lift within (L + 1) * 2^-24 * sum|d_r * ctx_r| (each product is rounded to
 fp32 first), so one dropped or doubled row fails in any cell.  Cells without an interval must be exactly +0.0.
 Each case prints its path and worst error as a fraction of the bound."""
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import torch
@@ -33,10 +27,7 @@ TUNED = (16, 32, 64, 80, 96, 128, 160, 256)
 U = 2.0 ** -24
 CANARY = 4096
 NUM_SMS = 132
-K_LONG_ROWS = 256          # v1 kernel: intervals longer than this are cut at 128-row chunk boundaries
-LAUNCHES = {"tma": 3, "generic": 1, "v1": 2}   # kernel launches of one forward call on each path
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
+LAUNCHES = {"tma": 3, "generic": 1}   # kernel launches of one forward call on each path
 
 
 # ---------------------------------------------------------------------------------------------------- tables
@@ -406,83 +397,6 @@ def test_forward_out_of_grid_rows(cuda, c, entry):
     check_forward(case, path, "%s %s C=%d out-of-grid" % (path, entry, c))
 
 
-# ---------------------------------------------------------------------------------------------------- v1 subprocess
-V1_CHILD = r"""
-import sys
-import numpy as np
-import torch
-sys.path[:0] = [sys.argv[1], sys.argv[2]]
-from bevfusion_b200 import _C
-_C.LIB_PATH = sys.argv[5]
-import test_bev_pool_dispatch_gpu as T
-dev = torch.device("cuda:0")
-src = np.load(sys.argv[3])
-res = {}
-for k in range(int(src["count"])):
-    case = T.case_from_arrays(src, k, dev)
-    res["out%d" % k] = T.pool_driver(case, launches=T.LAUNCHES["v1"]).cpu().numpy()
-np.savez(sys.argv[4], **res)
-"""
-
-
-def v1_cases(dev):
-    cases = []
-    for c in TUNED:
-        for entry in ("sorted", "perm"):
-            cases.append(("v1 %s C=%d long" % (entry, c),
-                          make_case(dev, c, 12000, "hot", use_perm=entry == "perm", seed=100 + c)))
-    for c in (16, 80, 256):
-        cases.append(("v1 sorted C=%d non-tiling" % c, make_case(dev, c, 20000, "hot", seed=7 + c, gaps=True)))
-    cases.append(("v1 sorted C=80 out-of-grid", make_case(dev, 80, 15000, "hot", seed=3, bad_cells=40, B=2)))
-    return cases
-
-
-def case_from_arrays(src, k, dev):
-    p = "c%d_" % k
-    case = Case.__new__(Case)
-    case.dims = tuple(int(v) for v in src[p + "dims"])
-    case.c, case.n = int(src[p + "x"].shape[1]), int(src[p + "n"])
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-    case.x, case.geom = t(src[p + "x"]), t(src[p + "geom"]).reshape(case.n, 4)
-    case.starts, case.lengths = t(src[p + "starts"]), t(src[p + "lengths"])
-    case.n_int = int(src[p + "starts"].size)
-    case.perm = t(src[p + "perm"]) if src[p + "perm"].size else None
-    case.n_total = int(src[p + "x"].shape[0])
-    return case
-
-
-@pytest.fixture(scope="module")
-def v1_results(cuda, tmp_path_factory):
-    """Every v1 case run once in a child process with BEVB200_POOL_VARIANT=1, loading the same library."""
-    cases = v1_cases(cuda)
-    d = tmp_path_factory.mktemp("v1")
-    arrays = {"count": np.array(len(cases))}
-    for k, (_, cs) in enumerate(cases):
-        p = "c%d_" % k
-        arrays.update({p + "dims": np.array(cs.dims), p + "x": cs.x_np, p + "n": np.array(cs.n), p + "geom": cs.geom_np,
-                       p + "starts": cs.starts_np, p + "lengths": cs.lengths_np,
-                       p + "perm": cs.perm_np if cs.perm_np is not None else np.zeros(0, np.int32)})
-    np.savez(d / "in.npz", **arrays)
-    env = dict(os.environ, BEVB200_POOL_VARIANT="1")
-    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [
-        "-c", V1_CHILD, HERE, ROOT, str(d / "in.npz"), str(d / "out.npz"), _C.LIB_PATH]
-    r = subprocess.run(cmd, env=env, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
-    out = np.load(d / "out.npz")
-    return [(name, cs, torch.from_numpy(out["out%d" % k]).to(cuda)) for k, (name, cs) in enumerate(cases)]
-
-
-def test_forward_v1_register_kernel(cuda, v1_results):
-    """bevpool_fwd_kernel at every tuned C through both entries, with intervals longer than kLongRows that cross
-    128-row chunks, a non-tiling table and out-of-grid rows."""
-    long_seen = False
-    for name, case, got in v1_results:
-        long_seen |= bool((case.lengths_np > K_LONG_ROWS).any() and
-                          ((case.starts_np[case.lengths_np > K_LONG_ROWS] % 128) != 0).any())
-        check_sums(got, *pool_reference(case), 0, name)
-    assert long_seen
-
-
 # ---------------------------------------------------------------------------------------------------- edges
 @pytest.mark.parametrize("entry", ["sorted", "perm"])
 @pytest.mark.parametrize("n,n_int", [(0, 0), (500, 0)])
@@ -640,7 +554,19 @@ def lift_reference(plan, depth, ctx):
     return ref, mag, cnt, cnt > 0
 
 
-def lift_rows_driver(plan, depth, ctx):
+def refused_once(fn, out):
+    """One call of fn() over a NaN prefill that must be refused: (return code, out, kernels launched)."""
+    out.fill_(float("nan"))
+    torch.cuda.synchronize()
+    _C.reset_launch_count()
+    rc = fn()
+    torch.cuda.synchronize()
+    return rc, out, _C.launch_count()
+
+
+def lift_rows_driver(plan, depth, ctx, ws_frac=None):
+    """bevb200_bev_pool_lift; with ws_frac, one call given that fraction of the queried workspace, expected to be
+    refused (see refused_once)."""
     L = _C.lib()
     t = plan.tables
     B, N, D, fH, fW = depth.shape
@@ -649,13 +575,17 @@ def lift_rows_driver(plan, depth, ctx):
     nbytes = L.bevb200_bev_pool_workspace_bytes(t.n_kept, c)
     ws, pattern = workspace(nbytes, dev)
     out = torch.empty(*t.dims, c, device=dev)
+    size = nbytes if ws_frac is None else int(nbytes * ws_frac)
     fn = lambda: L.bevb200_bev_pool_lift(*t.dims, t.n_kept, c, t.n_intervals, _C.ptr(depth), _C.ptr(ctx), D, fH * fW,
                                          _C.ptr(t.perm), _C.ptr(t.geom), _C.ptr(t.starts), _C.ptr(t.lengths),
-                                         _C.ptr(out), _C.ptr(ws), nbytes, _C.current_stream(dev))
+                                         _C.ptr(out), _C.ptr(ws), size, _C.current_stream(dev))
+    if ws_frac is not None:
+        return refused_once(fn, out)
     return run_twice(fn, out, ws, pattern, nbytes, launches=3)
 
 
-def lift_columns_driver(plan, depth, ctx, n_seg=None):
+def lift_columns_driver(plan, depth, ctx, n_seg=None, ws_frac=None):
+    """bevb200_bev_pool_lift_columns; ws_frac as for lift_rows_driver."""
     L = _C.lib()
     t = plan.tables
     B, N, D, fH, fW = depth.shape
@@ -666,10 +596,13 @@ def lift_columns_driver(plan, depth, ctx, n_seg=None):
     nbytes = L.bevb200_bev_pool_lift_columns_workspace_bytes(ns, t.n_intervals, c)
     ws, pattern = workspace(nbytes, dev)
     out = torch.empty(*t.dims, c, device=dev)
+    size = nbytes if ws_frac is None else int(nbytes * ws_frac)
     fn = lambda: L.bevb200_bev_pool_lift_columns(
         *t.dims, t.n_kept, c, t.n_intervals, _C.ptr(depth), _C.ptr(ctx), B * N, D, fH, fW, _C.ptr(t.geom),
         _C.ptr(t.starts), _C.ptr(col_begin), _C.ptr(seg_key), _C.ptr(seg_mask), _C.ptr(seg_slot), _C.ptr(ival_begin),
-        ns, _C.ptr(out), _C.ptr(ws), nbytes, _C.current_stream(dev))
+        ns, _C.ptr(out), _C.ptr(ws), size, _C.current_stream(dev))
+    if ws_frac is not None:
+        return refused_once(fn, out)
     return run_twice(fn, out, ws, pattern, nbytes, launches=3 if ns else 0)
 
 
@@ -714,6 +647,30 @@ def test_lift_untuned_width_is_refused(cuda, monkeypatch):
     monkeypatch.setenv("BEVB200_LIFT_VARIANT", "rows")
     with pytest.raises(_C.BevB200Error):
         plan.lift_pool(depth, ctx)
+
+
+LIFT_DRIVERS = {"rows": lift_rows_driver, "columns": lift_columns_driver}
+
+
+@pytest.mark.parametrize("form", ["rows", "columns"])
+@pytest.mark.parametrize("fault,code", [("untuned", EINVAL), ("misaligned", EINVAL), ("workspace", EWORKSPACE)])
+def test_lift_refused_call_leaves_out_untouched(cuda, form, fault, code):
+    """B = 2 (the grid is zeroed by a memset before the kernels run): a call refused for an untuned C, a ctx off
+    16-byte alignment or half the queried workspace returns its error code before anything writes `out`."""
+    plan, depth, ctx = lift_inputs(cuda, "b2", 20 if fault == "untuned" else 80, seed=0)
+    if fault == "misaligned":
+        ctx = misalign(ctx)
+    rc, out, _ = LIFT_DRIVERS[form](plan, depth, ctx, ws_frac=0.5 if fault == "workspace" else 1.0)
+    assert rc == code, _C.lib().bevb200_last_error()
+    assert bool(torch.isnan(out).all()), "out was written by a refused call"
+
+
+def test_lift_columns_untuned_width_launches_nothing(cuda):
+    """B = 1 (the kernels zero-fill the grid themselves): an untuned C is refused before the first launch."""
+    plan, depth, ctx = lift_inputs(cuda, "b1", 20, seed=0)
+    rc, out, launches = lift_columns_driver(plan, depth, ctx, ws_frac=1.0)
+    assert rc == EINVAL and launches == 0
+    assert bool(torch.isnan(out).all()), "out was written by a refused call"
 
 
 def test_lift_columns_without_segments_zero_the_grid(cuda):
