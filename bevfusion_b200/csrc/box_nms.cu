@@ -3,11 +3,9 @@
 //
 // Boxes are [x1, y1, x2, y2, ry] fp32.  A box is the axis-aligned extent turned by ry about its centre:
 //   x' = (x - cx) cos r + (y - cy) sin r + cx,   y' = -(x - cx) sin r + (y - cy) cos r + cy.
-// The overlap of two boxes is the area of their convex intersection polygon, whose vertices are the strict
-// edge crossings (both segments cut strictly) and the corners of each box that lie inside the other one
-// within 1e-5 (tested in the other box's own frame).  The vertices are ordered by pseudo-angle about their
-// mean and summed as a triangle fan.  iou = overlap / max(sa + sb - overlap, 1e-8), sa and sb the unrotated
-// extents' areas; a pair is suppressed when iou > thresh.
+// The overlap of two boxes is the area of one clipped by the other, in the other's own frame (rot_overlap.cuh).
+// iou = overlap / max(sa + sb - overlap, 1e-8), sa and sb the unrotated extents' areas; a pair is suppressed when
+// iou > thresh.
 //
 // NMS runs over S segments of up to Nmax boxes each (device-side counts), sorted by descending score:
 //   nms_mask_kernel      bit j of mask row i (j > i) = pair (i, j) is suppressed; upper-triangle 64x64 tiles only
@@ -29,10 +27,13 @@ constexpr float kIouEps = 1e-8f;
 constexpr int kDenseTile = 16;
 constexpr int kMaskSplit = 8;                                // lanes per mask row
 
-__device__ __forceinline__ float rot_iou(const float *pa, const float *pb) {
+__device__ __forceinline__ float iou_of_overlap(const float *pa, const float *pb, float ov) {
   const float sa = __fmul_rn(pa[2] - pa[0], pa[3] - pa[1]), sb = __fmul_rn(pb[2] - pb[0], pb[3] - pb[1]);
-  const float ov = rot_overlap(load_rot(pa), load_rot(pb));
   return ov / fmaxf(sa + sb - ov, kIouEps);
+}
+
+__device__ __forceinline__ float rot_iou(const float *pa, const float *pb) {
+  return iou_of_overlap(pa, pb, rot_overlap(load_rot(pa), load_rot(pb)));
 }
 
 // Axis-aligned IoU of nms_normal (iou3d_kernel.cu:335-343): the angle is ignored.
@@ -55,13 +56,9 @@ __global__ void __launch_bounds__(kDenseTile *kDenseTile)
                            float *__restrict__ out, bool iou) {
   const int i = blockIdx.y * kDenseTile + threadIdx.y, j = blockIdx.x * kDenseTile + threadIdx.x;
   if (i >= na || j >= nb) return;
-  float r;
-  if (iou) {
-    r = rot_iou(a + 5ll * i, b + 5ll * j);
-  } else {
-    r = rot_overlap(load_rot(a + 5ll * i), load_rot(b + 5ll * j));
-  }
-  out[(long long)i * nb + j] = r;
+  const float *pa = a + 5ll * i, *pb = b + 5ll * j;
+  const float ov = rot_overlap(load_rot(pa), load_rot(pb));
+  out[(long long)i * nb + j] = iou ? iou_of_overlap(pa, pb, ov) : ov;
 }
 
 __device__ __forceinline__ int segment_count(const int32_t *counts, int s, int nmax) {

@@ -4,6 +4,7 @@
                                         rotated rectangle clipped by the other (Sutherland-Hodgman)
     iou_matrix(A, B)                    [M, N] of the above (pairs whose circumscribed circles are apart
                                         are 0 without clipping)
+    iou3d_matrix(A, B)                  [M, N] 3D IoU of (x, y, z, dx, dy, dz, yaw) boxes, z the bottom
     greedy(iou, thresh)                 greedy keep list of score-sorted boxes given their IoU matrix
     nms(boxes, scores, thresh, pre, post)   nms_gpu's result (indices into boxes)
     circle_nms(dets, thresh, post)      circle NMS, squared distance <= thresh
@@ -64,6 +65,8 @@ def overlap_bev(a, b):
     a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
     if not (np.isfinite(a).all() and np.isfinite(b).all()) or _apart(a, b):
         return 0.0
+    if (a[2] - a[0]) * (a[3] - a[1]) == 0 or (b[2] - b[0]) * (b[3] - b[1]) == 0:
+        return 0.0                                  # exactly: clipping noise over a union of 1e-8 would not be
     poly = corners(a)
     cb = corners(b)
     for k in range(4):
@@ -97,6 +100,30 @@ def iou_matrix(A, B, overlap=False):
     for i, j in zip(*np.nonzero(cand)):
         out[i, j] = fn(A[i], B[j])
     return out
+
+
+def xywhr2xyxyr(boxes):
+    """[N, 7+] (x, y, z, dx, dy, dz, yaw, ...) boxes -> [N, 5] BEV [x1, y1, x2, y2, ry], in the boxes' own dtype
+    (LiDARInstance3DBoxes.bev, then xywhr2xyxyr as torch computes it)."""
+    b = np.asarray(boxes)
+    hx, hy = b[:, 3] / 2, b[:, 4] / 2
+    return np.stack([b[:, 0] - hx, b[:, 1] - hy, b[:, 0] + hx, b[:, 1] + hy, b[:, 6]], 1)
+
+
+def iou3d_matrix(A, B):
+    """[M, N] 3D IoU of (x, y, z, dx, dy, dz, yaw) boxes with z the bottom, as BaseInstance3DBoxes.overlaps
+    (mode iou) defines it: the BEV overlap of the xyxyr boxes times the overlap of [z, z + dz], over
+    max(va + vb - overlap, 1e-8).  The xyxyr corners and the tops z + dz are formed in the boxes' own dtype, as the
+    reference's torch code forms them; everything after that is float64."""
+    A, B = np.asarray(A).reshape(-1, np.shape(A)[-1]), np.asarray(B).reshape(-1, np.shape(B)[-1])
+    bev = iou_matrix(xywhr2xyxyr(A), xywhr2xyxyr(B), overlap=True)
+    top_a, top_b = (A[:, 2] + A[:, 5]).astype(np.float64), (B[:, 2] + B[:, 5]).astype(np.float64)
+    A, B = A.astype(np.float64), B.astype(np.float64)
+    h = np.minimum(top_a[:, None], top_b[None, :]) - np.maximum(A[:, None, 2], B[None, :, 2])
+    ov = bev * np.where(h < 0, 0.0, h)                          # clamp(min=0); NaN stays
+    va, vb = A[:, 3] * A[:, 4] * A[:, 5], B[:, 3] * B[:, 4] * B[:, 5]
+    u = va[:, None] + vb[None, :] - ov
+    return ov / np.where(u < 1e-8, 1e-8, u)
 
 
 def greedy(iou, thresh):

@@ -12,6 +12,7 @@ from scipy.optimize import linear_sum_assignment
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import lsap_oracle  # noqa: E402
+import nms_oracle as O  # noqa: E402
 from conftest import ref_module  # noqa: E402
 from test_transfusion_assign_cpu import large_cases, lsap_cases  # noqa: E402
 
@@ -22,7 +23,11 @@ from bevfusion_b200.head_targets import pad_gt  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 CFG, CODER = S.TRANSFUSION_TRAIN_CFG, S.TRANSFUSION_CODER
-COST_TOL = 1e-6   # largest |native cost - torch restatement| allowed (costs are O(1))
+# Largest |native cost - restatement| allowed (costs are O(1)), and largest |ious - restatement|.  The
+# restatement's IoU3D is float64, so both bound the kernel's fp32 overlap error (measured on an H100: 9e-8 and
+# 4e-7 on these batches).
+COST_TOL = 1e-6
+IOU_TOL = 1e-6
 
 
 def batch_solve(mats, dev, R=None, C=None):
@@ -99,7 +104,12 @@ def ref_decode(pred, b):
     return torch.cat([c, h, d, torch.atan2(r[0:1], r[1:2])], 0).T
 
 
-def ref_overlaps(a, b, bev_fn):
+def ref_overlaps(a, b, bev_fn=None):
+    """BaseInstance3DBoxes.overlaps(a, b), mode iou.  By default in float64 (nms_oracle.iou3d_matrix, on the fp32
+    boxes), so that an error of this package's overlap shows up on one side only; with bev_fn, a BEV overlap op on
+    xyxyr boxes, in fp32 torch over that op, as the reference computes it."""
+    if bev_fn is None:
+        return torch.from_numpy(O.iou3d_matrix(a.detach().cpu().numpy(), b.detach().cpu().numpy())).to(a.device)
     bev = bev_fn(iou3d.xywhr2xyxyr(a[:, [0, 1, 3, 4, 6]]).contiguous(),
                  iou3d.xywhr2xyxyr(b[:, [0, 1, 3, 4, 6]]).contiguous())
     top = torch.min((a[:, 2] + a[:, 5]).view(-1, 1), (b[:, 2] + b[:, 5]).view(1, -1))
@@ -109,8 +119,9 @@ def ref_overlaps(a, b, bev_fn):
     return ov / torch.clamp(va + vb - ov, min=1e-8)
 
 
-def ref_cost(boxes, logits, gt, gl, bev_fn=iou3d.boxes_overlap_bev):
-    """HungarianAssigner3D.assign's cost (hungarian_assigner.py:100-113, mmdet FocalLossCost) on CUDA tensors."""
+def ref_cost(boxes, logits, gt, gl, bev_fn=None):
+    """HungarianAssigner3D.assign's cost (hungarian_assigner.py:100-113, mmdet FocalLossCost) on CUDA tensors, the
+    IoU3D term from ref_overlaps (float64 unless bev_fn is given) rounded to fp32.  Returns (cost, iou)."""
     p = logits.T.sigmoid()
     neg = -(1 - p + 1e-12).log() * (1 - 0.25) * p.pow(2.0)
     pos = -(p + 1e-12).log() * 0.25 * (1 - p).pow(2.0)
@@ -119,7 +130,7 @@ def ref_cost(boxes, logits, gt, gl, bev_fn=iou3d.boxes_overlap_bev):
     span = boxes.new(CFG["point_cloud_range"][3:5]) - boxes.new(CFG["point_cloud_range"][0:2])
     reg = torch.cdist((boxes[:, :2] - start) / span, (gt[:, :2] - start) / span, p=1) * 0.25
     iou = ref_overlaps(boxes, gt, bev_fn)
-    return cls + reg + (-iou) * 0.25, iou
+    return cls + reg + (-iou.float()) * 0.25, iou
 
 
 def ref_encode(g):
@@ -152,7 +163,7 @@ def ref_get_targets(gts, labels, pred, P):
             r, c = linear_sum_assignment(cost.detach().cpu())
             r, c = torch.from_numpy(r).to(gt.device), torch.from_numpy(c).to(gt.device)
             gt_inds[r + layer * P] = c + 1
-            ious[r + layer * P] = torch.clamp(iou[r, c], 0, 1)
+            ious[r + layer * P] = torch.clamp(iou[r, c], 0, 1).float()
         pos = torch.nonzero(gt_inds > 0).squeeze(1)
         lab = torch.full((N,), 10, dtype=torch.long, device=gt.device)
         bt = torch.zeros((N, 10), device=gt.device)
@@ -194,14 +205,14 @@ def test_end_to_end_against_reference_loop(cuda, B, L):
     ref = ref_get_targets(gts, labels, pred, 200)
     got_inds = ex["gt_inds"].cpu().numpy()
     want_inds = torch.stack(ref["gt_inds"]).cpu().numpy()
-    differing = 0
+    differing, worst = 0, 0.0
     for s in range(B * L):
         b, layer = divmod(s, L)
         G = len(gts[b])
         cost = ex["cost"][s, :, :G]
         rc = ref["cost"][s]
         assert torch.isfinite(cost).all()
-        assert (cost - rc).abs().max().item() <= COST_TOL
+        worst = max(worst, (cost - rc).abs().max().item())
         # the solver in the pipeline: scipy on the call's own matrix gives the call's assignment
         r, c = linear_sum_assignment(cost.cpu().numpy())
         sl = slice(layer * 200, (layer + 1) * 200)
@@ -213,15 +224,18 @@ def test_end_to_end_against_reference_loop(cuda, B, L):
             c64 = rc.double().cpu().numpy()
             tot = lambda ind: sum(c64[p, g - 1] for p, g in enumerate(ind) if g > 0)   # noqa: E731
             assert abs(tot(got_inds[b, sl]) - tot(want_inds[b, sl])) <= COST_TOL * G
-    print("segments whose assignment differs from the reference's at equal cost: %d of %d" % (differing, B * L))
     same = torch.from_numpy((got_inds == want_inds).all(1)).to(cuda)
+    ious_err = (out[4][same] - torch.stack(ref["ious"])[same]).abs().max().item()
+    print("segments whose assignment differs from the reference's at equal cost: %d of %d; largest |cost - "
+          "restatement| %.3g, |ious - restatement| %.3g" % (differing, B * L, worst, ious_err))
+    assert worst <= COST_TOL
     for k in ("labels", "label_weights", "bbox_weights"):
         assert torch.equal(out[["labels", "label_weights", "bbox_targets", "bbox_weights"].index(k)][same],
                            torch.stack(ref[k])[same]), k
     assert out[5].cpu().tolist() == ref["num_pos"]
     assert ulp_diff(out[2][same], torch.stack(ref["bbox_targets"])[same]).max() <= 2
-    assert (out[4][same] - torch.stack(ref["ious"])[same]).abs().max().item() <= 1e-6
-    assert np.abs(out[6].cpu().numpy() - np.array(ref["mean_iou"]))[same.cpu().numpy()].max(initial=0) <= 1e-6
+    assert ious_err <= IOU_TOL
+    assert np.abs(out[6].cpu().numpy() - np.array(ref["mean_iou"]))[same.cpu().numpy()].max(initial=0) <= IOU_TOL
     assert (out[7] == 0).all()
 
 
@@ -397,6 +411,7 @@ def test_hungarian_assigner_mirror(cuda):
     assert np.array_equal(res.labels.cpu().numpy(), lab)
     mo = np.zeros(200, np.float32)
     mo[r] = iou.cpu().numpy()[r, c]
-    assert np.abs(res.max_overlaps.cpu().numpy() - mo).max() <= 1e-6
+    print("largest |max_overlaps - float64 restatement|: %.3g" % np.abs(res.max_overlaps.cpu().numpy() - mo).max())
+    assert np.abs(res.max_overlaps.cpu().numpy() - mo).max() <= IOU_TOL
     empty = TA.HungarianAssigner3D().assign(boxes, gts[0][:0], labels[0][:0], pred["heatmap"][0:1], CFG)
     assert empty.max_overlaps is None and (empty.gt_inds == 0).all()
