@@ -86,6 +86,9 @@ _SIGNATURES = {
                                    + [c_int] * 2 + [ctypes.c_double] * 10 + [_P] * 13 + [c_size_t, _P]),
     "bevb200_transfusion_proposals_workspace_bytes": (c_size_t, [c_int] * 4),
     "bevb200_transfusion_proposals": (c_int, [_P] + [c_int] * 9 + [_P] * 4 + [c_size_t, _P]),
+    "bevb200_centerhead_decode_workspace_bytes": (c_size_t, [c_int, c_int, _P, c_int, c_int]),
+    "bevb200_centerhead_decode": (c_int, [_P] * 7 + [c_int] * 7 + [ctypes.c_double] * 5 + [_P, c_int, ctypes.c_double]
+                                  + [_P] * 6 + [c_size_t, _P]),
     "bevb200_rulebook_workspace_bytes": (c_size_t, [c_int, c_int, _P]),
     "bevb200_rulebook_prepare": (c_int, [_P, c_int, c_int] + [_P] * 6 + [c_int, _P, _P, c_size_t, _P]),
     "bevb200_rulebook_fill": (c_int, [_P, c_int, c_int] + [_P] * 6 + [c_int, c_int, _P, _P, _P,

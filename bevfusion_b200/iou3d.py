@@ -9,8 +9,10 @@ and of core/post_processing/box3d_nms.py:
 
 Batched forms with no host synchronisation (CUDA-graph capturable):
     nms_batched(boxes, scores, counts, mode, thresh, pre_max_size, post_max_size) -> (keep, keep_count)
-    centerhead_nms(decoded, task_id, nms_type, test_cfg, nms_scale, num_classes=...)
+    centerhead_nms_batched(boxes, scores, labels, counts, task_id, nms_type, test_cfg, nms_scale, num_classes=...)
                                               the NMS step of CenterHead.get_bboxes for one task over the batch
+The same step on the coder's per-sample lists, with one read of the kept counts:
+    centerhead_nms(decoded, task_id, nms_type, test_cfg, nms_scale, num_classes=...)
 
 Boxes are [x1, y1, x2, y2, ry] fp32 (xywhr2xyxyr form).  The mirrors sort with the reference's own
 `scores.sort(0, descending=True)`, so equal scores order as in the reference on the same torch.  circle_nms
@@ -25,7 +27,7 @@ import torch
 from . import _C
 
 __all__ = ["boxes_iou_bev", "boxes_overlap_bev", "nms_gpu", "nms_normal_gpu", "circle_nms", "nms_batched",
-           "centerhead_nms", "xywhr2xyxyr", "MODES"]
+           "centerhead_nms", "centerhead_nms_batched", "xywhr2xyxyr", "MODES"]
 
 MODES = {"rotate": 0, "normal": 1, "circle": 2}   # BEVB200_NMS_ROTATE / _NORMAL / _CIRCLE
 MAX_BOXES = 65536                                  # BEVB200_NMS_MAX_BOXES
@@ -148,20 +150,14 @@ def _pad(tensors, fill=0):
     return out
 
 
-def centerhead_nms(decoded, task_id, nms_type, test_cfg, nms_scale=None, num_classes=None):
-    """The NMS step of CenterHead.get_bboxes for one task (models/heads/bbox/centerpoint.py:710-737 for
-    "circle", get_task_detections :768-884 otherwise) over every sample of the batch in one nms_batched call.
-
-    decoded: list over samples of dicts(bboxes [n, code_size], scores [n], labels [n]) from
-    bbox_coder.decode; test_cfg: the head's test_cfg (score_threshold, nms_thr, pre_max_size, post_max_size,
-    post_center_limit_range, min_radius); nms_scale: the BEV size scales of this task, a list over its
-    classes or one number for all (None, as when the config sets no nms_scale: 1.0); num_classes: the task's
-    class count, `self.num_classes[task_id]` (num_class_with_bg, :670; with one class every label becomes 0,
-    :804-811).  num_classes may be left out only when nms_scale is a per-class list, which get_bboxes builds
-    with one entry per class (:650-666); then it is the list's length.  Without either the class count is
-    unknown and ValueError is raised, rather than guessing one class and relabelling every box as class 0.
-    Returns the reference's list of per-sample dict(bboxes, scores, labels).  The kept counts are read back
-    once, to split the result per sample.  Lists are sorted stably (see nms_batched)."""
+def centerhead_nms_batched(boxes, scores, labels, counts, task_id, nms_type, test_cfg, nms_scale=None,
+                           num_classes=None):
+    """centerhead_nms on padded lists, without host synchronisation (CUDA-graph capturable): boxes
+    [B, N, code_size], scores [B, N], labels [B, N] (any dtype) and counts [B] int (sample b's detections are rows
+    [0, counts[b]); the other rows are ignored whatever they hold); the remaining arguments as centerhead_nms.
+    Returns (bboxes [B, P, code_size], scores [B, P], labels [B, P], lengths [B] int64), P = post_max_size: sample
+    b's kept detections are rows [0, lengths[b]) in the order centerhead_nms gives them, zeros after them.  Labels
+    keep their dtype for "circle" and are int64 otherwise (all 0 with one class), as in the reference."""
     if num_classes is None:
         if not isinstance(nms_scale, (list, tuple)):
             raise ValueError("centerhead_nms needs num_classes (self.num_classes[task_id]) unless nms_scale is a "
@@ -174,32 +170,27 @@ def centerhead_nms(decoded, task_id, nms_type, test_cfg, nms_scale=None, num_cla
         nms_scale = [1.0] * int(num_classes)
     elif not isinstance(nms_scale, (list, tuple)):
         nms_scale = [float(nms_scale)] * int(num_classes)
-    boxes = [d["bboxes"] for d in decoded]
-    scores = [d["scores"] for d in decoded]
-    labels = [d["labels"] for d in decoded]
-    for b in boxes:
-        _C.require_cuda(b, "bboxes", contiguous=False)
-    dev, B = boxes[0].device, len(decoded)
-    counts = torch.tensor([b.shape[0] for b in boxes], dtype=torch.int32).to(dev, non_blocking=True)
-    pb, ps = _pad(boxes), _pad(scores, float("-inf"))
+    for t, name in ((boxes, "bboxes"), (scores, "scores"), (labels, "labels"), (counts, "counts")):
+        _C.require_cuda(t, name, contiguous=False)
+    pb, ps, dev = boxes, scores, boxes.device
     post_max = int(test_cfg["post_max_size"])
     if nms_type == "circle":
         keep, kc = nms_batched(pb, ps, counts, "circle", test_cfg["min_radius"][task_id], None, post_max)
-        pl = _pad(labels)
+        pl = labels
         valid = torch.arange(keep.shape[1], device=dev)[None, :] < kc[:, None].long()
     else:
-        pl = _pad([l.long() if num_classes > 1 else torch.zeros_like(l, dtype=torch.long) for l in labels])
+        pl = labels.long() if num_classes > 1 else torch.zeros_like(labels, dtype=torch.long)
         live = torch.arange(pb.shape[1], device=dev)[None, :] < counts[:, None].long()
         thr = float(test_cfg["score_threshold"])
         if thr > 0.0:
-            live &= ps >= torch.tensor([thr], device=dev).type_as(ps)
+            live &= ps >= thr                              # compared in the scores' dtype, as the reference's tensor
         # the rows above the score threshold, moved to the front of each list in their order
         perm = torch.argsort((~live).to(torch.int8), dim=1, stable=True)
-        bev = pb[..., [0, 1, 3, 4, 6]]                     # LiDARInstance3DBoxes.bev
-        table = torch.tensor(list(nms_scale) + [1.0], dtype=bev.dtype, device=dev)
-        k = len(nms_scale)                                 # labels outside 0..k-1 keep their size, as in :829-832
-        cls = torch.where((pl >= 0) & (pl < k), pl, torch.full_like(pl, k))
-        bev[..., 2:4] *= table[cls][..., None]
+        bev = torch.stack([pb[..., c] for c in (0, 1, 3, 4, 6)], -1)   # LiDARInstance3DBoxes.bev
+        scale = torch.ones_like(ps)                        # labels outside the list keep their size, as in :829-832
+        for cls, factor in enumerate(nms_scale):           # built from scalars: no host-to-device copy
+            scale = torch.where(pl == cls, float(factor), scale)
+        bev[..., 2:4] *= scale[..., None]
         keep, kc = nms_batched(xywhr2xyxyr(bev).gather(1, perm[..., None].expand(-1, -1, 5)), ps.gather(1, perm),
                                live.sum(1, dtype=torch.int32), "rotate", test_cfg["nms_thr"],
                                test_cfg["pre_max_size"], post_max)
@@ -207,18 +198,36 @@ def centerhead_nms(decoded, task_id, nms_type, test_cfg, nms_scale=None, num_cla
         valid = torch.arange(keep.shape[1], device=dev)[None, :] < kc[:, None].long()
         rng = test_cfg["post_center_limit_range"]
         if len(rng) > 0:
-            rng = torch.tensor(rng, dtype=pb.dtype, device=dev)
-            ctr = pb.gather(1, keep[..., None].expand(-1, -1, pb.shape[2]))[..., :3]
-            valid &= (ctr >= rng[:3]).all(-1) & (ctr <= rng[3:]).all(-1)
-    # compact the valid slots of every row to its front, keeping their order; one read of the lengths
+            ctr = pb.gather(1, keep[..., None].expand(-1, -1, pb.shape[2]))
+            for d in range(3):                             # limits compared in the boxes' dtype, as a tensor's would be
+                valid &= (ctr[..., d] >= float(rng[d])) & (ctr[..., d] <= float(rng[3 + d]))
+    # compact the valid slots of every row to its front, keeping their order
     slot = torch.argsort((~valid).to(torch.int8), dim=1, stable=True)
     idx = keep.gather(1, slot).clamp(min=0)
-    lengths = valid.sum(1).tolist()
-    out = []
-    for i in range(B):
-        sel = idx[i, :lengths[i]]
-        if nms_type == "circle":
-            out.append(dict(bboxes=boxes[i][sel], scores=scores[i][sel], labels=labels[i][sel]))
-        else:
-            out.append(dict(bboxes=pb[i, sel], scores=ps[i, sel], labels=pl[i, sel]))
-    return out
+    lengths = valid.sum(1)
+    pad = torch.arange(idx.shape[1], device=dev)[None, :] >= lengths[:, None]
+    return (pb.gather(1, idx[..., None].expand(-1, -1, pb.shape[2])).masked_fill(pad[..., None], 0),
+            ps.gather(1, idx).masked_fill(pad, 0), pl.gather(1, idx).masked_fill(pad, 0), lengths)
+
+
+def centerhead_nms(decoded, task_id, nms_type, test_cfg, nms_scale=None, num_classes=None):
+    """The NMS step of CenterHead.get_bboxes for one task (models/heads/bbox/centerpoint.py:710-737 for
+    "circle", get_task_detections :768-884 otherwise) over every sample of the batch in one nms_batched call.
+
+    decoded: list over samples of dicts(bboxes [n, code_size], scores [n], labels [n]) from
+    bbox_coder.decode; test_cfg: the head's test_cfg (score_threshold, nms_thr, pre_max_size, post_max_size,
+    post_center_limit_range, min_radius); nms_scale: the BEV size scales of this task, a list over its
+    classes or one number for all (None, as when the config sets no nms_scale: 1.0); num_classes: the task's
+    class count, `self.num_classes[task_id]` (num_class_with_bg, :670; with one class every label becomes 0,
+    :804-811).  num_classes may be left out only when nms_scale is a per-class list, which get_bboxes builds
+    with one entry per class (:650-666); then it is the list's length.  Without either the class count is
+    unknown and ValueError is raised, rather than guessing one class and relabelling every box as class 0.
+    Returns the reference's list of per-sample dict(bboxes, scores, labels).  The lists are padded to one
+    length for centerhead_nms_batched, and the kept counts are read back once, to split the result per sample.
+    Lists are sorted stably (see nms_batched)."""
+    boxes = [d["bboxes"] for d in decoded]
+    counts = torch.tensor([b.shape[0] for b in boxes], dtype=torch.int32).to(boxes[0].device, non_blocking=True)
+    pb, ps, pl, lengths = centerhead_nms_batched(
+        _pad(boxes), _pad([d["scores"] for d in decoded], float("-inf")), _pad([d["labels"] for d in decoded]),
+        counts, task_id, nms_type, test_cfg, nms_scale, num_classes)
+    return [dict(bboxes=pb[i, :n], scores=ps[i, :n], labels=pl[i, :n]) for i, n in enumerate(lengths.tolist())]

@@ -357,3 +357,65 @@ def centerhead_detections(seed=0, batch=1, max_num=500):
                              labels=torch.from_numpy(np.array(labels)[pick].astype(np.int64))))
         out.append(task)
     return out
+
+
+def centerhead_coder_cfg(height=128, width=128, extent=54.0, max_num=500, score_threshold=0.1):
+    """The CenterPointBBoxCoder fields that put a +-extent m scene on a height x width map at out_size_factor 8 (the
+    nuScenes configs: extent 54, 180 x 180, voxel 0.075).  The coder's x runs along the map's rows."""
+    return dict(pc_range=[-extent, -extent], out_size_factor=8,
+                voxel_size=[2 * extent / height / 8, 2 * extent / width / 8],
+                post_center_range=[-61.2, -61.2, -10.0, 61.2, 61.2, 10.0], max_num=max_num,
+                score_threshold=score_threshold, code_size=9)
+
+
+def centerhead_head_outputs(seed, batch, height=128, width=128, gt=None, extent=54.0):
+    """Raw CenterHead outputs for the six nuScenes tasks (CENTERHEAD_TASKS), shaped like a trained head's: a list
+    over tasks of dict(heatmap [B, cat, H, W] logits, reg [B, 2, H, W], height [B, 1, H, W], dim [B, 3, H, W] log
+    sizes, rot [B, 2, H, W] (sine, cosine), vel [B, 2, H, W]) fp32 CPU tensors for centerhead_coder_cfg(height,
+    width, extent).  The heatmap is built like transfusion_heatmap: a smooth background around logit -3.5 (the
+    head's bias initialisation, -2.19, is sigmoid 0.1; a trained background lies below it) plus one Gaussian blob
+    per object of gt = (boxes, labels) (default gt_boxes(seed, batch)) in its class's channel, of a sigma of a quarter
+    of the object's footprint in cells (0.7 to 2), so that a few hundred
+    cells per task and sample exceed a 0.1 score threshold.  The regression maps hold the object's values (centre
+    offset, gravity-centre z, log size, yaw, velocity, lightly jittered) within two cells of its centre and noise
+    elsewhere.  The box x axis runs along the rows, as the coder decodes it."""
+    rng = np.random.default_rng(seed)
+    boxes, labels = gt if gt is not None else gt_boxes(seed=seed, batch=batch)
+    first = np.cumsum([0] + [len(c) for c in CENTERHEAD_TASKS])
+    rows, cols = np.arange(height)[:, None], np.arange(width)[None, :]
+    out = []
+    for t, classes in enumerate(CENTERHEAD_TASKS):
+        cat = len(classes)
+        noise = rng.standard_normal((batch, cat, height + 2, width + 2))
+        heat = sum(noise[:, :, dy:dy + height, dx:dx + width] for dy in range(3) for dx in range(3)) / 6.0 - 3.5
+        reg = rng.uniform(0.0, 1.0, (batch, 2, height, width))
+        hei = rng.normal(-0.5, 1.0, (batch, 1, height, width))
+        dim = np.log(rng.uniform(0.3, 8.0, (batch, 3, height, width)))
+        rot = rng.normal(0.0, 0.6, (batch, 2, height, width))
+        vel = rng.normal(0.0, 1.0, (batch, 2, height, width))
+        for b in range(batch):
+            g = boxes[b].numpy().astype(np.float64)
+            lab = labels[b].numpy()
+            for i in np.nonzero((lab >= first[t]) & (lab < first[t + 1]))[0]:
+                cx = (g[i, 0] + extent) / (2 * extent) * height          # x along the rows
+                cy = (g[i, 1] + extent) / (2 * extent) * width
+                if not (0 <= cx < height and 0 <= cy < width):
+                    continue
+                sigma = min(2.0, max(0.7, 0.25 * max(g[i, 3] / (2 * extent) * height, g[i, 4] / (2 * extent) * width)))
+                heat[b, lab[i] - first[t]] += rng.uniform(2.0, 7.0) * np.exp(
+                    -((rows - cx) ** 2 + (cols - cy) ** 2) / (2 * sigma * sigma))
+                r0, r1 = max(int(cx) - 2, 0), min(int(cx) + 3, height)
+                c0, c1 = max(int(cy) - 2, 0), min(int(cy) + 3, width)
+                n = (r1 - r0, c1 - c0)
+                reg[b, 0, r0:r1, c0:c1] = cx - np.arange(r0, r1)[:, None] + rng.normal(0, 0.05, n)
+                reg[b, 1, r0:r1, c0:c1] = cy - np.arange(c0, c1)[None, :] + rng.normal(0, 0.05, n)
+                hei[b, 0, r0:r1, c0:c1] = g[i, 2] + 0.5 * g[i, 5] + rng.normal(0, 0.05, n)
+                for d in range(3):
+                    dim[b, d, r0:r1, c0:c1] = np.log(g[i, 3 + d]) + rng.normal(0, 0.03, n)
+                yaw = g[i, 6] + rng.normal(0, 0.05, n)
+                rot[b, 0, r0:r1, c0:c1], rot[b, 1, r0:r1, c0:c1] = np.sin(yaw), np.cos(yaw)
+                for d in range(2):
+                    vel[b, d, r0:r1, c0:c1] = g[i, 7 + d] + rng.normal(0, 0.1, n)
+        out.append({k: torch.from_numpy(v.astype(np.float32)).contiguous() for k, v in
+                    dict(heatmap=heat, reg=reg, height=hei, dim=dim, rot=rot, vel=vel).items()})
+    return out

@@ -588,6 +588,51 @@ BEVB200_API int bevb200_transfusion_proposals(const void *heatmap, int dtype, in
                                               int64_t *labels, int64_t *index, void *query_heatmap_score,
                                               void *workspace, size_t workspace_bytes, void *stream);
 
+/* ---- CenterHead box decode (CenterHead.get_bboxes, centerpoint.py:669-698, and CenterPointBBoxCoder.decode,
+ * core/bbox/coders/centerpoint_bbox_coders.py:62-225) -----------------------------------------------------------
+ * The decode of all T tasks x B samples of a frame in two launches (candidates, select + decode), no host
+ * synchronisation, no allocation; CUDA-graph capturable and the same bit for bit on every run.  Segment
+ * s = t * B + b.  Host arrays of T entries give each task's device maps, fp32 contiguous NCHW:
+ *   heatmap[t] [B, cat[t], H, W]   reg[t] [B, 2, H, W]   height[t] [B, 1, H, W]   dim[t] [B, 3, H, W]
+ *   rot[t] [B, 2, H, W] (sine, cosine)   vel[t] [B, 2, H, W]
+ * reg may be NULL (no task has it: the centre is the cell's middle, + 0.5) and so may vel (box code size 7 instead
+ * of 9); otherwise every entry is a map.  heat_is_logit != 0: the score is sigmoid(heatmap) as torch computes it on
+ * CUDA (1 / (1 + expf(-x)), IEEE division), else the heatmap itself; dim_is_log != 0: dim is expf(dim) (the head's
+ * norm_bbox), else dim itself.
+ * Per segment, over the task's cat * H * W scores with flat index c * H * W + row * W + col, the first
+ * K = max_num in descending score (NaN above everything) with ties by ascending flat index are taken: the
+ * reference's per-class top-k followed by its top-k over cat * K, with stable sorts.  label = flat / (H * W),
+ * ind = flat % (H * W).  The reference names the map [B, N, W, H]: its xs = trunc(float(ind) / float(W)) is the ROW
+ * (equal to ind / W for ind < 2^24) and its ys = ind % W the column.  Each step is one fp32 rounding, in this order:
+ *   x = ((row + reg[0]) * out_size_factor) * voxel_x + pc_x      y = ((col + reg[1]) * out_size_factor) * voxel_y + pc_y
+ * (+ 0.5 without reg; the double arguments are rounded to fp32 first), and the box row is
+ *   [x, y, height, dim0, dim1, dim2, atan2f(rot[0], rot[1]), vel0, vel1]    all maps read at ind.
+ * A selected row survives when (use_score_threshold == 0 or score > score_threshold, strict, in fp32; a NaN score
+ * took one of the K places and fails this test) and post_center_range[0..2] <= (x, y, height) <=
+ * post_center_range[3..5] (6 host doubles, rounded to fp32; inclusive).  Survivors are compacted to the front of the
+ * segment in their descending-score order:
+ *   boxes  [T * B, K, code] fp32   scores [T * B, K] fp32   labels [T * B, K] fp32 (the reference's clses.float())
+ *   index  [T * B, K] int32, nullable: ind of each row      counts [T * B] int32
+ * Rows at and after counts[s] are zero in every output.  A refused call writes nothing.
+ * BEVB200_EINVAL: T, B, H, W or a class count < 1, max_num < 1 or > H * W (the reference's per-class topk raises), a
+ * null required pointer.  BEVB200_EUNSUPPORTED: T, T * B, a class count, cat * H * W or max_num above the limits
+ * below.  Workspace: bevb200_centerhead_decode_workspace_bytes(T, B, cat, H, W) = align256(8 * T * B * Tl * 1024) +
+ * align256(4 * T * B * Tl), Tl = ceil(max cat * H * W / 1024); 0 for unsupported sizes; a smaller one gives
+ * BEVB200_EWORKSPACE. */
+#define BEVB200_DECODE_MAX_TASKS 16
+#define BEVB200_DECODE_MAX_SEGMENTS 65535      /* T * B */
+#define BEVB200_DECODE_MAX_CLASSES 64          /* per task */
+#define BEVB200_DECODE_MAX_CELLS (1 << 24)     /* cat * H * W per task and sample */
+#define BEVB200_DECODE_MAX_K 4096
+BEVB200_API size_t bevb200_centerhead_decode_workspace_bytes(int T, int B, const int *cat, int H, int W);
+BEVB200_API int bevb200_centerhead_decode(
+    const float *const *heatmap, const float *const *reg, const float *const *height, const float *const *dim,
+    const float *const *rot, const float *const *vel, const int *cat, int T, int B, int H, int W, int max_num,
+    int heat_is_logit, int dim_is_log, double out_size_factor, double voxel_x, double voxel_y, double pc_x,
+    double pc_y, const double *post_center_range, int use_score_threshold, double score_threshold, float *boxes,
+    float *scores, float *labels, int32_t *index, int32_t *counts, void *workspace, size_t workspace_bytes,
+    void *stream);
+
 /* ---- LiDAR depth images for the depth-aware camera lift ------------------------------------
  * BaseDepthTransform.forward's per-sample loop (mmdet3d/models/vtransforms/base.py:279-329):
  * undo the lidar augmentation, project every point into every camera with lidar2image, clamp z to
