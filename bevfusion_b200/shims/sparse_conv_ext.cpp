@@ -66,12 +66,14 @@ std::vector<torch::Tensor> get_indice_pairs_3d(torch::Tensor indices, int64_t ba
   return {outInds, pairs, num};
 }
 
-// half tensors are widened, computed with fp32 accumulation on the tensor cores and narrowed once
+// half tensors are widened, computed with fp32 accumulation on the tensor cores and narrowed once; the
+// output is half when the features or the filters are (the rule of the python module's indice_conv)
 static torch::Tensor conv_impl(torch::Tensor features, torch::Tensor filters, const torch::Tensor *bias,
                                torch::Tensor indicePairs, torch::Tensor indiceNum, int64_t numActOut, int64_t inverse) {
   check_cuda(features, "features"); check_cuda(filters, "filters"); check_cuda(indicePairs, "indicePairs");
   c10::cuda::CUDAGuard guard(features.device());
-  const auto in_dtype = features.scalar_type();
+  const bool half = features.scalar_type() == torch::kHalf || filters.scalar_type() == torch::kHalf;
+  const auto in_dtype = half ? torch::kHalf : features.scalar_type();
   auto f = features.to(torch::kFloat32).contiguous();
   auto w = filters.to(torch::kFloat32).contiguous();
   const int K = indicePairs.size(0), cin = f.size(1), cout = w.size(w.dim() - 1);
@@ -104,7 +106,8 @@ std::vector<torch::Tensor> indice_conv_backward(torch::Tensor features, torch::T
   (void)_subM;
   check_cuda(features, "features"); check_cuda(filters, "filters"); check_cuda(outGrad, "outGrad");
   c10::cuda::CUDAGuard guard(features.device());
-  const auto in_dtype = features.scalar_type();
+  // each gradient in the dtype of the tensor it belongs to
+  const auto f_dtype = features.scalar_type(), w_dtype = filters.scalar_type();
   auto f = features.to(torch::kFloat32).contiguous();
   auto w = filters.to(torch::kFloat32).contiguous();
   auto g = outGrad.to(torch::kFloat32).contiguous();
@@ -121,7 +124,7 @@ std::vector<torch::Tensor> indice_conv_backward(torch::Tensor features, torch::T
                                            din.data_ptr<float>(), dw.data_ptr<float>(), ws.data_ptr(), (size_t)ws.numel(),
                                            cur_stream()),
               bevb200_last_error());
-  return {din.to(in_dtype), dw.to(in_dtype)};
+  return {din.to(f_dtype), dw.to(w_dtype)};
 }
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {

@@ -62,8 +62,9 @@ class SparseEncoder(nn.Module):
 
     def forward(self, voxel_features, coors, batch_size, fused=None, precision=None, out=None,
                 num_voxels=None, **kwargs):
-        """sparse_encoder.py:99-132.  voxel_features [N, C] fp32, coors [N, 4] int32
-        (batch, x, y, z).  Returns spatial features [B, C*D, H, W].
+        """sparse_encoder.py:99-132.  voxel_features [N, C] fp32 or fp16, coors [N, 4] int32
+        (batch, x, y, z).  Returns spatial features [B, C*D, H, W], in half when the features or the
+        conv weights are (each conv computes in fp32 and narrows its output once).
 
         fused=None picks the fused path (BN / ReLU / residual in the conv epilogues, dense()
         written directly in the output layout) whenever the module is in eval mode.  `out`
@@ -75,7 +76,8 @@ class SparseEncoder(nn.Module):
         if precision is None:
             precision = sp_ops.default_precision()
         if (fused and self.native_plan and precision == sp_ops.PREC_BF16X3 and not torch.is_grad_enabled()
-                and voxel_features.dtype == torch.float32 and self.plan() is not None):
+                and voxel_features.dtype == torch.float32 and self.conv_input[0].weight.dtype == torch.float32
+                and self.plan() is not None):
             # `num_voxels` (device int32[1]): only the first rows are valid -- no host round trip
             return self.plan().forward(voxel_features.contiguous(), coors.contiguous(), batch_size,
                                        n_voxels_dev=num_voxels, out=out, overlap_rulebooks=self.overlap_rulebooks)
@@ -164,6 +166,12 @@ class SparseEncoder(nn.Module):
             if ahead and queued >= 3:
                 ahead(next_strided(pos))                      # the rest, hidden behind >= 3 queued convs
         out = x
+        if out.features.dtype != torch.float32:
+            # half features (the native plan takes fp32 only): each conv above widened and narrowed its
+            # own rows; the scatter runs on widened rows and the output keeps the features' dtype
+            dense = sp_ops.sparse_to_dense(out.features.float(), out.indices, int(out.batch_size),
+                                           out.spatial_shape, z_major=True)
+            return dense.to(out.features.dtype) if dense_out is None else dense_out.copy_(dense)
         # dense() + permute(0,1,4,2,3) + view(N, C*D, H, W) in one kernel
         return sp_ops.sparse_to_dense(out.features, out.indices, int(out.batch_size),
                                       out.spatial_shape, z_major=True, out=dense_out)

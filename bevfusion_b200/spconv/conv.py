@@ -78,9 +78,10 @@ class SparseConvolution(SparseModule):
         if precision == ops.PREC_FP32:
             return None
         w = self.weight
-        key = (int(precision), w.data_ptr(), w._version, str(w.device))
+        # keyed on the parameter itself, so a half parameter is widened and packed once, not every call
+        key = (int(precision), w.data_ptr(), w._version, str(w.device), w.dtype)
         if self._packed_cache is None or self._packed_cache[0] != key:
-            self._packed_cache = (key, ops.pack_weights(w.detach().contiguous(), precision))
+            self._packed_cache = (key, ops.pack_weights(w.detach().float().contiguous(), precision))
         return self._packed_cache[1]
 
     def reset_parameters(self):
@@ -173,14 +174,23 @@ class SparseConvolution(SparseModule):
             torch.cuda.current_stream(features.device).wait_event(ready)
             rb.ready = None
         if fused or not needs_grad:
+            # half features or weights (mixed-precision training, ops.indice_conv's rule): widened to
+            # fp32 once, the same kernel, the output narrowed once after the epilogue
+            half = torch.half in (features.dtype, self.weight.dtype)
             if self.bias is not None:
                 # bias folds into the epilogue shift: (acc + b) * s + t = acc * s + (b * s + t)
-                b = self.bias.detach()
+                b = self.bias.detach().float()
                 shift = b * scale + shift if scale is not None and shift is not None else (
                     b * scale if scale is not None else (b + shift if shift is not None else b))
-            out_features = ops.sparse_conv(features.contiguous(), self.weight.detach().contiguous(),
+            weight = self.weight.detach()
+            if half:
+                features, weight = features.float(), weight.float()
+                residual = None if residual is None else residual.float().contiguous()
+            out_features = ops.sparse_conv(features.contiguous(), weight.contiguous(),
                                            rb.nbr, rb.n_out, scale, shift, residual, relu, precision,
                                            packed=self._packed_weight(precision))
+            if half:
+                out_features = out_features.half()
         else:
             fn = Fsp.indice_subm_conv if self.subm else Fsp.indice_conv
             out_features = fn(features, self.weight, rb, None, rb.n_out)

@@ -325,10 +325,12 @@ def indice_conv_backward(features, filters, out_bp, indice_pairs, indice_pair_nu
     """Drop-in for ops.indice_conv_backward (ops.py:177-189): returns [input_grad, filters_grad].
     `indice_pairs` may be the reference [K, 2, N] tensor or a Rulebook."""
     if torch.half in (filters.dtype, features.dtype, out_bp.dtype):
-        # indice_conv_backward_half (ops.py:183-186): widened, computed with fp32 accumulation, narrowed once
+        # indice_conv_backward_half (ops.py:183-186): widened, computed with fp32 accumulation, narrowed
+        # once -- each gradient to the dtype of the tensor it belongs to, so fp32 weights next to half
+        # features get an fp32 filter gradient (no fp16 rounding, no overflow the weights cannot have)
         din, dw = indice_conv_backward(features.float(), filters.float(), out_bp.float(), indice_pairs,
                                        indice_pair_num, inverse, subm, precision)
-        return [din.half(), dw.half()]
+        return [din.to(features.dtype), dw.to(filters.dtype)]
     if filters.dtype != torch.float32:
         raise NotImplementedError("filters must be fp32 or fp16")
     if isinstance(indice_pairs, Rulebook):

@@ -12,7 +12,9 @@ class _ToDenseFunction(torch.autograd.Function):
     def forward(ctx, features, indices, batch_size, spatial_shape):
         ctx.save_for_backward(indices)
         ctx.in_dtype = features.dtype
-        return ops.sparse_to_dense(features.float().contiguous(), indices, batch_size, spatial_shape, z_major=False)
+        # the scatter kernel takes fp32 rows; like the reference's scatter_nd the result has the features' dtype
+        out = ops.sparse_to_dense(features.float().contiguous(), indices, batch_size, spatial_shape, z_major=False)
+        return out.to(features.dtype)
 
     @staticmethod
     def backward(ctx, grad):

@@ -10,6 +10,8 @@ import torch
 
 import oracle
 from conftest import ref_module
+from encoder_oracle import conv_nbr
+from half_oracle import check as check_half
 
 pytestmark = pytest.mark.gpu
 
@@ -528,12 +530,16 @@ def test_half_features(cuda):
     feat = rng.standard_normal((n, cin)).astype(np.float16)
     W = (rng.standard_normal((*ks, cin, cout)) / 17).astype(np.float16)
     gold, _, _ = oracle.sparse_conv(feat.astype(np.float32), idx, B, shape, W.astype(np.float32), ks, st, pd,
-                                    [1, 1, 1], subm)
+                                    [1, 1, 1], subm, acc64=True)
+    gabs, _, _ = oracle.sparse_conv(np.abs(feat).astype(np.float32), idx, B, shape, np.abs(W).astype(np.float32), ks,
+                                    st, pd, [1, 1, 1], subm, acc64=True)
     outids, pairs, num = ops.get_indice_pairs(torch.from_numpy(idx).to(cuda), B, shape, ks, st, pd, 1, 0, subm)
     out = ops.sparse_conv_ext.indice_conv_half(torch.from_numpy(feat).to(cuda), torch.from_numpy(W).to(cuda),
                                                pairs, num, outids.shape[0], 0, int(subm))
     assert out.dtype == torch.half
-    assert rel_err(out.float().cpu().numpy(), gold) <= 2e-3      # one fp16 rounding of the result
+    # one fp16 rounding of the result (tests/half_oracle.py)
+    t64 = lambda a: torch.from_numpy(np.asarray(a, np.float64))
+    print("indice_conv_half worst ratio %.3f" % check_half(out.cpu(), t64(gold), t64(gabs), "indice_conv_half"))
 
 
 def test_fused_indice_conv_and_half_backward_shims(cuda):
@@ -550,15 +556,21 @@ def test_fused_indice_conv_and_half_backward_shims(cuda):
     plain = ext.indice_conv_fp32(feat, W, pairs, num, outids.shape[0], 0, 1)
     fused = ext.fused_indice_conv_fp32(feat, W, bias, pairs, num, outids.shape[0], 0, 1)
     assert float((fused - (plain + bias)).abs().max()) <= 1e-6 * float(plain.abs().max())
-    fused_h = ext.fused_indice_conv_half(feat.half(), W.half(), bias.half(), pairs, num, outids.shape[0], 0, 1)
+    fh, Wh, bh = feat.half(), W.half(), bias.half()
+    fused_h = ext.fused_indice_conv_half(fh, Wh, bh, pairs, num, outids.shape[0], 0, 1)
     assert fused_h.dtype == torch.half
-    assert float((fused_h.float() - fused).abs().max()) <= 2e-2 * float(fused.abs().max())
-    g = torch.randn_like(plain)
-    din, dw = ext.indice_conv_backward_fp32(feat, W, g, pairs, num, 0, 1)
-    din_h, dw_h = ext.indice_conv_backward_half(feat.half(), W.half(), g.half(), pairs, num, 0, 1)
+    # float64 on the half-rounded inputs, at one fp16 rounding (tests/half_oracle.py)
+    nbr = ops.nbr_from_pairs(pairs, num, outids.shape[0])
+    check_half(fused_h, conv_nbr(fh, Wh, nbr) + bh.double(), conv_nbr(fh.abs(), Wh.abs(), nbr) + bh.double().abs(),
+               "fused_indice_conv_half")
+    g = torch.randn_like(plain).half()
+    din_h, dw_h = ext.indice_conv_backward_half(fh, Wh, g, pairs, num, 0, 1)
     assert din_h.dtype == torch.half and dw_h.dtype == torch.half and dw_h.shape == W.shape
-    assert float((din_h.float() - din).abs().max()) <= 2e-2 * float(din.abs().max())
-    assert float((dw_h.float() - dw).abs().max()) <= 2e-2 * float(dw.abs().max())
+    from test_spconv_backward_gpu import reference
+    ref_din, ref_dw, _ = reference(fh, Wh.reshape(27, 16, 32), g, nbr)
+    abs_din, abs_dw, _ = reference(fh.abs(), Wh.abs().reshape(27, 16, 32), g.abs(), nbr)
+    check_half(din_h, ref_din, abs_din, "indice_conv_backward_half input grad")
+    check_half(dw_h.reshape(27, 16, 32), ref_dw, abs_dw, "indice_conv_backward_half filter grad")
     with pytest.raises(AttributeError):                         # out-of-scope names: a plain missing attribute
         ext.indice_maxpool_fp32
     assert not hasattr(ext, "get_indice_pairs_2d")
