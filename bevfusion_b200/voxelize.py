@@ -138,7 +138,12 @@ class _VoxelLayer:
         """voxelization.h:97-109 / scatter_points_cuda.cu:187-241.  Returns
         [reduced_feats [M, C], out_coors [M, ndim], coors_map [N] int32, reduce_count [M] int32];
         voxels are the unique coordinate rows in lexicographic order, rows with a negative
-        entry are dropped (coors_map -1)."""
+        entry are dropped (coors_map -1).
+
+        NaN features: sum and mean propagate them.  max ignores them, as the reference's fmaxf
+        reduction does (:22-30): a voxel's maximum is taken over its non-NaN values, a voxel
+        holding only NaN yields -inf, and the backward pass gives a NaN element no gradient
+        (NaN never equals the maximum, :162)."""
         out = _dynamic_scatter_forward(feats, coors, reduce_type)
         return [out[0], out[1], out[2], out[3]]
 
@@ -273,7 +278,7 @@ def voxelize_batch(points, voxelize_module, voxelize_reduce=True):
             feats.append(f); coords.append(c4); sizes.append(n)
             continue
         ret = voxelize_module(res)
-        if len(ret) == 3:
+        if isinstance(ret, tuple):     # not len(ret) == 3: dynamic coords of a 3-point sample are [3, 3]
             f, c, n = ret
             if voxelize_reduce:
                 f, c4 = voxelize_mean(f.contiguous(), c.contiguous(), n.contiguous(), k)

@@ -39,6 +39,8 @@ def points_to_depth(points, lidar2image, img_aug_matrix, lidar_aug_matrix, image
         _C.require_cuda(pts, "points[%d]" % b, torch.float32)
     dev = points[0].device
     F = int(points[0].shape[1])
+    if any(p.shape[1] != F for p in points):             # before any sample is rasterised
+        raise ValueError("all samples must have the same number of point features")
     channels = (int(depth_bins) if one_hot else 1) + (F if add_depth_features else 0)
     l2i = lidar2image.to(device=dev, dtype=torch.float32).contiguous()
     ia = img_aug_matrix.to(device=dev, dtype=torch.float32).contiguous()
@@ -49,8 +51,6 @@ def points_to_depth(points, lidar2image, img_aug_matrix, lidar_aug_matrix, image
         ws = torch.empty(max(nbytes, 256), dtype=torch.uint8, device=dev)
         for b in range(B):
             p = points[b]
-            if p.shape[1] != F:
-                raise ValueError("all samples must have the same number of point features")
             rc = _C.lib().bevb200_depth_rasterize(
                 _C.ptr(p), int(p.shape[0]), F, _C.ptr(la[b]), _C.ptr(l2i[b]), _C.ptr(ia[b]), ncam, iH, iW,
                 int(one_hot), int(depth_bins or 0), int(bool(add_depth_features)), _C.ptr(depth[b]),

@@ -182,11 +182,62 @@ def voxel_mean(voxels, num_points):
     return (voxels.astype(np.float64).sum(axis=1) / num_points.reshape(-1, 1)).astype(np.float32)
 
 
+_U32 = 2.0 ** -24     # unit roundoff of fp32
+
+
+def fp32_sum_bound(abs_sum, count, mean_of=None):
+    """Error bound of a left-to-right fp32 sum of `count` terms whose absolute values add up to
+    `abs_sum` (float64): |fl(sum) - sum| <= g * abs_sum, g = k / (1 - k), k = (count - 1) * 2^-24
+    (Higham, Accuracy and Stability, eq. 4.4).  With `mean_of` (the float64 mean) the bound is the
+    one of fl(fl(sum) / count): the sum's error over count, plus one rounding of the quotient."""
+    count = np.asarray(count, np.float64)
+    k = np.maximum(count - 1.0, 0.0) * _U32
+    b = k / (1.0 - k) * np.asarray(abs_sum, np.float64)
+    if mean_of is not None:
+        b = b / count
+        b = b + _U32 * (np.abs(mean_of) + b) + 2.0 ** -149
+    return b
+
+
+def assert_within(got, ref64, bound, what=""):
+    """Per element: |got - ref64| <= bound where ref64 is finite; identical (inf / NaN included)
+    where it is not."""
+    got = np.asarray(got, np.float64)
+    fin = np.isfinite(ref64)
+    assert np.array_equal(got[~fin], ref64[~fin], equal_nan=True), what + ": non-finite elements differ"
+    err = np.abs(got[fin] - ref64[fin])
+    bad = ~(err <= bound[fin])
+    assert not bad.any(), "%s: %d elements outside their bound, worst %g x bound" % (
+        what, int(bad.sum()), float(np.nanmax(err[bad] / np.maximum(bound[fin][bad], 1e-300))))
+
+
+def segment_reduce_f64(feats, seg, m, mean=False):
+    """float64 sum (or mean) of the rows of feats [N, C] over segment ids seg [N] (-1 = skipped)
+    -> (ref [m, C] float64, bound [m, C]): the fp32 result of adding each segment's rows one at
+    a time, in any fixed order, lies within `bound` of `ref` (fp32_sum_bound)."""
+    x = np.asarray(feats, np.float64)
+    seg = np.asarray(seg, np.int64)
+    keep = seg >= 0
+    ref = np.zeros((m, x.shape[1]))
+    mag = np.zeros((m, x.shape[1]))
+    with np.errstate(invalid="ignore"):
+        np.add.at(ref, seg[keep], x[keep])
+        np.add.at(mag, seg[keep], np.abs(x[keep]))
+    count = np.bincount(seg[keep], minlength=m).astype(np.float64)[:, None]
+    if mean:
+        with np.errstate(invalid="ignore", divide="ignore"):
+            ref = ref / count
+        return ref, fp32_sum_bound(mag, count, mean_of=ref)
+    return ref, fp32_sum_bound(mag, count)
+
+
 def dynamic_scatter(feats, coors, reduce_type="max"):
     """dynamic_point_to_voxel_forward (scatter_points_cuda.cu:187-241): rows with a negative
     entry are masked to -1 (:203), at::unique_dim sorts the rows lexicographically (:206-208) and
     the leading all -1 row is removed (:210-215); features are reduced per voxel (sum / mean in
     fp64 here, so the comparison with either GPU implementation is a tolerance one; max is exact).
+    The reference's max is a CAS loop on fmaxf starting from -inf (:22-30, :223), so NaN features
+    are ignored and a voxel holding only NaN reduces to -inf.
     Returns (reduced [M, C] f32, out_coors [M, ndim] i32, coors_map [N] i32, count [M] i32).
     PINNING: the reference has no CPU path for this op (voxelization.h:118); the restatement is
     checked on the GPU box against oracle/_ref's voxel_layer (tests/test_voxelize_gpu.py)."""
@@ -205,7 +256,7 @@ def dynamic_scatter(feats, coors, reduce_type="max"):
     keep = inv >= 0
     if reduce_type == "max":
         red = np.full((m, c), -np.inf, np.float32)
-        np.maximum.at(red, inv[keep], feats[keep])
+        np.fmax.at(red, inv[keep], feats[keep])     # fmaxf (:22-30): a NaN never replaces a number
     else:
         red = np.zeros((m, c), np.float64)
         np.add.at(red, inv[keep], feats[keep].astype(np.float64))
@@ -226,15 +277,14 @@ def dynamic_scatter_backward(grad_reduced, feats, reduced, coors_map, count, red
             g[keep] /= count[coors_map[keep]][:, None].astype(np.float32)
         return g
     m, c = reduced.shape
-    frm = np.full((m, c), feats.shape[0], np.int64)          # :286 full(num_input)
-    for i in np.nonzero(keep)[0]:                           # :145-160 smallest index attaining max
-        v = coors_map[i]
-        hit = feats[i] == reduced[v]
-        frm[v, hit] = np.minimum(frm[v, hit], i)
-    for v in range(m):
-        for ch in range(c):
-            if frm[v, ch] < feats.shape[0]:
-                g[frm[v, ch], ch] = grad_reduced[v, ch]
+    n = feats.shape[0]
+    frm = np.full((m, c), n, np.int64)                       # :286 full(num_input)
+    pts = np.nonzero(keep)[0]
+    seg = np.asarray(coors_map, np.int64)[pts]
+    hit = feats[pts] == np.asarray(reduced)[seg]             # :162 (NaN never equals the maximum)
+    np.minimum.at(frm, seg, np.where(hit, pts[:, None], n))  # :163 smallest index attaining the max
+    v, ch = np.nonzero(frm < n)
+    g[frm[v, ch], ch] = np.asarray(grad_reduced)[v, ch]
     return g
 
 
