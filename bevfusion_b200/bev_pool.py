@@ -317,7 +317,14 @@ class BEVPoolPlan:
         key = (cameras, D, fH, fW)
         cached = getattr(self, "_lift_cache", None)
         if cached is not None and cached[0] == key:
+            if torch.cuda.is_current_stream_capturing():
+                self._lift_captured = True
             return cached[1]
+        if cached is not None and getattr(self, "_lift_captured", False):
+            # a graph captured earlier still reads these tables at every replay: dropping them would let the
+            # allocator reuse the memory under it, so tables a capture used stay alive with the plan
+            self.__dict__.setdefault("_lift_graph_held", []).append(cached[1])
+        self._lift_captured = False
         t = self.tables
         dev = t.perm.device
         L = _C.lib()

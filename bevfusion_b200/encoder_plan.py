@@ -87,6 +87,8 @@ class EncoderPlan:
         self._params = None
         self._param_key = None
         self._ws = None
+        self._ws_captured = False    # a CUDA graph recorded a forward that uses self._ws
+        self._graph_held = []        # replaced workspaces that a captured graph still writes into
         self._side = None
         self.status = None           # int32[1 + levels] of the last forward (device)
 
@@ -165,8 +167,14 @@ class EncoderPlan:
             caps = self._caps_arg(level_caps)
             need = L.bevb200_encoder_workspace_bytes(self._h, n, B, caps)
             if self._ws is None or self._ws.device != dev or self._ws.numel() < need:
-                self._ws = None
+                # a graph captured earlier replays into the old block: once freed, the allocator would hand it
+                # to other tensors, so a captured workspace stays alive with the plan
+                if self._ws_captured:
+                    self._graph_held.append(self._ws)
+                self._ws, self._ws_captured = None, False
                 self._ws = torch.empty(int(need * 1.25) + 4096, dtype=torch.uint8, device=dev)
+            if torch.cuda.is_current_stream_capturing():
+                self._ws_captured = True
             if self.status is None or self.status.device != dev:
                 self.status = torch.zeros(1 + self.n_levels, dtype=torch.int32, device=dev)
             side = 0
