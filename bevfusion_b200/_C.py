@@ -89,6 +89,13 @@ _SIGNATURES = {
     "bevb200_centerhead_decode_workspace_bytes": (c_size_t, [c_int, c_int, _P, c_int, c_int]),
     "bevb200_centerhead_decode": (c_int, [_P] * 7 + [c_int] * 7 + [ctypes.c_double] * 5 + [_P, c_int, ctypes.c_double]
                                   + [_P] * 6 + [c_size_t, _P]),
+    "bevb200_centerhead_loss_workspace_bytes": (c_size_t, [c_int, c_int, _P] + [c_int] * 4),
+    "bevb200_centerhead_loss": (c_int, [_P] * 11 + [c_int] * 6 + [_P] + [ctypes.c_double] * 4 + [_P] * 4
+                                + [c_size_t, _P]),
+    "bevb200_centerhead_loss_backward": (c_int, [_P] * 11 + [c_int] * 6 + [_P] + [ctypes.c_double] * 4 + [_P] * 9),
+    "bevb200_transfusion_loss_workspace_bytes": (c_size_t, [c_int] * 8),
+    "bevb200_transfusion_loss": (c_int, [_P] * 13 + [c_int, _P, c_int] + [c_int] * 8 + [_P] * 7 + [c_size_t, _P]),
+    "bevb200_transfusion_loss_backward": (c_int, [_P] * 12 + [c_int] * 8 + [_P] * 3 + [_P] * 10),
     "bevb200_rulebook_workspace_bytes": (c_size_t, [c_int, c_int, _P]),
     "bevb200_rulebook_prepare": (c_int, [_P, c_int, c_int] + [_P] * 6 + [c_int, _P, _P, c_size_t, _P]),
     "bevb200_rulebook_fill": (c_int, [_P, c_int, c_int] + [_P] * 6 + [c_int, c_int, _P, _P, _P,

@@ -633,6 +633,78 @@ BEVB200_API int bevb200_centerhead_decode(
     float *scores, float *labels, int32_t *index, int32_t *counts, void *workspace, size_t workspace_bytes,
     void *stream);
 
+/* ---- CenterHead and TransFusion training losses ----------------------------------------------------------------
+ * CenterHead.loss (models/heads/bbox/centerpoint.py:584-634) and TransFusionHead.loss (transfusion.py:587-713) with
+ * mmdet 2.20's GaussianFocalLoss, FocalLoss(use_sigmoid=True) (mmcv 1.4's sigmoid_focal_loss CUDA op) and L1Loss,
+ * all reduction "mean".  Forward: two launches; backward: two (CenterHead) or one (TransFusion).  No allocation, no
+ * host synchronisation, stream-ordered, CUDA-graph capturable; every output element is written and the sums are
+ * taken in double in a fixed order, so results are reproducible bit for bit.
+ *   clip_sigmoid(x) = clamp(1 / (1 + expf(-x)), fp32(1e-4), fp32(1 - 1e-4)), its gradient 0 outside those bounds
+ *     (bounds included in the passing range).  Inputs are never modified (the reference's sigmoid_ is in place).
+ *   gaussian focal (alpha, gamma = focal_host pair): per element, p = clip_sigmoid(x), eps = 1e-12,
+ *     -log(p + eps) (1 - p)^alpha [t == 1] - log(1 - p + eps) p^alpha (1 - t)^gamma;  sum / max(count(t == 1), 1)
+ *   sigmoid focal (alpha, gamma), logits [R, K], int64 labels [R] with K the background:
+ *     -[l == c] alpha (1 - p)^gamma log(max(p, FLT_MIN)) - [l != c] (1 - alpha) p^gamma log(max(1 - p, FLT_MIN)),
+ *     times the row's int64 label weight, sum / avg; a label outside [0, K] skips its row and sets
+ *     BEVB200_LOSS_BAD_LABEL
+ *   L1: sum |pred - target| w / avg; a NaN target gives a NaN loss even at w = 0, its gradient is 0 (sgn(NaN) = 0)
+ *   each loss is multiplied by its loss_weight.
+ * CenterHead, per task t (maps [B, ch, H, W] fp32; vel only with code 10):
+ *   heatmap[t] [B, cat[t], H, W] logits vs heat_target[t];  pred = cat(reg, height, dim, rot[, vel]) gathered at
+ *   ind[t] [B, M] int64 (cell row * W + col) against anno_box[t] [B, M, code] with weights
+ *   fp32(mask[t] (uint8 [B, M]) * isnotnan(target)) * fp32(code_weights[c]) and avg fp32(sum mask[t] + 1e-4).
+ *   An ind outside [0, H * W) skips its slot; on a slot with mask != 0 it sets BEVB200_LOSS_BAD_IND.
+ *   losses / avg_factors [2T] fp32: heatmap of task t at 2t, bbox at 2t + 1; status [1] int32.
+ *   Backward: grad_losses [2T] (device); gradients of every map (same shapes), each element written once; slots that
+ *   share a cell add their contributions in slot order.
+ * TransFusion (the cls and box terms of trained layer l use columns l * P .. (l + 1) * P of N):
+ *   dense_heatmap [B, K, H, W] logits vs dense_target;  heatmap [B, K, N] logits, labels / label_weights [B, N]
+ *   int64;  center [B, 2, N], height [B, 1, N], dim [B, 3, N], rot [B, 2, N], vel [B, 2, N] against
+ *   bbox_targets [B, N, code] with weights fp32(bbox_weights * code_weights[c]);  avg max(sum num_pos, 1) with
+ *   num_pos int32 [n_num_pos].  losses: [0] heatmap, [1 + 2l] cls, [2 + 2l] bbox of layer l < Lt,
+ *   [1 + 2 Lt] matched_ious = mean of mean_iou fp32 [n_iou];  avg_factors [2]: heatmap, layers.  Backward:
+ *   grad_losses [1 + 2 Lt]; the cls and box gradients are dense over [B, c, N], 0 in columns of untrained layers.
+ * focal_host: 4 doubles (heatmap alpha, gamma, cls alpha, gamma; CenterHead: 2); loss_weights_host (TransFusion):
+ * heatmap, cls, bbox.  BEVB200_EINVAL: a size < 1, code not 8 or 10, N not a multiple of P, Lt > N / P, a null
+ * pointer.  BEVB200_EUNSUPPORTED: more than BEVB200_LOSS_MAX_TASKS tasks, BEVB200_LOSS_MAX_OBJS slots or
+ * BEVB200_LOSS_MAX_LAYERS trained layers.  A smaller workspace than the query gives BEVB200_EWORKSPACE. */
+#define BEVB200_LOSS_MAX_TASKS 16
+#define BEVB200_LOSS_MAX_OBJS 4096
+#define BEVB200_LOSS_MAX_LAYERS 15
+#define BEVB200_LOSS_BAD_IND 1
+#define BEVB200_LOSS_BAD_LABEL 2
+BEVB200_API size_t bevb200_centerhead_loss_workspace_bytes(int T, int B, const int *cat, int H, int W, int M,
+                                                           int code);
+BEVB200_API int bevb200_centerhead_loss(
+    const float *const *heatmap, const float *const *reg, const float *const *height, const float *const *dim,
+    const float *const *rot, const float *const *vel, const float *const *heat_target, const float *const *anno_box,
+    const int64_t *const *ind, const uint8_t *const *mask, const int *cat, int T, int B, int H, int W, int M, int code,
+    const float *code_weights_host, double cls_alpha, double cls_gamma, double cls_weight, double bbox_weight,
+    float *losses, float *avg_factors, int32_t *status, void *workspace, size_t workspace_bytes, void *stream);
+BEVB200_API int bevb200_centerhead_loss_backward(
+    const float *const *heatmap, const float *const *reg, const float *const *height, const float *const *dim,
+    const float *const *rot, const float *const *vel, const float *const *heat_target, const float *const *anno_box,
+    const int64_t *const *ind, const uint8_t *const *mask, const int *cat, int T, int B, int H, int W, int M, int code,
+    const float *code_weights_host, double cls_alpha, double cls_gamma, double cls_weight, double bbox_weight,
+    const float *grad_losses, const float *avg_factors, float *const *g_heatmap, float *const *g_reg,
+    float *const *g_height, float *const *g_dim, float *const *g_rot, float *const *g_vel, void *stream);
+BEVB200_API size_t bevb200_transfusion_loss_workspace_bytes(int B, int K, int H, int W, int N, int P, int Lt,
+                                                            int code);
+BEVB200_API int bevb200_transfusion_loss(
+    const float *dense_heatmap, const float *dense_target, const float *heatmap, const float *center,
+    const float *height, const float *dim, const float *rot, const float *vel, const int64_t *labels,
+    const int64_t *label_weights, const float *bbox_targets, const float *bbox_weights, const int32_t *num_pos,
+    int n_num_pos, const float *mean_iou, int n_iou, int B, int K, int H, int W, int N, int P, int Lt, int code,
+    const float *code_weights_host, const double *focal_host, const double *loss_weights_host, float *losses,
+    float *avg_factors, int32_t *status, void *workspace, size_t workspace_bytes, void *stream);
+BEVB200_API int bevb200_transfusion_loss_backward(
+    const float *dense_heatmap, const float *dense_target, const float *heatmap, const float *center,
+    const float *height, const float *dim, const float *rot, const float *vel, const int64_t *labels,
+    const int64_t *label_weights, const float *bbox_targets, const float *bbox_weights, int B, int K, int H, int W,
+    int N, int P, int Lt, int code, const float *code_weights_host, const double *focal_host,
+    const double *loss_weights_host, const float *grad_losses, const float *avg_factors, float *g_dense,
+    float *g_heatmap, float *g_center, float *g_height, float *g_dim, float *g_rot, float *g_vel, void *stream);
+
 /* ---- LiDAR depth images for the depth-aware camera lift ------------------------------------
  * BaseDepthTransform.forward's per-sample loop (mmdet3d/models/vtransforms/base.py:279-329):
  * undo the lidar augmentation, project every point into every camera with lidar2image, clamp z to
