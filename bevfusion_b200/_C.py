@@ -100,7 +100,14 @@ _SIGNATURES = {
     "bevb200_transfusion_loss_workspace_bytes": (c_size_t, [c_int] * 8),
     "bevb200_transfusion_loss": (c_int, [_P] * 13 + [c_int, _P, c_int] + [c_int] * 8 + [_P] * 7 + [c_size_t, _P]),
     "bevb200_transfusion_loss_backward": (c_int, [_P] * 12 + [c_int] * 8 + [_P] * 3 + [_P] * 10),
-    "bevb200_rulebook_workspace_bytes": (c_size_t, [c_int, c_int, _P]),
+    "bevb200_map_grid_smem_bytes": (c_size_t, [c_int] * 4),
+    "bevb200_map_grid_transform": (c_int, [_P, _P, c_int, ctypes.c_longlong] + [c_int] * 4 + [_P] * 6
+                                   + [c_int, _P, _P, c_int, c_int, _P]),
+    "bevb200_map_seg_loss_workspace_bytes": (c_size_t, [c_int] * 4),
+    "bevb200_map_seg_loss": (c_int, [_P, c_int, _P] + [c_int] * 6 + [_P, _P, c_size_t, _P]),
+    "bevb200_map_seg_loss_backward": (c_int, [_P, c_int, _P] + [c_int] * 6 + [_P, _P, _P]),
+    "bevb200_map_seg_counts": (c_int, [_P, c_int, _P] + [c_int] * 5 + [_P, c_int, _P, _P]),
+    "bevb200_rulebook_workspace_bytes":(c_size_t, [c_int, c_int, _P]),
     "bevb200_rulebook_prepare": (c_int, [_P, c_int, c_int] + [_P] * 6 + [c_int, _P, _P, c_size_t, _P]),
     "bevb200_rulebook_fill": (c_int, [_P, c_int, c_int] + [_P] * 6 + [c_int, c_int, _P, _P, _P,
                                                                        c_size_t, _P]),

@@ -419,3 +419,69 @@ def centerhead_head_outputs(seed, batch, height=128, width=128, gt=None, extent=
         out.append({k: torch.from_numpy(v.astype(np.float32)).contiguous() for k, v in
                     dict(heatmap=heat, reg=reg, height=hei, dim=dim, rot=rot, vel=vel).items()})
     return out
+
+
+# ---- BEV map segmentation ------------------------------------------------------------------------------------------
+MAP_CLASSES = ("drivable_area", "ped_crossing", "walkway", "stop_line", "carpark_area", "divider")
+MAP_SEG_CFG = dict(input_scope=[[-51.2, 51.2, 0.8], [-51.2, 51.2, 0.8]],
+                   output_scope=[[-50, 50, 0.5], [-50, 50, 0.5]])   # configs/nuscenes/seg/default.yaml
+
+
+def map_seg_features(seed=0, batch=1, channels=512, height=128, width=128, dtype=torch.float32):
+    """Seeded BEV features [B, C, H, W]: smooth fields (a few low-frequency sinusoids per channel) plus noise, the
+    value range of a decoder neck's ReLU output."""
+    g = torch.Generator().manual_seed(seed)
+    yy = torch.linspace(0, 1, height)[:, None]
+    xx = torch.linspace(0, 1, width)[None, :]
+    f = torch.rand((batch, channels, 3, 3), generator=g) * 6.0
+    ph = torch.rand((batch, channels, 3), generator=g) * 6.3
+    x = torch.zeros((batch, channels, height, width))
+    for k in range(3):
+        x += torch.sin(f[:, :, k, 0, None, None] * xx + f[:, :, k, 1, None, None] * yy + ph[:, :, k, None, None])
+    x = torch.relu(x + 0.3 * torch.randn((batch, channels, height, width), generator=g))
+    return x.to(dtype).contiguous()
+
+
+def map_seg_masks(seed=0, batch=1, height=200, width=200, classes=MAP_CLASSES, dtype=torch.int64):
+    """Seeded BEV map masks [B, K, H, W] with plausible shapes: drivable area as the union of a few straight roads
+    (axis-aligned or slanted bands) and a roundabout disc; pedestrian crossings as striped patches where roads meet
+    the edge of an intersection; walkways as bands along the road borders; stop lines as thin bars across a road;
+    car parks as rectangles off the road; dividers as thin lines along road centres.  Classes beyond these six get
+    random blobs.  dtype int64 is the loader's np.long."""
+    rng = np.random.default_rng(seed)
+    yy, xx = np.mgrid[0:height, 0:width].astype(np.float64)
+    out = np.zeros((batch, len(classes), height, width), np.uint8)
+    for b in range(batch):
+        road = np.zeros((height, width), bool)
+        centre = np.zeros((height, width), bool)
+        walk = np.zeros((height, width), bool)
+        cross = np.zeros((height, width), bool)
+        stop = np.zeros((height, width), bool)
+        for _ in range(rng.integers(2, 5)):
+            ang = rng.choice([0.0, np.pi / 2, rng.uniform(0, np.pi)])
+            off = rng.uniform(-0.35, 0.35) * min(height, width)
+            half = rng.uniform(6, 14)
+            d = (xx - width / 2) * np.sin(ang) - (yy - height / 2) * np.cos(ang) - off
+            along = (xx - width / 2) * np.cos(ang) + (yy - height / 2) * np.sin(ang)
+            road |= np.abs(d) <= half
+            centre |= np.abs(d) <= 0.6
+            walk |= (np.abs(d) > half) & (np.abs(d) <= half + 4)
+            a0 = rng.uniform(-0.3, 0.3) * min(height, width)
+            cross |= (np.abs(d) <= half) & (np.abs(along - a0) <= 4) & ((np.floor(d / 2) % 2) == 0)
+            stop |= (np.abs(d) <= half) & (np.abs(along - a0 - 6) <= 0.75) & (d > 0)
+        cy, cx, r = rng.uniform(0.3, 0.7) * height, rng.uniform(0.3, 0.7) * width, rng.uniform(8, 20)
+        road |= (yy - cy) ** 2 + (xx - cx) ** 2 <= r * r
+        park = np.zeros((height, width), bool)
+        for _ in range(rng.integers(1, 4)):
+            y0, x0 = rng.integers(0, height - 20), rng.integers(0, width - 20)
+            park[y0:y0 + rng.integers(8, 20), x0:x0 + rng.integers(8, 20)] = True
+        park &= ~road
+        shapes = {"drivable_area": road, "ped_crossing": cross, "walkway": walk & ~road, "stop_line": stop,
+                  "carpark_area": park, "divider": centre & road}
+        for k, name in enumerate(classes):
+            m = shapes.get(name)
+            if m is None:
+                y0, x0 = rng.uniform(0, height), rng.uniform(0, width)
+                m = (yy - y0) ** 2 + (xx - x0) ** 2 <= rng.uniform(5, 25) ** 2
+            out[b, k] = m
+    return torch.from_numpy(out).to(dtype)

@@ -758,6 +758,49 @@ BEVB200_API int bevb200_transfusion_loss_backward(
     const double *loss_weights_host, const float *grad_losses, const float *avg_factors, float *g_dense,
     float *g_heatmap, float *g_center, float *g_height, float *g_dim, float *g_rot, float *g_vel, void *stream);
 
+/* ---- BEV map segmentation (BEVSegmentationHead, models/heads/segm/vanilla.py; evaluate_map) ----------------------
+ * Grid transform: dst[p][i][j] = sum_{(r, wy) in rows[i]} wy * sum_{(c, wx) in cols[j]} wx * src[p][r][c] for every
+ * plane p (sample x channel) of NCHW maps, fp32 accumulation, fp32 (half == 0) or fp16 I/O.  rows / cols are CSR
+ * tables (ptr [dst_h + 1] / [dst_w + 1], int32 index, fp32 weight, entries in ascending index order); block b covers
+ * destination rows [b * rows_per_block, ...) and reads source rows [block_lo[b], block_lo[b] + block_rows[b]), which
+ * must hold every row its taps name, block_rows[b] <= max_block_rows.  BEVGridTransform's forward passes the
+ * composite prescale + grid_sample taps (<= 4 per output index; taps outside the input are absent: zeros padding);
+ * its backward passes the transposed tables to map grad_output to grad_input.  One launch; every destination element
+ * is written once (an empty sum is 0), no atomics: reproducible bit for bit.  The tables are built by
+ * bevfusion_b200/map_seg.py.  Shared memory is bevb200_map_grid_smem_bytes(); above 48 KiB gives
+ * BEVB200_EUNSUPPORTED.
+ * Losses, per class k of logits [B, K, H, W] (fp32, or fp16 with logits_half) against target [B, K, H, W]
+ * (target_type BEVB200_MAP_TARGET_*: fp32, uint8 / bool, int64; widened to fp32), evaluated in double:
+ *   ce = (1 - t) x + log(1 + exp(-x))          d ce / dx = (1 - t) p - t (1 - p),  p = sigmoid(x)
+ *   focal (sigmoid_focal_loss, alpha = -1, gamma = 2): m = t (1 - p) + (1 - t) p,  loss = ce m^2,
+ *     d / dx = (d ce / dx) m^2 + 2 ce m (1 - 2t) p (1 - p)
+ *   losses[k] = fp32(sum over B * H * W / (B * H * W)).  Forward: two launches (double partials per workspace slot,
+ *   fixed-order reduce); backward: one launch, grad_logits (logits' dtype) = grad_losses[k] / (B H W) * d / dx.
+ * Counts: for each class k and threshold t, with label = gt != 0 (NaN is a positive label) and pred >= thresholds[t]
+ *   in fp32 (a NaN pred is negative), ADDS tp, fp, fn into int64 counts [3, K, T] (tp at [0], fp [1], fn [2]).
+ *   pred fp32 or fp16 (pred_half), gt as target_type.  One launch; shared-memory counters and one integer atomic
+ *   per counter per CTA: exact and order-independent.  T <= BEVB200_MAP_MAX_THRESHOLDS. */
+#define BEVB200_MAP_TARGET_F32 0
+#define BEVB200_MAP_TARGET_U8 1
+#define BEVB200_MAP_TARGET_I64 2
+#define BEVB200_MAP_MAX_THRESHOLDS 16
+BEVB200_API size_t bevb200_map_grid_smem_bytes(int src_w, int dst_w, int col_nnz, int max_block_rows);
+BEVB200_API int bevb200_map_grid_transform(
+    const void *src, void *dst, int half, long long planes, int src_h, int src_w, int dst_h, int dst_w,
+    const int32_t *row_ptr, const int32_t *row_idx, const float *row_w, const int32_t *col_ptr, const int32_t *col_idx,
+    const float *col_w, int col_nnz, const int32_t *block_lo, const int32_t *block_rows, int rows_per_block,
+    int max_block_rows, void *stream);
+BEVB200_API size_t bevb200_map_seg_loss_workspace_bytes(int B, int K, int H, int W);
+BEVB200_API int bevb200_map_seg_loss(const void *logits, int logits_half, const void *target, int target_type, int B,
+                                     int K, int H, int W, int focal, float *losses, void *workspace,
+                                     size_t workspace_bytes, void *stream);
+BEVB200_API int bevb200_map_seg_loss_backward(const void *logits, int logits_half, const void *target,
+                                              int target_type, int B, int K, int H, int W, int focal,
+                                              const float *grad_losses, void *grad_logits, void *stream);
+BEVB200_API int bevb200_map_seg_counts(const void *pred, int pred_half, const void *gt, int gt_type, int B, int K,
+                                       int H, int W, const float *thresholds_host, int T, int64_t *counts,
+                                       void *stream);
+
 /* ---- LiDAR depth images for the depth-aware camera lift ------------------------------------
  * BaseDepthTransform.forward's per-sample loop (mmdet3d/models/vtransforms/base.py:279-329):
  * undo the lidar augmentation, project every point into every camera with lidar2image, clamp z to
