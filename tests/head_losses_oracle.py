@@ -99,8 +99,9 @@ def centerhead(preds, targets, code_weights, cls=(1.0, 2.0, 4.0), bbox_lw=0.25, 
         num = float(np.float32(np.float32(mask.sum()) + np.float32(1e-4)))
         losses["bbox/task%d" % t] = bbox_lw * s / num
         gfull = np.zeros_like(full)
-        for b in range(B):
-            np.add.at(gfull[b].T, ind[b], gp[b] * bbox_lw / num)
+        for b in range(B):   # sgn * w adds exactly, so cells whose duplicate slots cancel are exactly 0
+            np.add.at(gfull[b].T, ind[b], gp[b])
+        gfull *= bbox_lw / num
         off = 0
         for k, c in maps:
             g[k] = gfull[:, off:off + c].reshape(B, c, H, W)
