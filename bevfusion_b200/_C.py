@@ -139,6 +139,13 @@ _SIGNATURES = {
     "bevb200_encoder_workspace_bytes": (c_size_t, [_P, c_int, c_int, _P]),
     "bevb200_encoder_forward": (c_int, [_P, _P, _P, _P, c_int, _P, c_int, _P, _P, ctypes.c_longlong, _P, _P,
                                         c_size_t, _P, _P]),
+    "bevb200_encoder_train_state_bytes": (c_size_t, [_P, c_int, c_int, _P]),
+    "bevb200_encoder_train_saved": (c_int, [_P, c_int, c_int, _P, c_int, _P, _P]),
+    "bevb200_encoder_forward_train": (c_int, [_P, _P, _P, _P, _P, c_int, _P, c_int, _P, _P, ctypes.c_longlong, _P, _P,
+                                              c_size_t, _P, _P]),
+    "bevb200_encoder_backward_workspace_bytes": (c_size_t, [_P, c_int, c_int, _P]),
+    "bevb200_encoder_backward": (c_int, [_P, _P, _P, c_size_t, c_int, c_int, _P, _P, ctypes.c_longlong, _P, _P, _P,
+                                         _P, _P, c_size_t, _P]),
 }
 
 

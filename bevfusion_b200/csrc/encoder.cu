@@ -97,9 +97,9 @@ struct EWs {
   size_t bytes;
 };
 
-static size_t enc_layout(const bevb200_encoder *e, const std::vector<int> &caps, int batch, void *ws, size_t ws_bytes,
-                         EWs *w) {
-  Arena a(ws, ws_bytes);
+// feature_buffers = false: only the rulebook state (the training state keeps its own per-conv rows)
+static void enc_layout_into(const bevb200_encoder *e, const std::vector<int> &caps, int batch, Arena &a,
+                            bool feature_buffers, EWs *w) {
   const size_t nl = e->levels.size();
   w->sites.resize(nl); w->indices.resize(nl); w->counts.resize(nl);
   // --- region zeroed at the start of every forward: bitmaps, scan state ---
@@ -115,8 +115,9 @@ static size_t enc_layout(const bevb200_encoder *e, const std::vector<int> &caps,
   for (size_t r = 0; r < e->rulebooks.size(); ++r)
     w->nbr[r] = a.take<int32_t>((size_t)e->rulebooks[r].kvol * caps[e->rulebooks[r].level_q]);
   for (int s = 0; s < 2; ++s) {
-    w->split[s].resize(nl);
-    w->f32[s].resize(nl);
+    w->split[s].assign(nl, nullptr);
+    w->f32[s].assign(nl, nullptr);
+    if (!feature_buffers) continue;
     for (size_t l = 0; l < nl; ++l) {
       const size_t row = (size_t)e->levels[l].c_max * 4;
       w->split[s][l] = a.take<uint8_t>((size_t)caps[l] * row);
@@ -124,7 +125,92 @@ static size_t enc_layout(const bevb200_encoder *e, const std::vector<int> &caps,
     }
   }
   w->bytes = a.off;
+}
+
+static size_t enc_layout(const bevb200_encoder *e, const std::vector<int> &caps, int batch, void *ws, size_t ws_bytes,
+                         EWs *w) {
+  Arena a(ws, ws_bytes);
+  enc_layout_into(e, caps, batch, a, true, w);
   return a.off;
+}
+
+// Every rulebook of the plan, on stream ss (forked from st with the plan's events when ss != st): the level-0 count,
+// the site bitmaps, the output rows of the strided convs and the neighbour tables; status_dev[0] / [1 + l] as in
+// bevb200_encoder_forward.  The convs on st wait on events[1 + rulebook] before they read a table.
+static int enc_rulebooks(bevb200_encoder *e, const std::vector<int> &caps, int max_voxels, int batch_size,
+                         const int32_t *coors, const int32_t *n_voxels_dev, int32_t *status_dev, const EWs &w,
+                         cudaStream_t st, cudaStream_t ss) {
+  const bool forked = ss != st;
+  const size_t nl = e->levels.size(), nr = e->rulebooks.size();
+  if (forked) {
+    int dev = 0;
+    BEVB200_CUDA(cudaGetDevice(&dev));
+    if (e->event_device != dev) {
+      for (cudaEvent_t ev : e->events) cudaEventDestroy(ev);
+      e->events.assign(nr + 2, nullptr);
+      for (cudaEvent_t &ev : e->events) BEVB200_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+      e->event_device = dev;
+    }
+    BEVB200_CUDA(cudaEventRecord(e->events[0], st));       // the coordinates are ready
+    BEVB200_CUDA(cudaStreamWaitEvent(ss, e->events[0], 0));
+  }
+  auto geom_of = [&](const ERulebook &rb) {
+    ConvGeom g;
+    for (int d = 0; d < 3; ++d) {
+      g.in_shape[d] = e->levels[rb.level_in].shape[d];
+      g.out_shape[d] = e->levels[rb.level_q].shape[d];
+      g.ksize[d] = rb.ksize[d]; g.stride[d] = rb.stride[d]; g.pad[d] = rb.pad[d]; g.dil[d] = rb.dil[d];
+    }
+    g.batch = batch_size;
+    return g;
+  };
+
+  BEVB200_CUDA(cudaMemsetAsync(w.zero_begin, 0, (size_t)(w.zero_end - w.zero_begin), ss));
+  BEVB200_CUDA(cudaMemsetAsync(status_dev, 0, sizeof(int32_t) * (1 + nl), ss));
+  // level 0: the caller's rows
+  const int32_t *idx0 = coors;
+  if (n_voxels_dev) {
+    BEVB200_CUDA(cudaMemcpyAsync(w.counts[0], n_voxels_dev, sizeof(int32_t), cudaMemcpyDeviceToDevice, ss));
+  } else {
+    BEVB200_LAUNCH(enc_set_count_kernel, 1, 1, 0, ss, w.counts[0], max_voxels);
+  }
+  {
+    ConvGeom g;
+    memset(&g, 0, sizeof(g));
+    for (int d = 0; d < 3; ++d) g.in_shape[d] = e->levels[0].shape[d];
+    g.batch = batch_size;
+    int rc = rb_mark_rows(idx0, caps[0], w.counts[0], g, w.sites[0].cells, ss);
+    if (!rc) rc = rb_scan(w.sites[0], ss);
+    if (!rc) rc = rb_rank2row(idx0, caps[0], w.counts[0], g, w.sites[0].cells, w.rank2row, ss);
+    if (rc) return rc;
+  }
+  std::vector<char> level_ready(nl, 0);
+  level_ready[0] = 1;
+  for (size_t r = 0; r < nr; ++r) {
+    const ERulebook &rb = e->rulebooks[r];
+    const ConvGeom g = geom_of(rb);
+    const size_t lq = rb.level_q, li = rb.level_in;
+    if (!level_ready[lq]) {
+      // a new level: its sites are the outputs of this strided conv
+      const int32_t *idx_in = li == 0 ? idx0 : w.indices[li];
+      int rc = rb_mark_outputs(idx_in, caps[li], w.counts[li], g, w.sites[lq].cells, ss);
+      if (!rc) rc = rb_scan(w.sites[lq], ss);
+      if (!rc) rc = rb_count(w.sites[lq].total, caps[lq], w.counts[lq], status_dev, ss);
+      if (!rc) rc = rb_out_indices(w.sites[lq], e->levels[lq].shape, caps[lq], w.indices[lq], ss);
+      if (rc) return rc;
+      level_ready[lq] = 1;
+    }
+    const int32_t *qidx = lq == 0 ? idx0 : w.indices[lq];
+    int rc = rb_gather(qidx, caps[lq], w.counts[lq], g, w.sites[li].cells, li == 0 ? w.rank2row : nullptr, caps[li],
+                       w.nbr[r], (long long)caps[lq], ss);
+    if (rc) return rc;
+    if (forked) BEVB200_CUDA(cudaEventRecord(e->events[1 + r], ss));
+  }
+  // row counts for the caller: status[1 + l]
+  for (size_t l = 0; l < nl; ++l)
+    BEVB200_CUDA(cudaMemcpyAsync(status_dev + 1 + l, w.counts[l], sizeof(int32_t), cudaMemcpyDeviceToDevice, ss));
+  if (forked) BEVB200_CUDA(cudaEventRecord(e->events[1 + nr], ss));
+  return BEVB200_OK;
 }
 
 }  // namespace bevb200
@@ -299,79 +385,14 @@ int bevb200_encoder_forward(bevb200_encoder_t *e, const void *params, const floa
     return BEVB200_EWORKSPACE;
   }
   const size_t nl = e->levels.size(), nr = e->rulebooks.size();
-  if (forked) {
-    int dev = 0;
-    BEVB200_CUDA(cudaGetDevice(&dev));
-    if (e->event_device != dev) {
-      for (cudaEvent_t ev : e->events) cudaEventDestroy(ev);
-      e->events.assign(nr + 2, nullptr);
-      for (cudaEvent_t &ev : e->events) BEVB200_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-      e->event_device = dev;
-    }
-    BEVB200_CUDA(cudaEventRecord(e->events[0], st));       // the coordinates are ready
-    BEVB200_CUDA(cudaStreamWaitEvent(ss, e->events[0], 0));
-  }
   const char *pbase = (const char *)params;
-  auto geom_of = [&](const ERulebook &rb) {
-    ConvGeom g;
-    for (int d = 0; d < 3; ++d) {
-      g.in_shape[d] = e->levels[rb.level_in].shape[d];
-      g.out_shape[d] = e->levels[rb.level_q].shape[d];
-      g.ksize[d] = rb.ksize[d]; g.stride[d] = rb.stride[d]; g.pad[d] = rb.pad[d]; g.dil[d] = rb.dil[d];
-    }
-    g.batch = batch_size;
-    return g;
-  };
-
-  // ------------------------------ rulebooks (stream ss) ------------------------------------
-  BEVB200_CUDA(cudaMemsetAsync(w.zero_begin, 0, (size_t)(w.zero_end - w.zero_begin), ss));
-  BEVB200_CUDA(cudaMemsetAsync(status_dev, 0, sizeof(int32_t) * (1 + nl), ss));
-  // level 0: the caller's rows
   const int32_t *idx0 = coors;
-  if (n_voxels_dev) {
-    BEVB200_CUDA(cudaMemcpyAsync(w.counts[0], n_voxels_dev, sizeof(int32_t), cudaMemcpyDeviceToDevice, ss));
-  } else {
-    BEVB200_LAUNCH(enc_set_count_kernel, 1, 1, 0, ss, w.counts[0], max_voxels);
-  }
-  {
-    ConvGeom g;
-    memset(&g, 0, sizeof(g));
-    for (int d = 0; d < 3; ++d) g.in_shape[d] = e->levels[0].shape[d];
-    g.batch = batch_size;
-    int rc = rb_mark_rows(idx0, caps[0], w.counts[0], g, w.sites[0].cells, ss);
-    if (!rc) rc = rb_scan(w.sites[0], ss);
-    if (!rc) rc = rb_rank2row(idx0, caps[0], w.counts[0], g, w.sites[0].cells, w.rank2row, ss);
-    if (rc) return rc;
-  }
-  std::vector<char> level_ready(nl, 0);
-  level_ready[0] = 1;
-  for (size_t r = 0; r < nr; ++r) {
-    const ERulebook &rb = e->rulebooks[r];
-    const ConvGeom g = geom_of(rb);
-    const size_t lq = rb.level_q, li = rb.level_in;
-    if (!level_ready[lq]) {
-      // a new level: its sites are the outputs of this strided conv
-      const int32_t *idx_in = li == 0 ? idx0 : w.indices[li];
-      int rc = rb_mark_outputs(idx_in, caps[li], w.counts[li], g, w.sites[lq].cells, ss);
-      if (!rc) rc = rb_scan(w.sites[lq], ss);
-      if (!rc) rc = rb_count(w.sites[lq].total, caps[lq], w.counts[lq], status_dev, ss);
-      if (!rc) rc = rb_out_indices(w.sites[lq], e->levels[lq].shape, caps[lq], w.indices[lq], ss);
-      if (rc) return rc;
-      level_ready[lq] = 1;
-    }
-    const int32_t *qidx = lq == 0 ? idx0 : w.indices[lq];
-    int rc = rb_gather(qidx, caps[lq], w.counts[lq], g, w.sites[li].cells, li == 0 ? w.rank2row : nullptr, caps[li],
-                       w.nbr[r], (long long)caps[lq], ss);
-    if (rc) return rc;
-    if (forked) BEVB200_CUDA(cudaEventRecord(e->events[1 + r], ss));
-  }
-  // row counts for the caller: status[1 + l]
-  for (size_t l = 0; l < nl; ++l)
-    BEVB200_CUDA(cudaMemcpyAsync(status_dev + 1 + l, w.counts[l], sizeof(int32_t), cudaMemcpyDeviceToDevice, ss));
-  if (forked) BEVB200_CUDA(cudaEventRecord(e->events[1 + nr], ss));
+  // ------------------------------ rulebooks (stream ss) ------------------------------------
+  int rc = enc_rulebooks(e, caps, max_voxels, batch_size, coors, n_voxels_dev, status_dev, w, st, ss);
+  if (rc) return rc;
 
   // ------------------------------ features (stream st) -------------------------------------
-  int rc = spconv_v6_split_rows(voxel_features, caps[0], n_voxels_dev, e->in_channels, e->c0_eff, w.split[0][0], st);
+  rc = spconv_v6_split_rows(voxel_features, caps[0], n_voxels_dev, e->in_channels, e->c0_eff, w.split[0][0], st);
   if (rc) return rc;
   std::vector<int> split_turn(nl, 0), f32_turn(nl, 0);
   split_turn[0] = 1;
@@ -420,6 +441,591 @@ int bevb200_encoder_forward(bevb200_encoder_t *e, const void *params, const floa
                        batch_size, e->levels[ll].shape, 1, out_batch_stride, dense_out, st);
   if (rc) return rc;
   if (forked) BEVB200_CUDA(cudaStreamWaitEvent(st, e->events[1 + nr], 0));   // join (also what a graph capture needs)
+  return BEVB200_OK;
+}
+
+}  // extern "C"
+
+// ================================== training ====================================================
+// forward_train: rulebooks as above, then per conv
+//   conv (no epilogue) -> z fp32 | stats partials (double, fixed 2048-row chunks) | stats reduce (mean, invstd,
+//   scale = gamma invstd, shift = beta - mean scale; running statistics) | apply y = relu(z scale + shift [+ y_res])
+//   into the split image the next conv gathers (and the backward reads again).
+// backward, in reverse conv order, on the same tables:
+//   ReLU mask + BN sums (double partials of g and g x^, fixed order) | reduce (dgamma, dbeta) | dz |
+//   filter gradient on the saved input image (spconv_wgrad_tc_split) | input gradient = the forward kernel on W^T:
+//   SubM: the forward table with mirrored offsets, strided: a transposed table; a block's identity gradient rides in
+//   the residual epilogue of the input gradient of the conv that reads the identity.
+#include "tc_ptx.cuh"
+
+namespace bevb200 {
+
+constexpr int kStatRows = 2048;   // rows per partial of the BN sums
+constexpr int kStatThreads = 256;
+
+static int stat_chunks(int cap) { return cap > 0 ? (cap + kStatRows - 1) / kStatRows : 1; }
+
+__device__ __forceinline__ int enc_rows(const int32_t *n_dev, int cap) { return min(max(__ldg(n_dev), 0), cap); }
+
+// value of channel ch of row r of a split image with c channels per row
+__device__ __forceinline__ float split_value(const uint8_t *img, long long r, int c, int ch) {
+  const uint8_t *p = img + r * (c * 4) + (ch >> 4) * 64 + (ch & 15) * 2;
+  const uint32_t h = *reinterpret_cast<const uint16_t *>(p), l = *reinterpret_cast<const uint16_t *>(p + 32);
+  return __uint_as_float(h << 16) + __uint_as_float(l << 16);
+}
+
+// thread (group g, channel ch) of a 256-thread block over c channels: c <= 128, so >= 2 groups
+#define STAT_THREAD(c)                                 \
+  const int groups = kStatThreads / (c);               \
+  const int ch = threadIdx.x % (c), grp = threadIdx.x / (c)
+
+// per-channel sums of v and v^2 (double) over the rows of one chunk; the groups add in ascending order
+__global__ void __launch_bounds__(kStatThreads)
+    bn_stats_partial_kernel(const float *__restrict__ z, const int32_t *__restrict__ n_dev, int cap, int c,
+                            double *__restrict__ partial) {
+  __shared__ double sh[2][kStatThreads];
+  STAT_THREAD(c);
+  const int n = enc_rows(n_dev, cap);
+  const int r0 = blockIdx.x * kStatRows, r1 = min(n, r0 + kStatRows);
+  if (r0 >= n) return;                           // chunks past the count are never read
+  double s = 0.0, ss = 0.0;
+  if (grp < groups)
+    for (int r = r0 + grp; r < r1; r += groups) {
+      const double v = z[(long long)r * c + ch];
+      s += v;
+      ss += v * v;
+    }
+  sh[0][threadIdx.x] = s;
+  sh[1][threadIdx.x] = ss;
+  __syncthreads();
+  if (threadIdx.x < c) {
+    for (int q = 1; q < groups; ++q) { s += sh[0][q * c + ch]; ss += sh[1][q * c + ch]; }
+    partial[(long long)blockIdx.x * 2 * c + ch] = s;
+    partial[(long long)blockIdx.x * 2 * c + c + ch] = ss;
+  }
+}
+
+// sums of the partials of the chunks that hold rows, in a fixed order; thread ch < c returns its channel's two sums
+__device__ __forceinline__ void stat_sums(const double *__restrict__ partial, int n, int c, double *sh, double &s,
+                                          double &ss) {
+  STAT_THREAD(c);
+  const int chunks = (n + kStatRows - 1) / kStatRows;
+  s = 0.0; ss = 0.0;
+  if (grp < groups)
+    for (int k = grp; k < chunks; k += groups) {
+      s += partial[(long long)k * 2 * c + ch];
+      ss += partial[(long long)k * 2 * c + c + ch];
+    }
+  sh[threadIdx.x] = s;
+  sh[kStatThreads + threadIdx.x] = ss;
+  __syncthreads();
+  if (threadIdx.x < c)
+    for (int q = 1; q < groups; ++q) { s += sh[q * c + ch]; ss += sh[kStatThreads + q * c + ch]; }
+}
+
+// batch statistics -> stat [mean | invstd | scale | shift] and the running statistics (torch's BatchNorm1d, train)
+__global__ void __launch_bounds__(kStatThreads)
+    bn_stats_reduce_kernel(const double *__restrict__ partial, const int32_t *__restrict__ n_dev, int cap, int c,
+                           bevb200_encoder_bn_t bn, float *__restrict__ stat, int32_t *__restrict__ status) {
+  __shared__ double sh[2 * kStatThreads];
+  const int n = enc_rows(n_dev, cap);
+  double s, ss;
+  stat_sums(partial, n, c, sh, s, ss);
+  const int ch = threadIdx.x;
+  if (ch >= c) return;
+  const double mean = n > 0 ? s / n : 0.0;
+  const double var = n > 0 ? fmax(ss / n - mean * mean, 0.0) : 0.0;    // biased: the normalisation's
+  const double invstd = 1.0 / sqrt(var + (double)bn.eps);
+  const double scale = (double)bn.weight[ch] * invstd;
+  stat[ch] = (float)mean;
+  stat[c + ch] = (float)invstd;
+  stat[2 * c + ch] = (float)scale;
+  stat[3 * c + ch] = (float)((double)bn.bias[ch] - mean * scale);
+  if (n >= 2) {
+    const double m = bn.momentum;
+    bn.running_mean[ch] = (float)((1.0 - m) * bn.running_mean[ch] + m * mean);
+    bn.running_var[ch] = (float)((1.0 - m) * bn.running_var[ch] + m * var * n / (n - 1.0));
+    if (ch == 0 && bn.num_batches_tracked) *bn.num_batches_tracked += 1;
+  } else if (ch == 0) {
+    atomicOr(status, BEVB200_ENCODER_FEW_ROWS);
+  }
+}
+
+// y = relu(z scale + shift [+ residual image]) -> split image (and fp32 rows); one thread per (row, 8 channels)
+__global__ void bn_apply_kernel(const float *__restrict__ z, const float *__restrict__ stat,
+                                const uint8_t *__restrict__ res_split, const int32_t *__restrict__ n_dev, int cap,
+                                int c, int relu, uint8_t *__restrict__ ysplit, float *__restrict__ yf32) {
+  const int n = enc_rows(n_dev, cap);
+  const int per_row = c >> 3;
+  const long long total = (long long)n * per_row;
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total;
+       t += (long long)gridDim.x * blockDim.x) {
+    const int j = (int)(t % per_row), c0 = 8 * j;
+    const long long r = t / per_row;
+    const float4 a = *reinterpret_cast<const float4 *>(z + r * c + c0);
+    const float4 b = *reinterpret_cast<const float4 *>(z + r * c + c0 + 4);
+    float y[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+#pragma unroll
+    for (int e = 0; e < 8; ++e) y[e] = y[e] * __ldg(stat + 2 * c + c0 + e) + __ldg(stat + 3 * c + c0 + e);
+    if (res_split) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) y[e] += split_value(res_split, r, c, c0 + e);
+    }
+    if (relu) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) y[e] = fmaxf(y[e], 0.f);
+    }
+    if (yf32) {
+      *reinterpret_cast<float4 *>(yf32 + r * c + c0) = make_float4(y[0], y[1], y[2], y[3]);
+      *reinterpret_cast<float4 *>(yf32 + r * c + c0 + 4) = make_float4(y[4], y[5], y[6], y[7]);
+    }
+    uint32_t hi[4], lo[4];
+#pragma unroll
+    for (int e = 0; e < 8; e += 2) split_pair(y[e], y[e + 1], hi[e / 2], lo[e / 2]);
+    uint8_t *dst = ysplit + r * (c * 4) + (j >> 1) * 64 + (j & 1) * 16;
+    *reinterpret_cast<uint4 *>(dst) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+    *reinterpret_cast<uint4 *>(dst + 32) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+  }
+}
+
+// rows of the last level from the dense gradient (the inverse of sparse_to_dense with z_major)
+__global__ void dense_gather_kernel(const float *__restrict__ dense, const int32_t *__restrict__ idx,
+                                    const int32_t *__restrict__ n_dev, int cap, int c, int batch, int X, int Y, int Z,
+                                    long long out_batch_stride, float *__restrict__ rows) {
+  const int n = enc_rows(n_dev, cap);
+  const long long total = (long long)n * c, plane = (long long)X * Y * Z;
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total;
+       t += (long long)gridDim.x * blockDim.x) {
+    const int i = (int)(t % n), ch = (int)(t / n);
+    const int4 p = *reinterpret_cast<const int4 *>(idx + 4ll * i);
+    float v = 0.f;
+    if ((unsigned)p.x < (unsigned)batch && (unsigned)p.y < (unsigned)X && (unsigned)p.z < (unsigned)Y &&
+        (unsigned)p.w < (unsigned)Z)
+      v = dense[p.x * out_batch_stride + ch * plane + ((long long)p.w * X + p.y) * Y + p.z];
+    rows[(long long)i * c + ch] = v;
+  }
+}
+
+// ReLU mask applied to g in place, then per-channel sums of g and g x^ (x^ = (z - mean) invstd) per chunk
+__global__ void __launch_bounds__(kStatThreads)
+    bn_bwd_partial_kernel(float *__restrict__ g, const uint8_t *__restrict__ ysplit, const float *__restrict__ yf32,
+                          int relu, const float *__restrict__ z, const float *__restrict__ stat,
+                          const int32_t *__restrict__ n_dev, int cap, int c, double *__restrict__ partial) {
+  __shared__ double sh[2][kStatThreads];
+  STAT_THREAD(c);
+  const int n = enc_rows(n_dev, cap);
+  const int r0 = blockIdx.x * kStatRows, r1 = min(n, r0 + kStatRows);
+  if (r0 >= n) return;
+  double s = 0.0, sx = 0.0;
+  if (grp < groups) {
+    const float mean = stat[ch], invstd = stat[c + ch];
+    for (int r = r0 + grp; r < r1; r += groups) {
+      const long long e = (long long)r * c + ch;
+      float gv = g[e];
+      if (relu) {
+        const float y = yf32 ? yf32[e] : split_value(ysplit, r, c, ch);
+        if (!(y > 0.f)) gv = 0.f;
+        g[e] = gv;
+      }
+      s += gv;
+      sx += (double)gv * (double)((z[e] - mean) * invstd);
+    }
+  }
+  sh[0][threadIdx.x] = s;
+  sh[1][threadIdx.x] = sx;
+  __syncthreads();
+  if (threadIdx.x < c) {
+    for (int q = 1; q < groups; ++q) { s += sh[0][q * c + ch]; sx += sh[1][q * c + ch]; }
+    partial[(long long)blockIdx.x * 2 * c + ch] = s;
+    partial[(long long)blockIdx.x * 2 * c + c + ch] = sx;
+  }
+}
+
+// dbeta = sum g, dgamma = sum g x^; coef = [sum g / n | sum g x^ / n]
+__global__ void __launch_bounds__(kStatThreads)
+    bn_bwd_reduce_kernel(const double *__restrict__ partial, const int32_t *__restrict__ n_dev, int cap, int c,
+                         float *__restrict__ dgamma, float *__restrict__ dbeta, float *__restrict__ coef) {
+  __shared__ double sh[2 * kStatThreads];
+  const int n = enc_rows(n_dev, cap);
+  double s, sx;
+  stat_sums(partial, n, c, sh, s, sx);
+  const int ch = threadIdx.x;
+  if (ch >= c) return;
+  dbeta[ch] = (float)s;
+  dgamma[ch] = (float)sx;
+  coef[ch] = n > 0 ? (float)(s / n) : 0.f;
+  coef[c + ch] = n > 0 ? (float)(sx / n) : 0.f;
+}
+
+// dz = gamma invstd (g - mean(g) - x^ mean(g x^))
+__global__ void bn_bwd_apply_kernel(const float *__restrict__ g, const float *__restrict__ z,
+                                    const float *__restrict__ stat, const float *__restrict__ coef,
+                                    const int32_t *__restrict__ n_dev, int cap, int c, float *__restrict__ dz) {
+  const int n = enc_rows(n_dev, cap);
+  const long long total = (long long)n * c;
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total;
+       t += (long long)gridDim.x * blockDim.x) {
+    const int ch = (int)(t % c);
+    const float xh = (z[t] - __ldg(stat + ch)) * __ldg(stat + c + ch);
+    dz[t] = __ldg(stat + 2 * c + ch) * (g[t] - __ldg(coef + ch) - xh * __ldg(coef + c + ch));
+  }
+}
+
+// wt[k][co][ci] = w[mirror ? K-1-k : k][ci][co], ci zero padded to ci_pad
+__global__ void enc_weight_t_kernel(const float *__restrict__ w, int kvol, int c_in, int c_out, int ci_pad, int mirror,
+                                    float *__restrict__ wt) {
+  const long long total = (long long)kvol * c_out * ci_pad;
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total;
+       t += (long long)gridDim.x * blockDim.x) {
+    const int ci = (int)(t % ci_pad), co = (int)((t / ci_pad) % c_out), k = (int)(t / ((long long)ci_pad * c_out));
+    const int ks = mirror ? kvol - 1 - k : k;
+    wt[t] = ci < c_in ? w[((long long)ks * c_in + ci) * c_out + co] : 0.f;
+  }
+}
+
+// nbr_t[k][j] = -1 for the valid input rows j, then nbr_t[k][nbr[k][o]] = o for the valid output rows o
+__global__ void enc_nbr_t_fill_kernel(const int32_t *__restrict__ n_in_dev, int cap_in, int kvol,
+                                      int32_t *__restrict__ nbr_t) {
+  const int n = enc_rows(n_in_dev, cap_in);
+  const long long total = (long long)kvol * n;
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total;
+       t += (long long)gridDim.x * blockDim.x)
+    nbr_t[(t / n) * cap_in + t % n] = -1;
+}
+__global__ void enc_nbr_t_scatter_kernel(const int32_t *__restrict__ nbr, const int32_t *__restrict__ n_out_dev,
+                                         int cap_out, const int32_t *__restrict__ n_in_dev, int cap_in, int kvol,
+                                         int32_t *__restrict__ nbr_t) {
+  const int n = enc_rows(n_out_dev, cap_out), n_in = enc_rows(n_in_dev, cap_in);
+  const long long total = (long long)kvol * n;
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total;
+       t += (long long)gridDim.x * blockDim.x) {
+    const long long k = t / n;
+    const int o = (int)(t % n);
+    const int j = nbr[k * cap_out + o];
+    if (j >= 0 && j < n_in) nbr_t[k * cap_in + j] = o;   // one writer per (k, j)
+  }
+}
+
+// split image rows of c_src channels -> rows of c_dst >= c_src channels (zero padded), for the filter gradient
+__global__ void enc_widen_image_kernel(const uint8_t *__restrict__ src, int c_src, int c_dst,
+                                       const int32_t *__restrict__ n_dev, int cap, uint8_t *__restrict__ dst) {
+  const int n = enc_rows(n_dev, cap);
+  const int per_row = c_dst / 4;   // 16-byte chunks
+  const long long total = (long long)n * per_row;
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total;
+       t += (long long)gridDim.x * blockDim.x) {
+    const long long r = t / per_row;
+    const int q = (int)(t % per_row);
+    const uint4 v = q < c_src / 4 ? *reinterpret_cast<const uint4 *>(src + r * c_src * 4 + 16 * q) : make_uint4(0, 0, 0, 0);
+    *reinterpret_cast<uint4 *>(dst + r * c_dst * 4 + 16 * q) = v;
+  }
+}
+
+// input gradient rows [cap, c_eff] -> grad_voxel_features [rows, c_in]: the valid rows narrowed, the rest zero
+__global__ void enc_narrow_grad_kernel(const float *__restrict__ src, int c_eff, const int32_t *__restrict__ n_dev,
+                                       int cap, int rows, int c_in, float *__restrict__ dst) {
+  const int n = enc_rows(n_dev, cap);
+  const long long total = (long long)rows * c_in;
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total;
+       t += (long long)gridDim.x * blockDim.x) {
+    const long long r = t / c_in;
+    dst[t] = r < n ? src[r * c_eff + t % c_in] : 0.f;
+  }
+}
+
+// ---- state and workspace layouts ----
+struct ETrain {
+  EWs w;
+  char *params;
+  uint8_t *in_split;              // level-0 split image of the voxel features
+  std::vector<float *> z;         // pre-BN rows per conv
+  std::vector<uint8_t *> y;       // split image of every conv's output
+  std::vector<float *> stat;      // per conv [mean | invstd | scale | shift][c_out]
+  float *y_last;                  // fp32 rows of the last conv (dense() and its ReLU mask)
+  double *partial;
+};
+
+static size_t train_layout(const bevb200_encoder *e, const std::vector<int> &caps, int batch, void *base,
+                           size_t bytes, ETrain *t) {
+  Arena a(base, bytes);
+  enc_layout_into(e, caps, batch, a, false, &t->w);
+  t->params = a.take<char>(e->param_bytes);
+  t->in_split = a.take<uint8_t>((size_t)caps[0] * e->c0_eff * 4);
+  const size_t n = e->convs.size();
+  t->z.resize(n); t->y.resize(n); t->stat.resize(n);
+  size_t part = 0;
+  for (size_t i = 0; i < n; ++i) {
+    const EConv &cv = e->convs[i];
+    const size_t cap = caps[cv.level_out];
+    t->z[i] = a.take<float>(cap * cv.d.c_out);
+    t->y[i] = a.take<uint8_t>(cap * cv.d.c_out * 4);
+    t->stat[i] = a.take<float>(4 * (size_t)cv.d.c_out);
+    part = std::max(part, (size_t)stat_chunks(caps[cv.level_out]) * 2 * cv.d.c_out);
+  }
+  t->y_last = a.take<float>((size_t)caps.back() * e->convs.back().d.c_out);
+  t->partial = a.take<double>(part);
+  return a.off;
+}
+
+struct EBwd {
+  std::vector<float *> d[2], dz;  // per level: two gradient row buffers and the dz rows
+  int32_t *nbr_t;
+  float *wt, *coef, *din0;
+  char *packed, *wg;
+  uint8_t *fwide, *g16;
+  double *partial;
+};
+
+static size_t bwd_layout(const bevb200_encoder *e, const std::vector<int> &caps, void *base, size_t bytes, EBwd *b) {
+  Arena a(base, bytes);
+  const size_t nl = e->levels.size();
+  for (int s = 0; s < 2; ++s) b->d[s].resize(nl);
+  b->dz.resize(nl);
+  for (size_t l = 0; l < nl; ++l) {
+    const size_t n = (size_t)caps[l] * e->levels[l].c_max;
+    b->d[0][l] = a.take<float>(n);
+    b->d[1][l] = a.take<float>(n);
+    b->dz[l] = a.take<float>(n);
+  }
+  size_t nbrt = 0, wt = 0, pk = 0, wg = 0, fw = 0, g16 = 0, part = 0, cmax = 0;
+  for (const EConv &cv : e->convs) {
+    const int li = cv.level_in, lo = cv.level_out, cip = spconv_v6_cin_eff(cv.d.c_in);
+    if (!cv.d.subm) nbrt = std::max(nbrt, (size_t)cv.kvol * caps[li]);
+    wt = std::max(wt, (size_t)cv.kvol * cv.d.c_out * cip);
+    pk = std::max(pk, spconv_v6_packed_bytes(cv.d.c_out, cip, cv.kvol));
+    wg = std::max(wg, spconv_wgrad_tc_split_workspace_bytes(caps[lo], cv.d.c_in, cv.d.c_out, cv.kvol));
+    const int wide = spconv_wgrad_tc_image_channels(cv.d.c_in);
+    if (wide != cip) fw = std::max(fw, (size_t)caps[li] * wide * 4);
+    if (cv.d.c_out == 16) g16 = std::max(g16, (size_t)caps[lo] * 64);
+    part = std::max(part, (size_t)stat_chunks(caps[lo]) * 2 * cv.d.c_out);
+    cmax = std::max(cmax, (size_t)cv.d.c_out);
+  }
+  b->nbr_t = a.take<int32_t>(nbrt);
+  b->wt = a.take<float>(wt);
+  b->packed = a.take<char>(pk);
+  b->wg = a.take<char>(wg);
+  b->fwide = a.take<uint8_t>(fw);
+  b->g16 = a.take<uint8_t>(g16);
+  b->din0 = a.take<float>((size_t)caps[0] * e->c0_eff);
+  b->coef = a.take<float>(2 * cmax);
+  b->partial = a.take<double>(part);
+  return a.off;
+}
+
+}  // namespace bevb200
+
+extern "C" {
+
+size_t bevb200_encoder_train_state_bytes(const bevb200_encoder_t *e, int max_voxels, int batch_size,
+                                         const int32_t *user_caps) {
+  if (!e || max_voxels <= 0 || batch_size <= 0) return 0;
+  std::vector<int> caps;
+  level_caps(e, max_voxels, batch_size, user_caps, &caps);
+  ETrain t;
+  return train_layout(e, caps, batch_size, nullptr, 0, &t);
+}
+
+int bevb200_encoder_train_saved(const bevb200_encoder_t *e, int max_voxels, int batch_size, const int32_t *user_caps,
+                                int conv, size_t *pre_bn_offset, size_t *out_image_offset) {
+  BEVB200_REQUIRE(e && max_voxels > 0 && batch_size > 0 && pre_bn_offset && out_image_offset, "bad argument");
+  BEVB200_REQUIRE(conv >= 0 && conv < (int)e->convs.size(), "bad conv index");
+  std::vector<int> caps;
+  level_caps(e, max_voxels, batch_size, user_caps, &caps);
+  // laid out from a stand-in base: every offset is pointer - base
+  char *const base = (char *)(uintptr_t)4096;
+  ETrain o;
+  train_layout(e, caps, batch_size, base, 0, &o);
+  *pre_bn_offset = (size_t)((char *)o.z[conv] - base);
+  *out_image_offset = (size_t)((char *)o.y[conv] - base);
+  return BEVB200_OK;
+}
+
+int bevb200_encoder_forward_train(bevb200_encoder_t *e, const float *const *weights, const bevb200_encoder_bn_t *bn,
+                                  const float *voxel_features, const int32_t *coors, int max_voxels,
+                                  const int32_t *n_voxels_dev, int batch_size, const int32_t *user_caps,
+                                  float *dense_out, long long out_batch_stride, int32_t *status_dev, void *state,
+                                  size_t state_bytes, void *stream, void *rulebook_stream) {
+  BEVB200_REQUIRE(e && weights && bn && dense_out && status_dev && max_voxels > 0 && batch_size > 0, "bad argument");
+  BEVB200_REQUIRE(voxel_features && coors, "null input");
+  const size_t nc = e->convs.size();
+  for (size_t i = 0; i < nc; ++i)
+    BEVB200_REQUIRE(weights[i] && bn[i].weight && bn[i].bias && bn[i].running_mean && bn[i].running_var,
+                    "null conv weight / BN tensor");
+  cudaStream_t st = (cudaStream_t)stream, ss = rulebook_stream ? (cudaStream_t)rulebook_stream : st;
+  const bool forked = ss != st;
+  std::vector<int> caps;
+  level_caps(e, max_voxels, batch_size, user_caps, &caps);
+  ETrain t;
+  const size_t need = train_layout(e, caps, batch_size, state, state_bytes, &t);
+  if (state == nullptr || state_bytes < need) {
+    snprintf(g_last_error, sizeof(g_last_error), "encoder_forward_train: state too small (%zu < %zu)", state_bytes, need);
+    return BEVB200_EWORKSPACE;
+  }
+  const size_t nl = e->levels.size(), nr = e->rulebooks.size();
+  const EWs &w = t.w;
+  int rc = enc_rulebooks(e, caps, max_voxels, batch_size, coors, n_voxels_dev, status_dev, w, st, ss);
+  if (rc) return rc;
+  // the live weights, packed on every call (a graph replay after an in-place optimizer step sees the new values)
+  for (size_t i = 0; i < nc; ++i) {
+    const EConv &cv = e->convs[i];
+    rc = spconv_v6_pack_weights(weights[i], cv.d.c_in, cv.d.c_out, cv.kvol, t.params + cv.packed_off, st);
+    if (rc) return rc;
+  }
+  rc = spconv_v6_split_rows(voxel_features, caps[0], n_voxels_dev, e->in_channels, e->c0_eff, t.in_split, st);
+  if (rc) return rc;
+  std::vector<char> rb_waited(nr, 0);
+  const uint8_t *cur = t.in_split;
+  for (size_t i = 0; i < nc; ++i) {
+    const EConv &cv = e->convs[i];
+    if (forked && !rb_waited[cv.rulebook]) {
+      BEVB200_CUDA(cudaStreamWaitEvent(st, e->events[1 + cv.rulebook], 0));
+      rb_waited[cv.rulebook] = 1;
+    }
+    const int lo = cv.level_out, c = cv.d.c_out;
+    const bool last = i + 1 == nc;
+    rc = spconv_v6_forward(cur, t.params + cv.packed_off, w.nbr[cv.rulebook], (long long)caps[lo], caps[cv.level_in],
+                           caps[lo], w.counts[lo], cv.c_in_eff, c, cv.kvol, nullptr, nullptr, nullptr, nullptr, 0,
+                           t.z[i], nullptr, st);
+    if (rc) return rc;
+    BEVB200_LAUNCH(bn_stats_partial_kernel, stat_chunks(caps[lo]), kStatThreads, 0, st, t.z[i], w.counts[lo], caps[lo],
+                   c, t.partial);
+    BEVB200_LAUNCH(bn_stats_reduce_kernel, 1, kStatThreads, 0, st, t.partial, w.counts[lo], caps[lo], c, bn[i],
+                   t.stat[i], status_dev);
+    BEVB200_LAUNCH(bn_apply_kernel, grid_for((long long)caps[lo] * (c / 8), 256), 256, 0, st, t.z[i], t.stat[i],
+                   cv.d.residual_from >= 0 ? t.y[cv.d.residual_from] : nullptr, w.counts[lo], caps[lo], c, cv.d.relu,
+                   t.y[i], last ? t.y_last : nullptr);
+    cur = t.y[i];
+  }
+  const size_t ll = nl - 1;
+  rc = sparse_to_dense(t.y_last, w.indices[ll] ? w.indices[ll] : coors, caps[ll], w.counts[ll], e->convs.back().d.c_out,
+                       batch_size, e->levels[ll].shape, 1, out_batch_stride, dense_out, st);
+  if (rc) return rc;
+  if (forked) BEVB200_CUDA(cudaStreamWaitEvent(st, e->events[1 + nr], 0));
+  return BEVB200_OK;
+}
+
+size_t bevb200_encoder_backward_workspace_bytes(const bevb200_encoder_t *e, int max_voxels, int batch_size,
+                                                const int32_t *user_caps) {
+  if (!e || max_voxels <= 0 || batch_size <= 0) return 0;
+  std::vector<int> caps;
+  level_caps(e, max_voxels, batch_size, user_caps, &caps);
+  EBwd b;
+  return bwd_layout(e, caps, nullptr, 0, &b);
+}
+
+int bevb200_encoder_backward(const bevb200_encoder_t *e, const float *const *weights, const void *state,
+                             size_t state_bytes, int max_voxels, int batch_size, const int32_t *user_caps,
+                             const float *grad_dense, long long out_batch_stride, float *grad_voxel_features,
+                             float *const *grad_weights, float *const *grad_bn_weight, float *const *grad_bn_bias,
+                             void *workspace, size_t workspace_bytes, void *stream) {
+  BEVB200_REQUIRE(e && weights && state && grad_dense && grad_weights && grad_bn_weight && grad_bn_bias &&
+                      max_voxels > 0 && batch_size > 0, "bad argument");
+  const size_t nc = e->convs.size(), nl = e->levels.size();
+  for (size_t i = 0; i < nc; ++i)
+    BEVB200_REQUIRE(weights[i] && grad_weights[i] && grad_bn_weight[i] && grad_bn_bias[i], "null conv / BN tensor");
+  cudaStream_t st = (cudaStream_t)stream;
+  std::vector<int> caps;
+  level_caps(e, max_voxels, batch_size, user_caps, &caps);
+  ETrain t;
+  const size_t need_state = train_layout(e, caps, batch_size, (void *)state, state_bytes, &t);
+  BEVB200_REQUIRE(state_bytes >= need_state, "state smaller than train_state_bytes");
+  EBwd b;
+  const size_t need = bwd_layout(e, caps, workspace, workspace_bytes, &b);
+  if (workspace == nullptr || workspace_bytes < need) {
+    snprintf(g_last_error, sizeof(g_last_error), "encoder_backward: workspace too small (%zu < %zu)", workspace_bytes, need);
+    return BEVB200_EWORKSPACE;
+  }
+  const EWs &w = t.w;
+  if (out_batch_stride == 0) {
+    const int *s = e->levels.back().shape;
+    out_batch_stride = (long long)e->convs.back().d.c_out * s[0] * s[1] * s[2];
+  }
+  // the last level's rows from the dense gradient
+  const size_t ll = nl - 1;
+  BEVB200_REQUIRE(ll > 0, "a plan without a strided conv has no training path");
+  {
+    const int *s = e->levels[ll].shape;
+    const int c = e->convs.back().d.c_out;
+    BEVB200_LAUNCH(dense_gather_kernel, grid_for((long long)caps[ll] * c, 256), 256, 0, st, grad_dense, w.indices[ll],
+                   w.counts[ll], caps[ll], c, batch_size, s[0], s[1], s[2], out_batch_stride, b.d[0][ll]);
+  }
+  std::vector<int> cur(nl, 0), held(nl, -1);
+  const float *pending = nullptr;   // a block's identity gradient, added to the input gradient of conv pending_for
+  int pending_for = -1;
+  int rc;
+  for (int i = (int)nc - 1; i >= 0; --i) {
+    const EConv &cv = e->convs[i];
+    const int lo = cv.level_out, li = cv.level_in, c = cv.d.c_out;
+    const bool last = i + 1 == (int)nc;
+    float *g = b.d[cur[lo]][lo];
+    // ReLU mask, BN backward
+    BEVB200_LAUNCH(bn_bwd_partial_kernel, stat_chunks(caps[lo]), kStatThreads, 0, st, g, t.y[i],
+                   last ? t.y_last : nullptr, cv.d.relu, t.z[i], t.stat[i], w.counts[lo], caps[lo], c, b.partial);
+    BEVB200_LAUNCH(bn_bwd_reduce_kernel, 1, kStatThreads, 0, st, b.partial, w.counts[lo], caps[lo], c,
+                   grad_bn_weight[i], grad_bn_bias[i], b.coef);
+    BEVB200_LAUNCH(bn_bwd_apply_kernel, grid_for((long long)caps[lo] * c, 256), 256, 0, st, g, t.z[i], t.stat[i],
+                   b.coef, w.counts[lo], caps[lo], c, b.dz[lo]);
+    if (cv.d.residual_from >= 0) {   // g (after the mask) is also the gradient of the identity
+      BEVB200_REQUIRE(pending_for < 0, "two pending residual gradients");
+      held[lo] = cur[lo];
+      pending = g;
+      pending_for = cv.d.residual_from + 1;
+    }
+    // filter gradient on the saved input image
+    const int cip = spconv_v6_cin_eff(cv.d.c_in), wide = spconv_wgrad_tc_image_channels(cv.d.c_in);
+    const uint8_t *fimg = i == 0 ? t.in_split : t.y[i - 1];
+    if (wide != cip) {
+      BEVB200_LAUNCH(enc_widen_image_kernel, grid_for((long long)caps[li] * (wide / 4), 256), 256, 0, st, fimg, cip,
+                     wide, w.counts[li], caps[li], b.fwide);
+      fimg = b.fwide;
+    }
+    rc = spconv_wgrad_tc_split(fimg, b.dz[lo], w.nbr[cv.rulebook], caps[li], caps[lo], w.counts[lo], cv.d.c_in, c,
+                               cv.kvol, grad_weights[i], b.wg, st);
+    if (rc) return rc;
+    // input gradient
+    if (i == 0 && grad_voxel_features == nullptr) break;
+    BEVB200_LAUNCH(enc_weight_t_kernel, grid_for((long long)cv.kvol * c * cip, 256), 256, 0, st, weights[i], cv.kvol,
+                   cv.d.c_in, c, cip, cv.d.subm, b.wt);
+    rc = spconv_v6_pack_weights(b.wt, c, cip, cv.kvol, b.packed, st);
+    if (rc) return rc;
+    const void *gimg = b.wg;   // c_out 32 / 64 / 128: the filter gradient's image of dz is the forward's row image
+    if (c == 16) {
+      rc = spconv_v6_split_rows(b.dz[lo], caps[lo], w.counts[lo], c, c, b.g16, st);
+      if (rc) return rc;
+      gimg = b.g16;
+    }
+    const int32_t *table = w.nbr[cv.rulebook];   // SubM: the forward table with mirrored offsets (in the weights)
+    if (!cv.d.subm) {
+      BEVB200_LAUNCH(enc_nbr_t_fill_kernel, grid_for((long long)cv.kvol * caps[li], 256), 256, 0, st, w.counts[li],
+                     caps[li], cv.kvol, b.nbr_t);
+      BEVB200_LAUNCH(enc_nbr_t_scatter_kernel, grid_for((long long)cv.kvol * caps[lo], 256), 256, 0, st,
+                     w.nbr[cv.rulebook], w.counts[lo], caps[lo], w.counts[li], caps[li], cv.kvol, b.nbr_t);
+      table = b.nbr_t;
+    }
+    const float *res = pending_for == i ? pending : nullptr;
+    float *out;
+    int oi = 0;
+    if (i == 0) {
+      out = b.din0;
+    } else {
+      oi = (li == lo && held[lo] == cur[lo]) ? cur[lo] ^ 1 : (li == lo ? cur[lo] : 0);
+      out = b.d[oi][li];
+    }
+    rc = spconv_v6_forward(gimg, b.packed, table, (long long)caps[li], caps[lo], caps[li], w.counts[li], c, cip,
+                           cv.kvol, nullptr, nullptr, res, nullptr, 0, out, nullptr, st);
+    if (rc) return rc;
+    if (res) {
+      pending = nullptr;
+      pending_for = -1;
+      held[lo] = -1;
+    }
+    if (i == 0) {
+      BEVB200_LAUNCH(enc_narrow_grad_kernel, grid_for((long long)max_voxels * e->in_channels, 256), 256, 0, st,
+                     b.din0, e->c0_eff, w.counts[0], caps[0], max_voxels, e->in_channels, grad_voxel_features);
+    } else {
+      cur[li] = oi;
+    }
+  }
   return BEVB200_OK;
 }
 

@@ -62,6 +62,15 @@ int spconv_wgrad_tc(const float *features, const float *out_grad, const int32_t 
                     int c_out, int kvol, float *weight_grad, void *workspace, cudaStream_t st);
 // the split image of out_grad that spconv_wgrad_tc() leaves in its workspace
 const void *spconv_wgrad_tc_grad_image(const void *workspace, int n_in, int c_in);
+// channels per row of the filter gradient's operand images: 32 / 64 / 128 (c zero padded)
+int spconv_wgrad_tc_image_channels(int c);
+// The same filter gradient on a ready feature image ([n_in][image_channels(c_in) * 4 B], rows reached through nbr)
+// and fp32 out_grad rows, of which only the first min(n_out, *n_out_dev) count (nullable n_out_dev).  The split image
+// of out_grad is left at the start of the workspace.
+size_t spconv_wgrad_tc_split_workspace_bytes(int n_out, int c_in, int c_out, int kvol);
+int spconv_wgrad_tc_split(const void *features_split, const float *out_grad, const int32_t *nbr, int n_in, int n_out,
+                          const int32_t *n_out_dev, int c_in, int c_out, int kvol, float *weight_grad,
+                          void *workspace, cudaStream_t st);
 
 // ---- spconv_bwd.cu ---------------------------------------------------------------------------
 // weight_grad[e] = sum over the chunks, in ascending order, of partial[chunk][e]: bit-reproducible

@@ -45,14 +45,6 @@ struct V6Params {
   int nkb, cin_shift;
 };
 
-// hi = rn_bf16(x), lo = rn_bf16(x - hi) for a pair of values, packed (first value in the low half)
-__device__ __forceinline__ void split_pair(float x0, float x1, uint32_t &hi, uint32_t &lo) {
-  const uint32_t h = cvt_bf16x2(x1, x0);
-  const float h0 = __uint_as_float(h << 16), h1 = __uint_as_float(h & 0xffff0000u);
-  hi = h;
-  lo = cvt_bf16x2(x1 - h1, x0 - h0);
-}
-
 // Epilogue of NC (8 or 16) consecutive channels [c0, c0 + NC) of one row: folded BN, residual, ReLU,
 // then the fp32 row and / or its split image.  NC channels = NC/8 16-byte chunks of hi and of lo.
 template <int NC>

@@ -30,6 +30,7 @@ struct WgtParams {
   const uint8_t *fsplit;       // [n_in][ci_eff * 4 B]
   const uint8_t *gsplit;       // [n_out][co_eff * 4 B]
   const int32_t *nbr;          // [kvol][n_out]
+  const int32_t *n_out_dev;    // nullable device row count (<= n_out): rows past it count as missing
   float *partial;              // [n_chunks][kvol][c_in][c_out]
   int n_in, n_out, c_in, c_out, kvol;
   int n_chunks, tiles_per_chunk, n_tiles;   // tiles of kWgtRows rows
@@ -61,10 +62,17 @@ __global__ void __launch_bounds__(kWgtThreads, 1) spconv_wgrad_tc_kernel(const W
   const unsigned long long fbase = reinterpret_cast<unsigned long long>(p.fsplit);
   const unsigned long long gbase = reinterpret_cast<unsigned long long>(p.gsplit);
   const int n_items = p.n_chunks * p.kvol;
+  // with a device row count the valid rows are re-spread over the same chunks (the partial layout stays put)
+  int n_valid = p.n_out, n_tiles = p.n_tiles, tiles_per_chunk = p.tiles_per_chunk;
+  if (p.n_out_dev) {
+    n_valid = min(p.n_out, max(__ldg(p.n_out_dev), 0));
+    n_tiles = (n_valid + kWgtRows - 1) / kWgtRows;
+    tiles_per_chunk = max((n_tiles + p.n_chunks - 1) / p.n_chunks, 1);
+  }
 
   for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
     const int chunk = item / p.kvol, k = item - chunk * p.kvol;
-    const int t_begin = chunk * p.tiles_per_chunk, t_end = min(p.n_tiles, t_begin + p.tiles_per_chunk);
+    const int t_begin = chunk * tiles_per_chunk, t_end = min(n_tiles, t_begin + tiles_per_chunk);
     const int nt_items = t_end - t_begin;
     const int32_t *nbr_k = p.nbr + (long long)k * p.n_out;
     auto load_stage = [&](int i) {
@@ -72,13 +80,13 @@ __global__ void __launch_bounds__(kWgtThreads, 1) spconv_wgrad_tc_kernel(const W
       const int o0 = (t_begin + i) * kWgtRows;
       for (int u = tid; u < kWgtRows * FCH; u += kWgtThreads) {
         const int r = u / FCH, c = u - r * FCH;
-        int src = o0 + r < p.n_out ? __ldg(nbr_k + o0 + r) : -1;
+        int src = o0 + r < n_valid ? __ldg(nbr_k + o0 + r) : -1;
         if (src >= p.n_in) src = -1;
         cp_async16_row(f + wgt_off(r, c, FR), fbase + (unsigned long long)(uint32_t)max(src, 0) * FR + c * 16, src);
       }
       for (int u = tid; u < kWgtRows * GCH; u += kWgtThreads) {
         const int r = u / GCH, c = u - r * GCH;
-        const int o = o0 + r < p.n_out ? o0 + r : -1;
+        const int o = o0 + r < n_valid ? o0 + r : -1;
         cp_async16_row(g + wgt_off(r, c, GR), gbase + (unsigned long long)(uint32_t)max(o, 0) * GR + c * 16, o);
       }
     };
@@ -221,6 +229,27 @@ static int wgt_launch_co(const WgtParams &p, int co_eff, cudaStream_t st) {
   return wgt_launch<CI, 128>(p, st);
 }
 
+static int wgt_run(const uint8_t *fsplit, const uint8_t *gsplit, const int32_t *nbr, int n_in, int n_out,
+                   const int32_t *n_out_dev, int c_in, int c_out, int kvol, float *partial, float *weight_grad,
+                   cudaStream_t st) {
+  const WgtPlan w = wgt_plan(n_out, c_in, c_out, kvol);
+  WgtParams p;
+  memset(&p, 0, sizeof(p));
+  p.fsplit = fsplit;
+  p.gsplit = gsplit;
+  p.nbr = nbr;
+  p.n_out_dev = n_out_dev;
+  p.partial = partial;
+  p.n_in = n_in; p.n_out = n_out; p.c_in = c_in; p.c_out = c_out; p.kvol = kvol;
+  p.n_tiles = w.n_tiles; p.n_chunks = w.n_chunks; p.tiles_per_chunk = w.tiles_per_chunk;
+  int rc;
+  if (w.ci_eff == 32) rc = wgt_launch_co<32>(p, w.co_eff, st);
+  else if (w.ci_eff == 64) rc = wgt_launch_co<64>(p, w.co_eff, st);
+  else rc = wgt_launch_co<128>(p, w.co_eff, st);
+  if (rc) return rc;
+  return spconv_wgrad_reduce(partial, (long long)kvol * c_in * c_out, p.n_chunks, weight_grad, st);
+}
+
 int spconv_wgrad_tc(const float *features, const float *out_grad, const int32_t *nbr, int n_in, int n_out,
                     int c_in, int c_out, int kvol, float *weight_grad, void *workspace, cudaStream_t st) {
   BEVB200_REQUIRE(spconv_wgrad_tc_ok(c_in, c_out, kvol), "shape has no tensor-core filter gradient");
@@ -232,19 +261,29 @@ int spconv_wgrad_tc(const float *features, const float *out_grad, const int32_t 
   int rc = spconv_v6_split_rows(features, n_in, nullptr, c_in, ci_eff, fsplit, st);
   if (!rc) rc = spconv_v6_split_rows(out_grad, n_out, nullptr, c_out, co_eff, gsplit, st);
   if (rc) return rc;
-  WgtParams p;
-  memset(&p, 0, sizeof(p));
-  p.fsplit = fsplit;
-  p.gsplit = gsplit;
-  p.nbr = nbr;
-  p.partial = partial;
-  p.n_in = n_in; p.n_out = n_out; p.c_in = c_in; p.c_out = c_out; p.kvol = kvol;
-  p.n_tiles = w.n_tiles; p.n_chunks = w.n_chunks; p.tiles_per_chunk = w.tiles_per_chunk;
-  if (ci_eff == 32) rc = wgt_launch_co<32>(p, co_eff, st);
-  else if (ci_eff == 64) rc = wgt_launch_co<64>(p, co_eff, st);
-  else rc = wgt_launch_co<128>(p, co_eff, st);
+  return wgt_run(fsplit, gsplit, nbr, n_in, n_out, nullptr, c_in, c_out, kvol, partial, weight_grad, st);
+}
+
+int spconv_wgrad_tc_image_channels(int c) { return wgt_eff(c); }
+
+size_t spconv_wgrad_tc_split_workspace_bytes(int n_out, int c_in, int c_out, int kvol) {
+  if (!spconv_wgrad_tc_ok(c_in, c_out, kvol) || n_out <= 0) return 0;
+  const WgtPlan w = wgt_plan(n_out, c_in, c_out, kvol);
+  return align_up((size_t)n_out * w.co_eff * 4) + align_up((size_t)w.n_chunks * kvol * c_in * c_out * sizeof(float));
+}
+
+int spconv_wgrad_tc_split(const void *features_split, const float *out_grad, const int32_t *nbr, int n_in, int n_out,
+                          const int32_t *n_out_dev, int c_in, int c_out, int kvol, float *weight_grad,
+                          void *workspace, cudaStream_t st) {
+  BEVB200_REQUIRE(spconv_wgrad_tc_ok(c_in, c_out, kvol), "shape has no tensor-core filter gradient");
+  BEVB200_REQUIRE(n_out > 0 && n_in > 0, "empty operands");
+  const WgtPlan w = wgt_plan(n_out, c_in, c_out, kvol);
+  uint8_t *gsplit = (uint8_t *)workspace;
+  float *partial = (float *)(gsplit + align_up((size_t)n_out * w.co_eff * 4));
+  int rc = spconv_v6_split_rows(out_grad, n_out, n_out_dev, c_out, w.co_eff, gsplit, st);
   if (rc) return rc;
-  return spconv_wgrad_reduce(partial, (long long)kvol * c_in * c_out, p.n_chunks, weight_grad, st);
+  return wgt_run((const uint8_t *)features_split, gsplit, nbr, n_in, n_out, n_out_dev, c_in, c_out, kvol, partial,
+                 weight_grad, st);
 }
 
 }  // namespace bevb200

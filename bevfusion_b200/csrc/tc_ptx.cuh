@@ -16,6 +16,14 @@ __device__ __forceinline__ uint32_t cvt_bf16x2(float hi, float lo) {
   return d;
 }
 
+// hi = rn_bf16(x), lo = rn_bf16(x - hi) for a pair of values (the split images of spconv_v6.cu), packed (first value in the low half)
+__device__ __forceinline__ void split_pair(float x0, float x1, uint32_t &hi, uint32_t &lo) {
+  const uint32_t h = cvt_bf16x2(x1, x0);
+  const float h0 = __uint_as_float(h << 16), h1 = __uint_as_float(h & 0xffff0000u);
+  hi = h;
+  lo = cvt_bf16x2(x1 - h1, x0 - h0);
+}
+
 // 16-byte cp.async; `row` < 0 = the ignore-src form: nothing is read, the 16 bytes are zero-filled
 __device__ __forceinline__ void cp_async16_row(uint32_t dst_smem, unsigned long long src, int row) {
   asm volatile(

@@ -1,7 +1,10 @@
 """EncoderPlan -- host side of bevb200_encoder_* (csrc/encoder.cu): a SparseEncoder in eval mode as ONE
 native call with no host synchronisation (row counts stay on the device), so a frame can be captured in
 a CUDA graph.  Replaces the python loop of mmdet3d/models/backbones/sparse_encoder.py:113-130 over
-spconv/conv.py:114-223 (one rulebook build + ~80 launches + one device->host count per conv there)."""
+spconv/conv.py:114-223 (one rulebook build + ~80 launches + one device->host count per conv there).
+
+forward_train() is the same chain in training mode (batch-statistics BatchNorm, running statistics updated
+in place) with a native whole-encoder backward, also sync-free and capturable."""
 import ctypes
 
 import torch
@@ -15,6 +18,13 @@ class _ConvDesc(ctypes.Structure):
     _fields_ = [("c_in", ctypes.c_int32), ("c_out", ctypes.c_int32), ("ksize", ctypes.c_int32 * 3),
                 ("stride", ctypes.c_int32 * 3), ("padding", ctypes.c_int32 * 3), ("dilation", ctypes.c_int32 * 3),
                 ("subm", ctypes.c_int32), ("relu", ctypes.c_int32), ("residual_from", ctypes.c_int32)]
+
+
+class _BNDesc(ctypes.Structure):
+    # mirrors bevb200_encoder_bn_t (include/bevfusion_b200.h)
+    _fields_ = [("weight", ctypes.c_void_p), ("bias", ctypes.c_void_p), ("running_mean", ctypes.c_void_p),
+                ("running_var", ctypes.c_void_p), ("num_batches_tracked", ctypes.c_void_p),
+                ("eps", ctypes.c_float), ("momentum", ctypes.c_float)]
 
 
 def _chain_of(encoder):
@@ -189,6 +199,148 @@ class EncoderPlan:
         _C.check(rc, "encoder_forward")
         return out
 
+    # -- training ------------------------------------------------------------------------------
+    def train_state_bytes(self, max_voxels, batch_size, level_caps=None):
+        """Device bytes one training forward keeps for its backward (sized by the level caps)."""
+        return int(_C.lib().bevb200_encoder_train_state_bytes(self._h, int(max_voxels), int(batch_size),
+                                                              self._caps_arg(level_caps)))
+
+    def backward_workspace_bytes(self, max_voxels, batch_size, level_caps=None):
+        return int(_C.lib().bevb200_encoder_backward_workspace_bytes(self._h, int(max_voxels), int(batch_size),
+                                                                     self._caps_arg(level_caps)))
+
+    def saved_rows(self, state, max_voxels, batch_size, conv, level_caps=None):
+        """(pre-BN rows z, output rows y) of conv `conv` as saved by a training forward into `state`: fp32
+        [cap, c_out] each (y decoded from its split image); only the level's first status[1 + l] rows are
+        defined."""
+        zo, yo = ctypes.c_size_t(), ctypes.c_size_t()
+        _C.check(_C.lib().bevb200_encoder_train_saved(self._h, int(max_voxels), int(batch_size),
+                                                      self._caps_arg(level_caps), int(conv), ctypes.byref(zo),
+                                                      ctypes.byref(yo)), "encoder_train_saved")
+        c = self.chain[conv][0].out_channels
+        cap = self.level_caps(max_voxels, batch_size, level_caps)[self.level_of(conv)]
+        z = state[zo.value:zo.value + cap * c * 4].view(torch.float32).view(cap, c)
+        img = state[yo.value:yo.value + cap * c * 4].view(torch.bfloat16).view(cap, c // 16, 2, 16).float()
+        return z, (img[:, :, 0] + img[:, :, 1]).reshape(cap, c)
+
+    def level_of(self, conv):
+        """level of conv `conv`'s output rows (0 = the voxels)."""
+        return sum(1 for cv, _, _, _ in self.chain[:conv + 1] if not cv.subm)
+
+    def _bn_descs(self, bn_weights, bn_biases):
+        descs = (_BNDesc * len(self.chain))()
+        for d, (_, bn, _, _), g, b in zip(descs, self.chain, bn_weights, bn_biases):
+            d.weight, d.bias = g.data_ptr(), b.data_ptr()
+            d.running_mean, d.running_var = bn.running_mean.data_ptr(), bn.running_var.data_ptr()
+            d.num_batches_tracked = _C.ptr(bn.num_batches_tracked)
+            d.eps, d.momentum = float(bn.eps), float(bn.momentum)
+        return descs
+
+    def _forward_train_native(self, voxel_features, coors, batch_size, n_voxels_dev, level_caps, overlap_rulebooks,
+                              weights, bn_weights, bn_biases):
+        """One training forward: returns (dense output, state).  Updates the running statistics in place."""
+        dev = voxel_features.device
+        n = voxel_features.shape[0]
+        B = int(batch_size)
+        X, Y, Z = self.out_shape
+        L = _C.lib()
+        with torch.cuda.device(dev):
+            out = torch.empty((B, self.out_channels * Z, X, Y), dtype=torch.float32, device=dev)
+            caps = self._caps_arg(level_caps)
+            state = torch.empty(L.bevb200_encoder_train_state_bytes(self._h, n, B, caps), dtype=torch.uint8,
+                                device=dev)
+            if self.status is None or self.status.device != dev:
+                self.status = torch.zeros(1 + self.n_levels, dtype=torch.int32, device=dev)
+            side = 0
+            if overlap_rulebooks:
+                if self._side is None or self._side.device != dev:
+                    self._side = torch.cuda.Stream(device=dev)
+                side = self._side.cuda_stream
+            wp = (ctypes.c_void_p * len(weights))(*[w.data_ptr() for w in weights])
+            rc = L.bevb200_encoder_forward_train(self._h, wp, self._bn_descs(bn_weights, bn_biases),
+                                                 _C.ptr(voxel_features), _C.ptr(coors), n, _C.ptr(n_voxels_dev), B,
+                                                 caps, _C.ptr(out), 0, _C.ptr(self.status), _C.ptr(state),
+                                                 state.numel(), _C.current_stream(dev), side)
+        _C.check(rc, "encoder_forward_train")
+        # torch's BatchNorm bumps num_batches_tracked's version (add_(1)); the eval plan's fold key reads it
+        for _, bn, _, _ in self.chain:
+            if bn.num_batches_tracked is not None:
+                torch.autograd.graph.increment_version(bn.num_batches_tracked)
+        return out, state
+
+    def _backward_native(self, state, n, batch_size, level_caps, grad_out, weights, need_input):
+        dev = grad_out.device
+        L = _C.lib()
+        with torch.cuda.device(dev):
+            caps = self._caps_arg(level_caps)
+            ws = torch.empty(L.bevb200_encoder_backward_workspace_bytes(self._h, n, int(batch_size), caps),
+                             dtype=torch.uint8, device=dev)
+            gfeat = (torch.empty((n, self.encoder.in_channels), dtype=torch.float32, device=dev)
+                     if need_input else None)
+            gw = [torch.empty_like(w) for w in weights]
+            gg = [torch.empty(cv.out_channels, dtype=torch.float32, device=dev) for cv, _, _, _ in self.chain]
+            gb = [torch.empty_like(g) for g in gg]
+
+            def arr(ts):
+                return (ctypes.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
+
+            rc = L.bevb200_encoder_backward(self._h, arr(weights), _C.ptr(state), state.numel(), n, int(batch_size),
+                                            caps, _C.ptr(grad_out), 0, _C.ptr(gfeat), arr(gw), arr(gg), arr(gb),
+                                            _C.ptr(ws), ws.numel(), _C.current_stream(dev))
+        _C.check(rc, "encoder_backward")
+        return gfeat, gw, gg, gb
+
+    def forward_train(self, voxel_features, coors, batch_size, n_voxels_dev=None, level_caps=None,
+                      overlap_rulebooks=True):
+        """Training-mode forward of the encoder (torch's BatchNorm1d in train mode, ReLU, residuals):
+        voxel_features [N, C] fp32, coors [N, 4] int32, n_voxels_dev as in forward().  Differentiable in the
+        features, every conv weight and every BN weight / bias; the backward is one native call on this
+        forward's rulebooks.  Under torch.no_grad() it still normalises with batch statistics and updates the
+        running statistics, and keeps nothing for a backward."""
+        _C.require_cuda(voxel_features, "voxel_features", torch.float32)
+        _C.require_cuda(coors, "coors", torch.int32)
+        n = voxel_features.shape[0]
+        assert coors.shape[0] == n and coors.shape[1] == 4 and voxel_features.shape[1] == self.encoder.in_channels
+        if n == 0:
+            raise ValueError("a training forward needs at least one voxel (BatchNorm statistics)")
+        weights = [conv.weight for conv, _, _, _ in self.chain]
+        for w in weights:
+            _C.require_cuda(w, "conv weight", torch.float32)
+        bn_w = [bn.weight for _, bn, _, _ in self.chain]
+        bn_b = [bn.bias for _, bn, _, _ in self.chain]
+        params = weights + bn_w + bn_b
+        if torch.is_grad_enabled() and (voxel_features.requires_grad or any(p.requires_grad for p in params)):
+            return _EncoderTrainFn.apply(self, coors, batch_size, n_voxels_dev, level_caps, overlap_rulebooks,
+                                         voxel_features, *params)
+        with torch.no_grad():
+            out, _ = self._forward_train_native(voxel_features, coors, batch_size, n_voxels_dev, level_caps,
+                                                overlap_rulebooks, weights, bn_w, bn_b)
+        return out
+
     def overflowed(self):
         """True when a level cap truncated the last forward (host sync)."""
         return self.status is not None and int(self.status[0].item()) != 0
+
+
+class _EncoderTrainFn(torch.autograd.Function):
+    """EncoderPlan.forward_train with the native backward.  The conv and BN parameters are saved with
+    save_for_backward, so an in-place update between forward and backward raises; the state (rulebooks,
+    pre-BN rows, output images, batch statistics) is allocated per call and saved alongside them."""
+
+    @staticmethod
+    def forward(ctx, plan, coors, batch_size, n_voxels_dev, level_caps, overlap_rulebooks, voxel_features, *params):
+        nc = len(plan.chain)
+        out, state = plan._forward_train_native(voxel_features, coors, batch_size, n_voxels_dev, level_caps,
+                                                overlap_rulebooks, params[:nc], params[nc:2 * nc], params[2 * nc:])
+        ctx.save_for_backward(state, *params)     # the state is freed with the graph's saved tensors
+        ctx.plan, ctx.n, ctx.batch_size, ctx.level_caps = plan, voxel_features.shape[0], batch_size, level_caps
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        state, *params = ctx.saved_tensors
+        plan = ctx.plan
+        nc = len(plan.chain)
+        gfeat, gw, gg, gb = plan._backward_native(state, ctx.n, ctx.batch_size, ctx.level_caps,
+                                                  grad_out.contiguous(), params[:nc], ctx.needs_input_grad[6])
+        return (None,) * 6 + (gfeat,) + tuple(gw) + tuple(gg) + tuple(gb)

@@ -81,6 +81,8 @@ class SparseEncoder(nn.Module):
             # `num_voxels` (device int32[1]): only the first rows are valid -- no host round trip
             return self.plan().forward(voxel_features.contiguous(), coors.contiguous(), batch_size,
                                        n_voxels_dev=num_voxels, out=out, overlap_rulebooks=self.overlap_rulebooks)
+        if num_voxels is not None and self.training:
+            return self._forward_train_native(voxel_features, coors, batch_size, num_voxels, precision, out)
         if num_voxels is not None:
             raise ValueError("num_voxels= needs the native plan (eval mode, bf16x3, no grad)")
         x = spconv.SparseConvTensor(voxel_features, coors, self.sparse_shape, batch_size)
@@ -98,6 +100,29 @@ class SparseEncoder(nn.Module):
         N, C, H, W, D = spatial_features.shape
         spatial_features = spatial_features.permute(0, 1, 4, 2, 3).contiguous()
         return spatial_features.view(N, C * D, H, W)
+
+    def _forward_train_native(self, voxel_features, coors, batch_size, num_voxels, precision, out):
+        """Training mode with a device-side voxel count: the native training plan (EncoderPlan.forward_train),
+        sync-free and capturable.  What it does not cover raises instead of falling back."""
+        def refuse(reason):
+            raise ValueError("num_voxels= in training mode runs the native training plan, which needs " + reason)
+        if precision != sp_ops.PREC_BF16X3:
+            refuse("the bf16x3 precision")
+        if voxel_features.dtype != torch.float32 or any(p.dtype != torch.float32 for p in self.parameters()):
+            refuse("fp32 features and weights (no half)")
+        if out is not None:
+            refuse("no out= (the output is a fresh tensor)")
+        if self.plan() is None:
+            refuse("a chain of (conv, norm, act) modules with tensor-core channel counts")
+        for conv, bn, _, _ in self.plan().chain:
+            if conv.bias is not None:
+                refuse("convs without bias")
+            if bn is None or not bn.affine or not bn.track_running_stats:
+                refuse("an affine BatchNorm1d with running statistics after every conv")
+            if bn.momentum is None:
+                refuse("a BatchNorm momentum (momentum=None, the cumulative average, is not covered)")
+        return self.plan().forward_train(voxel_features.contiguous(), coors.contiguous(), batch_size,
+                                         n_voxels_dev=num_voxels, overlap_rulebooks=self.overlap_rulebooks)
 
     @staticmethod
     def _convmodule_fused(seq, x, precision):

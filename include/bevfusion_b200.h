@@ -1084,6 +1084,58 @@ BEVB200_API int bevb200_encoder_forward(bevb200_encoder_t *enc, const void *para
                             long long out_batch_stride, int32_t *status_dev, void *workspace,
                             size_t workspace_bytes, void *stream, void *rulebook_stream);
 
+/* status_dev[0] bits of the encoder calls */
+#define BEVB200_ENCODER_TRUNCATED 1  /* a level cap truncated a level's rows */
+#define BEVB200_ENCODER_FEW_ROWS 2   /* training: a level had fewer than 2 valid rows (torch's BatchNorm1d raises);
+                                        its BN used what rows it had, and the running statistics were left alone */
+
+/* Training mode of the same plan: torch's BatchNorm1d in train mode in place of the folded BN, with a
+ * whole-encoder backward on the forward's rulebooks.  Both calls are sync-free and may be captured in a CUDA graph.
+ *   train_state_bytes  device bytes that live from forward_train to backward (rulebooks, the packed weights, and per
+ *                      conv its fp32 pre-BN rows, its output's split image and its batch statistics), sized by the
+ *                      caps of (max_voxels, batch_size, level_caps_host)
+ *   forward_train      weights[i]: conv i's live fp32 weight [K, c_in, c_out] (packed on every call); bn[i]: its
+ *                      BatchNorm1d.  Per conv: the conv without epilogue into fp32 rows z; per-channel batch mean and
+ *                      biased variance over the level's valid rows (double partials over fixed 2048-row chunks, added
+ *                      in a fixed order: bit-reproducible); running_mean / running_var updated in place with
+ *                      `momentum` (unbiased variance) and *num_batches_tracked += 1 (nullable) when the level has
+ *                      >= 2 rows, else BEVB200_ENCODER_FEW_ROWS is set; then y = relu(gamma (z - mean) invstd + beta
+ *                      [+ y of residual_from]).  The other arguments are those of bevb200_encoder_forward.
+ *   train_saved        byte offsets inside the state of conv i's pre-BN rows z ([cap, c_out] fp32) and of its
+ *                      output's split image ([cap, c_out * 4 B]: per 16 channels 16 bf16 hi, then 16 bf16 lo;
+ *                      y = hi + lo); only the level's first status_dev[1 + l] rows are defined
+ *   backward           grad_dense [B, C*Z, X, Y] (out_batch_stride floats, 0 = dense) -> grad_voxel_features
+ *                      [max_voxels, in_channels] (nullable: skipped; rows past the valid count are 0),
+ *                      grad_weights[i] [K, c_in, c_out], grad_bn_weight[i] / grad_bn_bias[i] [c_out].  Every output
+ *                      is overwritten, never accumulated.  weights are the ones forward_train read; state is only
+ *                      read, so one state may be differentiated more than once. */
+typedef struct {
+  const float *weight, *bias;         /* gamma, beta [c_out] */
+  float *running_mean, *running_var;  /* [c_out], updated in place */
+  int64_t *num_batches_tracked;       /* [1], nullable */
+  float eps, momentum;
+} bevb200_encoder_bn_t;
+BEVB200_API size_t bevb200_encoder_train_state_bytes(const bevb200_encoder_t *enc, int max_voxels, int batch_size,
+                                         const int32_t *level_caps_host);
+BEVB200_API int bevb200_encoder_train_saved(const bevb200_encoder_t *enc, int max_voxels, int batch_size,
+                                const int32_t *level_caps_host, int conv, size_t *pre_bn_offset,
+                                size_t *out_image_offset);
+BEVB200_API int bevb200_encoder_forward_train(bevb200_encoder_t *enc, const float *const *weights,
+                                  const bevb200_encoder_bn_t *bn, const float *voxel_features,
+                                  const int32_t *coors, int max_voxels, const int32_t *n_voxels_dev,
+                                  int batch_size, const int32_t *level_caps_host, float *dense_out,
+                                  long long out_batch_stride, int32_t *status_dev, void *state,
+                                  size_t state_bytes, void *stream, void *rulebook_stream);
+BEVB200_API size_t bevb200_encoder_backward_workspace_bytes(const bevb200_encoder_t *enc, int max_voxels,
+                                                int batch_size, const int32_t *level_caps_host);
+BEVB200_API int bevb200_encoder_backward(const bevb200_encoder_t *enc, const float *const *weights,
+                             const void *state, size_t state_bytes, int max_voxels, int batch_size,
+                             const int32_t *level_caps_host, const float *grad_dense,
+                             long long out_batch_stride, float *grad_voxel_features,
+                             float *const *grad_weights, float *const *grad_bn_weight,
+                             float *const *grad_bn_bias, void *workspace, size_t workspace_bytes,
+                             void *stream);
+
 #ifdef __cplusplus
 }
 #endif
