@@ -146,6 +146,12 @@ _SIGNATURES = {
     "bevb200_encoder_backward_workspace_bytes": (c_size_t, [_P, c_int, c_int, _P]),
     "bevb200_encoder_backward": (c_int, [_P, _P, _P, c_size_t, c_int, c_int, _P, _P, ctypes.c_longlong, _P, _P, _P,
                                          _P, _P, c_size_t, _P]),
+    "bevb200_pillar_train_state_bytes": (c_size_t, [c_int, c_int]),
+    "bevb200_pillar_train_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "bevb200_pillar_forward_train": (c_int, [_P, _P, _P, c_int, c_int, _P, c_int, c_int] + [c_float] * 4
+                                     + [_P, _P, _P, _P, c_int, c_int, c_int, _P, _P, c_size_t, _P, c_size_t, _P]),
+    "bevb200_pillar_backward_train": (c_int, [_P, _P, _P, c_int, c_int, _P, c_int, c_int] + [c_float] * 4
+                                      + [_P, c_int, c_int, c_int, _P, c_size_t] + [_P] * 6 + [_P, c_size_t, _P]),
 }
 
 

@@ -18,6 +18,7 @@ from torch.autograd import Function
 from torch.nn import functional as F
 
 from . import _C
+from .encoder_plan import _BNDesc
 from .sparse_block import bn_fold_key, bn_scale_shift, build_norm_layer
 from .spconv.ops import sparse_to_dense
 from .voxelize import Voxelization, _floats
@@ -127,6 +128,109 @@ class PillarFeatureNet(nn.Module):
     def _geometry(self):
         return float(self.vx), float(self.vy), float(self.x_offset), float(self.y_offset)
 
+    def _train_refusal(self, features, max_points):
+        """Why the native training step cannot run this net on `features`, or None."""
+        layers = list(self.pfn_layers)
+        if not self.training:
+            return "the native training step needs training mode"
+        if not self.native_supported(max_points):
+            return ("the native training step needs the native pillar net shape (feat_channels [64, 64], "
+                    "with_distance False, F <= 8, P <= 32)")
+        if any(l.norm.training != self.training for l in layers):
+            return "every BN module must share the pillar net's training flag"
+        if any(l.norm.momentum is None for l in layers):
+            return "momentum=None (cumulative averages) is not supported by the native training step"
+        if features.dtype != torch.float32:
+            return "the native training step needs fp32 features"
+        if features.requires_grad:
+            return "the native training step produces no features gradient; detach the voxel features"
+        return None
+
+    def _bn_descs(self):
+        descs = (_BNDesc * 2)()
+        for d, layer in zip(descs, self.pfn_layers):
+            bn = layer.norm
+            d.weight, d.bias = bn.weight.data_ptr(), bn.bias.data_ptr()
+            d.running_mean, d.running_var = bn.running_mean.data_ptr(), bn.running_var.data_ptr()
+            d.num_batches_tracked = _C.ptr(bn.num_batches_tracked)
+            d.eps, d.momentum = float(bn.eps), float(bn.momentum)
+        return descs
+
+    def _train_params(self):
+        l1, l2 = self.pfn_layers
+        return [l1.linear.weight, l2.linear.weight, l1.norm.weight, l1.norm.bias, l2.norm.weight, l2.norm.bias]
+
+    def forward_train(self, voxels, num_points, coords4, n_dev, canvas_shape):
+        """Native training step: voxels [R, P, F] fp32 (S = n_dev.numel() segments of R / S rows, the first
+        n_dev[s] of each valid), num_points [R], coords4 [R, 4] (b, x, y, z) int32 -> canvas [B, 64, nx, ny].
+        BN uses the batch statistics over all slots of the valid pillars and updates the running statistics;
+        differentiable in both linear weights and both BN weights / biases.  No host synchronisation."""
+        why = self._train_refusal(voxels, voxels.shape[1] if voxels.dim() == 3 else 0)
+        if why:
+            raise ValueError(why)
+        _C.require_cuda(voxels, "voxels", torch.float32)
+        _C.require_cuda(num_points, "num_points", torch.int32)
+        _C.require_cuda(coords4, "coords4", torch.int32)
+        _C.require_cuda(n_dev, "voxel_num", torch.int32)
+        R, P, F_ = voxels.shape
+        S = n_dev.numel()
+        if F_ != self.in_channels or num_points.shape != (R,) or coords4.shape != (R, 4) or S < 1 or R % S:
+            raise ValueError("expected voxels [R, P, %d], num_points [R], coords4 [R, 4] and voxel_num [S] with "
+                             "S dividing R" % self.in_channels)
+        params = self._train_params()
+        for p in params:
+            _C.require_cuda(p, "pillar net parameter", torch.float32)
+        args = (self, voxels, num_points, coords4, n_dev, tuple(int(x) for x in canvas_shape))
+        if torch.is_grad_enabled() and any(p.requires_grad for p in params):
+            return _PillarTrainFn.apply(*args, *params)
+        with torch.no_grad():
+            return self._forward_train_native(*args[1:])[0]
+
+    def _row_args(self, voxels, num_points, coords4, n_dev):
+        R, P, F_ = voxels.shape
+        return (_C.ptr(voxels), _C.ptr(num_points), _C.ptr(coords4), R, n_dev.numel(), _C.ptr(n_dev), P, F_,
+                *self._geometry())
+
+    def _forward_train_native(self, voxels, num_points, coords4, n_dev, canvas_shape):
+        """One training forward: returns (canvas, state).  Updates the running statistics in place."""
+        dev = voxels.device
+        R, P = voxels.shape[0], voxels.shape[1]
+        B, C, nx, ny = canvas_shape
+        L = _C.lib()
+        l1, l2 = self.pfn_layers
+        with torch.cuda.device(dev):
+            canvas = torch.zeros(canvas_shape, dtype=torch.float32, device=dev)
+            state = torch.empty(L.bevb200_pillar_train_state_bytes(R, P), dtype=torch.uint8, device=dev)
+            ws = torch.empty(L.bevb200_pillar_train_workspace_bytes(R, P), dtype=torch.uint8, device=dev)
+            self.train_status = torch.empty(1, dtype=torch.int32, device=dev)
+            rc = L.bevb200_pillar_forward_train(*self._row_args(voxels, num_points, coords4, n_dev),
+                                                _C.ptr(l1.linear.weight), _C.ptr(l2.linear.weight), self._bn_descs(),
+                                                _C.ptr(canvas), B, nx, ny, _C.ptr(self.train_status), _C.ptr(state),
+                                                state.numel(), _C.ptr(ws), ws.numel(), _C.current_stream(dev))
+        _C.check(rc, "pillar_forward_train")
+        # torch's BatchNorm bumps num_batches_tracked's version (add_(1)); the eval path's fold key reads it
+        for layer in self.pfn_layers:
+            if layer.norm.num_batches_tracked is not None:
+                torch.autograd.graph.increment_version(layer.norm.num_batches_tracked)
+        return canvas, state
+
+    def _backward_native(self, voxels, num_points, coords4, n_dev, state, grad_canvas):
+        dev = grad_canvas.device
+        R, P = voxels.shape[0], voxels.shape[1]
+        B, _, nx, ny = grad_canvas.shape
+        L = _C.lib()
+        l1, l2 = self.pfn_layers
+        with torch.cuda.device(dev):
+            ws = torch.empty(L.bevb200_pillar_train_workspace_bytes(R, P), dtype=torch.uint8, device=dev)
+            grads = [torch.empty_like(p) for p in self._train_params()]
+            gw1, gw2, gg1, gb1, gg2, gb2 = grads
+            rc = L.bevb200_pillar_backward_train(*self._row_args(voxels, num_points, coords4, n_dev),
+                                                 _C.ptr(grad_canvas), B, nx, ny, _C.ptr(state), state.numel(),
+                                                 _C.ptr(gw1), _C.ptr(gw2), _C.ptr(gg1), _C.ptr(gb1), _C.ptr(gg2),
+                                                 _C.ptr(gb2), _C.ptr(ws), ws.numel(), _C.current_stream(dev))
+        _C.check(rc, "pillar_backward_train")
+        return grads
+
     def forward(self, features, num_voxels, coors):
         _C.require_cuda(features, "features", contiguous=False)
         if self._use_native(features):
@@ -167,6 +271,25 @@ class PillarFeatureNet(nn.Module):
             features = pfn(features)
         # the reference squeezes every unit dimension; only the slot one is meant
         return features.squeeze(1)
+
+
+class _PillarTrainFn(Function):
+    """PillarFeatureNet.forward_train with the native backward.  The parameters are saved with
+    save_for_backward, so an in-place update between forward and backward raises; the per-call state
+    (packed weights, batch statistics, per-pillar layer-2 argmax and x^ there) is saved alongside them."""
+
+    @staticmethod
+    def forward(ctx, net, voxels, num_points, coords4, n_dev, canvas_shape, *params):
+        canvas, state = net._forward_train_native(voxels, num_points, coords4, n_dev, canvas_shape)
+        ctx.save_for_backward(state, voxels, num_points, coords4, n_dev, *params)
+        ctx.net = net
+        return canvas
+
+    @staticmethod
+    def backward(ctx, grad_canvas):
+        state, voxels, num_points, coords4, n_dev, *_ = ctx.saved_tensors
+        grads = ctx.net._backward_native(voxels, num_points, coords4, n_dev, state, grad_canvas.contiguous())
+        return (None,) * 6 + tuple(grads)
 
 
 class _Scatter(Function):
@@ -223,7 +346,20 @@ class PointPillarsEncoder(nn.Module):
         self.pts_voxel_encoder = _build(pts_voxel_encoder)
         self.pts_middle_encoder = _build(pts_middle_encoder)
 
-    def forward(self, feats, coords, batch_size, sizes):
+    def forward(self, feats, coords, batch_size, sizes, voxel_num=None):
+        """voxel_num (device int32 [S], training mode only): run the native training step on feats [R, P, F]
+        whose S segments of R / S rows hold voxel_num[s] valid pillars each (the rest is ignored), with no host
+        synchronisation.  Without it, the module path below."""
+        if voxel_num is not None:
+            enc, scat = self.pts_voxel_encoder, self.pts_middle_encoder
+            if not self.training:
+                raise ValueError("voxel_num= runs the native training step, which needs training mode")
+            why = enc._train_refusal(feats, feats.shape[1] if feats.dim() == 3 else 0)
+            if why:
+                raise ValueError(why)
+            shape = (int(batch_size), enc.pfn_layers[-1].units, int(scat.nx), int(scat.ny))
+            return enc.forward_train(feats, sizes.to(torch.int32).contiguous(), coords.to(torch.int32).contiguous(),
+                                     voxel_num, shape)
         x = self.pts_voxel_encoder(feats, sizes, coords)
         return self.pts_middle_encoder(x, coords, batch_size)
 
@@ -232,10 +368,17 @@ class PointPillarsEncoder(nn.Module):
         `points_list` ([N_k, F] fp32 CUDA tensors), straight into one zeroed [B, C, nx, ny] canvas.
         Same result as voxelize_batch(voxelize_reduce=False) -> forward(), without the [M, P, F]
         voxel tensor and without a host synchronisation (CUDA-graph capturable).  Eval mode and no
-        autograd only; the voxel grid must be (nx, ny, 1)."""
+        autograd only; the voxel grid must be (nx, ny, 1).
+
+        In training mode it takes the native training step instead: every sample is hard-voxelized with the
+        training cap max_voxels[0] into its segment of one zeroed [B * cap, P, F] buffer, which goes through
+        forward_train (batch statistics, differentiable in the pillar net's parameters), still without a host
+        synchronisation."""
         enc, scat = self.pts_voxel_encoder, self.pts_middle_encoder
         if not isinstance(voxelize, Voxelization) or voxelize.max_num_points <= 0:
             raise ValueError("forward_points needs a hard Voxelization module")
+        if self.training:
+            return self._forward_points_train(points_list, voxelize)
         if self.training or enc.training or voxelize.training or torch.is_grad_enabled():
             raise RuntimeError("forward_points runs in eval mode under torch.no_grad() only")
         grid = [int(g) for g in voxelize.grid_size]
@@ -269,3 +412,38 @@ class PointPillarsEncoder(nn.Module):
                     _C.current_stream(dev))
                 _C.check(rc, "hard_voxelize_pillars")
         return canvas
+
+    def _forward_points_train(self, points_list, voxelize):
+        enc, scat = self.pts_voxel_encoder, self.pts_middle_encoder
+        grid = [int(g) for g in voxelize.grid_size]
+        if grid != [int(scat.nx), int(scat.ny), 1]:
+            raise ValueError("voxel grid %s differs from the scatter output shape (%d, %d, 1)"
+                             % (grid, scat.nx, scat.ny))
+        P, F_ = int(voxelize.max_num_points), enc.in_channels
+        for k, pts in enumerate(points_list):
+            _C.require_cuda(pts, "points[%d]" % k, torch.float32)
+            if pts.dim() != 2 or pts.shape[1] != F_:
+                raise ValueError("points[%d] must be [N, %d]" % (k, F_))
+        dev = points_list[0].device
+        B = len(points_list)
+        cap = int(voxelize.max_voxels[0] if voxelize.training else voxelize.max_voxels[1])
+        vs, cr = _floats(voxelize.voxel_size, 3), _floats(voxelize.point_cloud_range, 6)
+        with torch.cuda.device(dev):
+            voxels = torch.zeros((B * cap, P, F_), dtype=torch.float32, device=dev)
+            coors = torch.zeros((B * cap, 3), dtype=torch.int32, device=dev)
+            num = torch.zeros(B * cap, dtype=torch.int32, device=dev)
+            voxel_num = torch.zeros(B, dtype=torch.int32, device=dev)
+            nmax = max(int(p.shape[0]) for p in points_list)
+            ws = torch.empty(max(_C.lib().bevb200_hard_voxelize_workspace_bytes(nmax, P), 256), dtype=torch.uint8,
+                             device=dev)
+            for k, pts in enumerate(points_list):
+                rows = slice(k * cap, (k + 1) * cap)
+                rc = _C.lib().bevb200_hard_voxelize(
+                    _C.ptr(pts), int(pts.shape[0]), F_, ctypes.cast(vs, ctypes.c_void_p),
+                    ctypes.cast(cr, ctypes.c_void_p), P, cap, _C.ptr(voxels[rows]), _C.ptr(coors[rows]),
+                    _C.ptr(num[rows]), _C.ptr(voxel_num[k:k + 1]), _C.ptr(ws), ws.numel(), _C.current_stream(dev))
+                _C.check(rc, "hard_voxelize")
+            batch = torch.div(torch.arange(B * cap, device=dev), cap, rounding_mode="floor").to(torch.int32)
+            coords4 = torch.cat([batch.view(-1, 1), coors], dim=1)
+        shape = (B, enc.pfn_layers[-1].units, int(scat.nx), int(scat.ny))
+        return enc.forward_train(voxels, num, coords4, voxel_num, shape)

@@ -1136,6 +1136,45 @@ BEVB200_API int bevb200_encoder_backward(const bevb200_encoder_t *enc, const flo
                              float *const *grad_bn_bias, void *workspace, size_t workspace_bytes,
                              void *stream);
 
+/* ---- PointPillars pillar feature net, training mode (pillar_encoder.py:43-176, BatchNorm1d in train mode) ----
+ * The net of bevb200_pillar_features (F 3..8, P 1..32, feat_channels [64, 64], no distance feature; anything else
+ * gives BEVB200_EUNSUPPORTED) with batch statistics over all M * P slots, padded slots included (n = P * valid
+ * pillars, biased variance for the normalisation), and the backward of both linears and both BNs.
+ * Row source: voxels [rows, P, F] fp32, num_points [rows] int32, coords4 [rows, 4] int32 (b, x, y, z).  The rows
+ * form `segments` segments of cap = rows / segments rows; rows [s cap, s cap + min(n_dev[s], cap)) are valid
+ * (n_dev: DEVICE int32 [segments], nullable: every row), everything else is never read.
+ *   forward_train   w1 [32, F+5], w2 [64, 64] fp32 (nn.Linear layout, read on every call); bn: HOST array of the two
+ *                   layers' BatchNorm1d (bevb200_encoder_bn_t).  running_mean / running_var are updated in place with
+ *                   `momentum` (unbiased variance) and *num_batches_tracked += 1 (nullable).  The pillar maxes land in
+ *                   the caller-zeroed canvas [batch, 64, nx, ny] at (b, x, y).  status_dev[0] is set to 0 or
+ *                   BEVB200_PILLAR_FEW_ROWS (n < 2): then the running statistics and the canvas are left alone and
+ *                   the backward writes zero gradients.
+ *   backward_train  grad_canvas [batch, 64, nx, ny] -> grad_w1 [32, F+5], grad_w2 [64, 64], grad_gamma / grad_beta
+ *                   of each layer; every output is overwritten.  The row source must be the forward's; state is only
+ *                   read, so one state may be differentiated more than once.
+ * Sums are double over fixed 128-row chunks added in a fixed order: bit-reproducible, no float atomics, independent of
+ * the grid.  No per-slot buffer, no host synchronisation, no allocation.  state (forward -> backward) and workspace
+ * (both calls) come from the queries (0 for an unsupported P); a smaller one gives BEVB200_EWORKSPACE before any
+ * write. */
+#define BEVB200_PILLAR_FEW_ROWS 2
+BEVB200_API size_t bevb200_pillar_train_state_bytes(int rows, int max_points);
+BEVB200_API size_t bevb200_pillar_train_workspace_bytes(int rows, int max_points);
+BEVB200_API int bevb200_pillar_forward_train(const float *voxels, const int32_t *num_points, const int32_t *coords4,
+                                             int rows, int segments, const int32_t *n_dev, int max_points,
+                                             int num_features, float vx, float vy, float x_off, float y_off,
+                                             const float *w1, const float *w2, const bevb200_encoder_bn_t *bn,
+                                             float *canvas, int batch, int nx, int ny, int32_t *status_dev,
+                                             void *state, size_t state_bytes, void *workspace,
+                                             size_t workspace_bytes, void *stream);
+BEVB200_API int bevb200_pillar_backward_train(const float *voxels, const int32_t *num_points, const int32_t *coords4,
+                                              int rows, int segments, const int32_t *n_dev, int max_points,
+                                              int num_features, float vx, float vy, float x_off, float y_off,
+                                              const float *grad_canvas, int batch, int nx, int ny, const void *state,
+                                              size_t state_bytes, float *grad_w1, float *grad_w2,
+                                              float *grad_gamma1, float *grad_beta1, float *grad_gamma2,
+                                              float *grad_beta2, void *workspace, size_t workspace_bytes,
+                                              void *stream);
+
 #ifdef __cplusplus
 }
 #endif
