@@ -131,6 +131,8 @@ _SIGNATURES = {
     "bevb200_sparse_to_dense": (c_int, [_P, _P, c_int, c_int, c_int, _P, c_int, ctypes.c_longlong, _P, _P]),
     "bevb200_encoder_create": (c_int, [c_int, _P, _P, c_int, _P]),
     "bevb200_encoder_destroy": (None, [_P]),
+    "bevb200_encoder_set_precision": (c_int, [_P, c_int]),
+    "bevb200_encoder_precision": (c_int, [_P]),
     "bevb200_encoder_param_bytes": (c_size_t, [_P]),
     "bevb200_encoder_num_levels": (c_int, [_P]),
     "bevb200_encoder_output_shape": (c_int, [_P, _P, _P]),
@@ -139,13 +141,19 @@ _SIGNATURES = {
     "bevb200_encoder_workspace_bytes": (c_size_t, [_P, c_int, c_int, _P]),
     "bevb200_encoder_forward": (c_int, [_P, _P, _P, _P, c_int, _P, c_int, _P, _P, ctypes.c_longlong, _P, _P,
                                         c_size_t, _P, _P]),
+    "bevb200_encoder_forward_f16": (c_int, [_P, _P, _P, _P, c_int, _P, c_int, _P, _P, ctypes.c_longlong, _P, _P,
+                                            c_size_t, _P, _P]),
     "bevb200_encoder_train_state_bytes": (c_size_t, [_P, c_int, c_int, _P]),
     "bevb200_encoder_train_saved": (c_int, [_P, c_int, c_int, _P, c_int, _P, _P]),
     "bevb200_encoder_forward_train": (c_int, [_P, _P, _P, _P, _P, c_int, _P, c_int, _P, _P, ctypes.c_longlong, _P, _P,
                                               c_size_t, _P, _P]),
+    "bevb200_encoder_forward_train_f16": (c_int, [_P, _P, _P, _P, _P, c_int, _P, c_int, _P, _P, ctypes.c_longlong,
+                                                  _P, _P, c_size_t, _P, _P]),
     "bevb200_encoder_backward_workspace_bytes": (c_size_t, [_P, c_int, c_int, _P]),
     "bevb200_encoder_backward": (c_int, [_P, _P, _P, c_size_t, c_int, c_int, _P, _P, ctypes.c_longlong, _P, _P, _P,
                                          _P, _P, c_size_t, _P]),
+    "bevb200_encoder_backward_f16": (c_int, [_P, _P, _P, c_size_t, c_int, c_int, _P, _P, ctypes.c_longlong, _P, _P,
+                                             _P, _P, _P, c_size_t, _P]),
     "bevb200_pillar_train_state_bytes": (c_size_t, [c_int, c_int]),
     "bevb200_pillar_train_workspace_bytes": (c_size_t, [c_int, c_int]),
     "bevb200_pillar_forward_train": (c_int, [_P, _P, _P, c_int, c_int, _P, c_int, c_int] + [c_float] * 4

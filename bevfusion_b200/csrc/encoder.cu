@@ -54,6 +54,7 @@ using namespace bevb200;
 
 struct bevb200_encoder {
   int in_channels, c0_eff;
+  int precision;                     // BEVB200_PREC_BF16X3 (default) or BEVB200_PREC_FP16
   std::vector<EConv> convs;
   std::vector<ELevel> levels;
   std::vector<ERulebook> rulebooks;
@@ -63,6 +64,28 @@ struct bevb200_encoder {
 };
 
 namespace bevb200 {
+
+static bool enc_f16(const bevb200_encoder *e) { return e->precision == BEVB200_PREC_FP16; }
+// bytes per channel of the plan's operand images: BF16x3 split images 4, fp16 images 2
+static size_t enc_img_bytes(const bevb200_encoder *e) { return enc_f16(e) ? 2 : 4; }
+
+// offsets of every conv's packed weights, scale and shift in the parameter buffer (the weight image of the precision)
+static void enc_param_layout(bevb200_encoder *e) {
+  size_t poff = 0;
+  for (EConv &cv : e->convs) {
+    cv.packed_off = poff;
+    poff += align_up(enc_f16(e) ? spconv_v6_packed_bytes_f16(cv.d.c_in, cv.d.c_out, cv.kvol)
+                                : spconv_v6_packed_bytes(cv.d.c_in, cv.d.c_out, cv.kvol));
+    cv.scale_off = poff; poff += align_up((size_t)cv.d.c_out * 4);
+    cv.shift_off = poff; poff += align_up((size_t)cv.d.c_out * 4);
+  }
+  e->param_bytes = poff;
+}
+
+static int enc_pack(const bevb200_encoder *e, const EConv &cv, const float *weight, char *params, cudaStream_t st) {
+  return enc_f16(e) ? spconv_v6_pack_weights_f16(weight, cv.d.c_in, cv.d.c_out, cv.kvol, params + cv.packed_off, st)
+                    : spconv_v6_pack_weights(weight, cv.d.c_in, cv.d.c_out, cv.kvol, params + cv.packed_off, st);
+}
 
 static long long level_sites(const ELevel &l, int batch) {
   return (long long)batch * l.shape[0] * l.shape[1] * l.shape[2];
@@ -119,9 +142,10 @@ static void enc_layout_into(const bevb200_encoder *e, const std::vector<int> &ca
     w->f32[s].assign(nl, nullptr);
     if (!feature_buffers) continue;
     for (size_t l = 0; l < nl; ++l) {
-      const size_t row = (size_t)e->levels[l].c_max * 4;
+      const size_t row = (size_t)e->levels[l].c_max * enc_img_bytes(e);
       w->split[s][l] = a.take<uint8_t>((size_t)caps[l] * row);
-      w->f32[s][l] = a.take<float>((size_t)caps[l] * e->levels[l].c_max);
+      // FP16: dense() scatters the last conv's fp16 image, and residuals are read from images: no fp32 rows
+      if (!enc_f16(e)) w->f32[s][l] = a.take<float>((size_t)caps[l] * e->levels[l].c_max);
     }
   }
   w->bytes = a.off;
@@ -224,13 +248,13 @@ int bevb200_encoder_create(int in_channels, const int32_t *sparse_shape_host, co
   BEVB200_REQUIRE(e != nullptr, "out of host memory");
   e->in_channels = in_channels;
   e->c0_eff = spconv_v6_cin_eff(in_channels);
+  e->precision = BEVB200_PREC_BF16X3;
   e->event_device = -1;
   ELevel l0;
   for (int d = 0; d < 3; ++d) l0.shape[d] = sparse_shape_host[d];
   l0.c_max = e->c0_eff;
   e->levels.push_back(l0);
   int level = 0, c_prev = in_channels;
-  size_t poff = 0;
   auto fail = [&](const char *msg) {
     snprintf(g_last_error, sizeof(g_last_error), "bevb200_encoder_create: %s", msg);
     delete e;
@@ -297,9 +321,6 @@ int bevb200_encoder_create(int in_channels, const int32_t *sparse_shape_host, co
       e->rulebooks.push_back(rb);
     }
     cv.want_fp32 = i == n_convs - 1;
-    cv.packed_off = poff; poff += align_up(spconv_v6_packed_bytes(cv.d.c_in, cv.d.c_out, cv.kvol));
-    cv.scale_off = poff; poff += align_up((size_t)cv.d.c_out * 4);
-    cv.shift_off = poff; poff += align_up((size_t)cv.d.c_out * 4);
     cv.has_scale = cv.has_shift = false;
     e->convs.push_back(cv);
     c_prev = cv.d.c_out;
@@ -309,7 +330,7 @@ int bevb200_encoder_create(int in_channels, const int32_t *sparse_shape_host, co
   static const bool f32_residual = [] { const char *v = getenv("BEVB200_ENCODER_F32_RESIDUAL"); return v && atoi(v) != 0; }();
   for (EConv &cv : e->convs)
     if (f32_residual && cv.d.residual_from >= 0) e->convs[cv.d.residual_from].want_fp32 = true;
-  e->param_bytes = poff;
+  enc_param_layout(e);
   *out = e;
   return BEVB200_OK;
 }
@@ -319,6 +340,17 @@ void bevb200_encoder_destroy(bevb200_encoder_t *e) {
   for (cudaEvent_t ev : e->events) cudaEventDestroy(ev);
   delete e;
 }
+
+int bevb200_encoder_set_precision(bevb200_encoder_t *e, int precision) {
+  BEVB200_REQUIRE(e, "null plan");
+  BEVB200_REQUIRE(precision == BEVB200_PREC_BF16X3 || precision == BEVB200_PREC_FP16,
+                  "an encoder plan runs BEVB200_PREC_BF16X3 or BEVB200_PREC_FP16");
+  e->precision = precision;
+  enc_param_layout(e);
+  return BEVB200_OK;
+}
+
+int bevb200_encoder_precision(const bevb200_encoder_t *e) { return e ? e->precision : BEVB200_EINVAL; }
 
 size_t bevb200_encoder_param_bytes(const bevb200_encoder_t *e) { return e ? e->param_bytes : 0; }
 
@@ -338,7 +370,7 @@ int bevb200_encoder_set_conv(bevb200_encoder_t *e, int conv, const float *weight
   EConv &cv = e->convs[conv];
   cudaStream_t st = (cudaStream_t)stream;
   char *base = (char *)params;
-  int rc = spconv_v6_pack_weights(weight, cv.d.c_in, cv.d.c_out, cv.kvol, base + cv.packed_off, st);
+  int rc = enc_pack(e, cv, weight, base, st);
   if (rc) return rc;
   cv.has_scale = scale != nullptr;
   cv.has_shift = shift != nullptr;
@@ -367,11 +399,17 @@ size_t bevb200_encoder_workspace_bytes(const bevb200_encoder_t *e, int max_voxel
   return enc_layout(e, caps, batch_size, nullptr, 0, &w);
 }
 
-int bevb200_encoder_forward(bevb200_encoder_t *e, const void *params, const float *voxel_features,
-                            const int32_t *coors, int max_voxels, const int32_t *n_voxels_dev, int batch_size,
-                            const int32_t *user_caps, float *dense_out, long long out_batch_stride,
-                            int32_t *status_dev, void *workspace, size_t workspace_bytes, void *stream,
-                            void *rulebook_stream) {
+}  // extern "C"
+
+// bevb200_encoder_forward(_f16): voxel_features and dense_out are fp32 (BF16x3 plan) or fp16 (FP16 plan)
+static int enc_forward(bevb200_encoder_t *e, bool f16, const void *params, const void *voxel_features,
+                       const int32_t *coors, int max_voxels, const int32_t *n_voxels_dev, int batch_size,
+                       const int32_t *user_caps, void *dense_out, long long out_batch_stride, int32_t *status_dev,
+                       void *workspace, size_t workspace_bytes, void *stream, void *rulebook_stream) {
+  // the precision first: a call of the wrong family is refused before any other argument is looked at
+  BEVB200_REQUIRE(e, "null plan");
+  BEVB200_REQUIRE(enc_f16(e) == f16, f16 ? "the _f16 calls need a plan set to BEVB200_PREC_FP16"
+                                         : "an fp16 plan runs the _f16 calls");
   BEVB200_REQUIRE(e && params && dense_out && status_dev && max_voxels > 0 && batch_size > 0, "bad argument");
   BEVB200_REQUIRE(voxel_features && coors, "null input");
   cudaStream_t st = (cudaStream_t)stream, ss = rulebook_stream ? (cudaStream_t)rulebook_stream : st;
@@ -392,7 +430,10 @@ int bevb200_encoder_forward(bevb200_encoder_t *e, const void *params, const floa
   if (rc) return rc;
 
   // ------------------------------ features (stream st) -------------------------------------
-  rc = spconv_v6_split_rows(voxel_features, caps[0], n_voxels_dev, e->in_channels, e->c0_eff, w.split[0][0], st);
+  rc = f16 ? spconv_v6_f16_rows((const __half *)voxel_features, caps[0], n_voxels_dev, e->in_channels, e->c0_eff,
+                                 w.split[0][0], st)
+           : spconv_v6_split_rows((const float *)voxel_features, caps[0], n_voxels_dev, e->in_channels, e->c0_eff,
+                                  w.split[0][0], st);
   if (rc) return rc;
   std::vector<int> split_turn(nl, 0), f32_turn(nl, 0);
   split_turn[0] = 1;
@@ -410,12 +451,12 @@ int bevb200_encoder_forward(bevb200_encoder_t *e, const void *params, const floa
     const size_t lo = cv.level_out;
     const bool last = i + 1 == e->convs.size();
     uint8_t *osplit = nullptr;
-    if (!last) {
+    if (!last || f16) {   // FP16: the last conv's image is what dense() scatters
       osplit = w.split[split_turn[lo]][lo];
       split_turn[lo] ^= 1;
     }
     float *of32 = nullptr;
-    if (cv.want_fp32) {
+    if (cv.want_fp32 && !f16) {
       of32 = w.f32[f32_turn[lo]][lo];
       f32_turn[lo] ^= 1;
       f32_of[i] = of32;
@@ -425,11 +466,10 @@ int bevb200_encoder_forward(bevb200_encoder_t *e, const void *params, const floa
     const float *res = cv.d.residual_from >= 0 ? f32_of[cv.d.residual_from] : nullptr;
     const uint8_t *res_split = (cv.d.residual_from >= 0 && res == nullptr) ? split_of[cv.d.residual_from] : nullptr;
     BEVB200_REQUIRE(cv.d.residual_from < 0 || res || res_split, "residual source has no rows");
-    rc = spconv_v6_forward(cur_split, pbase + cv.packed_off, w.nbr[cv.rulebook], (long long)caps[lo], caps[cv.level_in],
-                           caps[lo], w.counts[lo], cv.c_in_eff, cv.d.c_out, cv.kvol,
-                           cv.has_scale ? (const float *)(pbase + cv.scale_off) : nullptr,
-                           cv.has_shift ? (const float *)(pbase + cv.shift_off) : nullptr, res, res_split, cv.d.relu,
-                           of32, osplit, st);
+    rc = (f16 ? spconv_v6_forward_f16 : spconv_v6_forward)(
+        cur_split, pbase + cv.packed_off, w.nbr[cv.rulebook], (long long)caps[lo], caps[cv.level_in], caps[lo],
+        w.counts[lo], cv.c_in_eff, cv.d.c_out, cv.kvol, cv.has_scale ? (const float *)(pbase + cv.scale_off) : nullptr,
+        cv.has_shift ? (const float *)(pbase + cv.shift_off) : nullptr, res, res_split, cv.d.relu, of32, osplit, st);
     if (rc) return rc;
     split_of[i] = osplit;
     cur_split = osplit;
@@ -437,11 +477,34 @@ int bevb200_encoder_forward(bevb200_encoder_t *e, const void *params, const floa
   }
   // dense(): [B, C*Z, X, Y]
   const size_t ll = nl - 1;
-  rc = sparse_to_dense(last_f32, w.indices[ll] ? w.indices[ll] : idx0, caps[ll], w.counts[ll], e->convs.back().d.c_out,
-                       batch_size, e->levels[ll].shape, 1, out_batch_stride, dense_out, st);
+  const int32_t *lidx = w.indices[ll] ? w.indices[ll] : idx0;
+  rc = f16 ? sparse_to_dense((const __half *)cur_split, lidx, caps[ll], w.counts[ll], e->convs.back().d.c_out,
+                             batch_size, e->levels[ll].shape, 1, out_batch_stride, (__half *)dense_out, st)
+           : sparse_to_dense(last_f32, lidx, caps[ll], w.counts[ll], e->convs.back().d.c_out, batch_size,
+                             e->levels[ll].shape, 1, out_batch_stride, (float *)dense_out, st);
   if (rc) return rc;
   if (forked) BEVB200_CUDA(cudaStreamWaitEvent(st, e->events[1 + nr], 0));   // join (also what a graph capture needs)
   return BEVB200_OK;
+}
+
+extern "C" {
+
+int bevb200_encoder_forward(bevb200_encoder_t *e, const void *params, const float *voxel_features,
+                            const int32_t *coors, int max_voxels, const int32_t *n_voxels_dev, int batch_size,
+                            const int32_t *user_caps, float *dense_out, long long out_batch_stride,
+                            int32_t *status_dev, void *workspace, size_t workspace_bytes, void *stream,
+                            void *rulebook_stream) {
+  return enc_forward(e, false, params, voxel_features, coors, max_voxels, n_voxels_dev, batch_size, user_caps,
+                     dense_out, out_batch_stride, status_dev, workspace, workspace_bytes, stream, rulebook_stream);
+}
+
+int bevb200_encoder_forward_f16(bevb200_encoder_t *e, const void *params, const void *voxel_features,
+                                const int32_t *coors, int max_voxels, const int32_t *n_voxels_dev, int batch_size,
+                                const int32_t *user_caps, void *dense_out, long long out_batch_stride,
+                                int32_t *status_dev, void *workspace, size_t workspace_bytes, void *stream,
+                                void *rulebook_stream) {
+  return enc_forward(e, true, params, voxel_features, coors, max_voxels, n_voxels_dev, batch_size, user_caps,
+                     dense_out, out_batch_stride, status_dev, workspace, workspace_bytes, stream, rulebook_stream);
 }
 
 }  // extern "C"
@@ -456,6 +519,9 @@ int bevb200_encoder_forward(bevb200_encoder_t *e, const void *params, const floa
 //   filter gradient on the saved input image (spconv_wgrad_tc_split) | input gradient = the forward kernel on W^T:
 //   SubM: the forward table with mirrored offsets, strided: a transposed table; a block's identity gradient rides in
 //   the residual epilogue of the input gradient of the conv that reads the identity.
+// FP16 plans (BEVB200_PREC_FP16) run the same sequence with fp16 rows: the conv writes z16 = fp16(acc), the statistics
+// and the BN backward read z16, the apply writes the fp16 image y16 that the next conv gathers, dense() scatters the
+// last y16, and dz is rounded once to an fp16 image that both the filter gradient and the input gradient read.
 #include "tc_ptx.cuh"
 
 namespace bevb200 {
@@ -467,8 +533,18 @@ static int stat_chunks(int cap) { return cap > 0 ? (cap + kStatRows - 1) / kStat
 
 __device__ __forceinline__ int enc_rows(const int32_t *n_dev, int cap) { return min(max(__ldg(n_dev), 0), cap); }
 
-// value of channel ch of row r of a split image with c channels per row
+__device__ __forceinline__ float ld_f(const float *p) { return *p; }
+__device__ __forceinline__ float ld_f(const __half *p) { return __half2float(*p); }
+__device__ __forceinline__ void st_f(float *p, float v) { *p = v; }
+__device__ __forceinline__ void st_f(__half *p, float v) { *p = __float2half_rn(v); }
+// rows of the BF16x3 / FP16 forms: pre-BN rows z and dz are fp32 / fp16
+template <bool F16>
+using enc_row_t = typename std::conditional<F16, __half, float>::type;
+
+// value of channel ch of row r of a split image (F16: an fp16 image) with c channels per row
+template <bool F16 = false>
 __device__ __forceinline__ float split_value(const uint8_t *img, long long r, int c, int ch) {
+  if (F16) return __half2float(reinterpret_cast<const __half *>(img)[r * c + ch]);
   const uint8_t *p = img + r * (c * 4) + (ch >> 4) * 64 + (ch & 15) * 2;
   const uint32_t h = *reinterpret_cast<const uint16_t *>(p), l = *reinterpret_cast<const uint16_t *>(p + 32);
   return __uint_as_float(h << 16) + __uint_as_float(l << 16);
@@ -480,8 +556,9 @@ __device__ __forceinline__ float split_value(const uint8_t *img, long long r, in
   const int ch = threadIdx.x % (c), grp = threadIdx.x / (c)
 
 // per-channel sums of v and v^2 (double) over the rows of one chunk; the groups add in ascending order
+template <typename T>
 __global__ void __launch_bounds__(kStatThreads)
-    bn_stats_partial_kernel(const float *__restrict__ z, const int32_t *__restrict__ n_dev, int cap, int c,
+    bn_stats_partial_kernel(const T *__restrict__ z, const int32_t *__restrict__ n_dev, int cap, int c,
                             double *__restrict__ partial) {
   __shared__ double sh[2][kStatThreads];
   STAT_THREAD(c);
@@ -491,7 +568,7 @@ __global__ void __launch_bounds__(kStatThreads)
   double s = 0.0, ss = 0.0;
   if (grp < groups)
     for (int r = r0 + grp; r < r1; r += groups) {
-      const double v = z[(long long)r * c + ch];
+      const double v = ld_f(z + (long long)r * c + ch);
       s += v;
       ss += v * v;
     }
@@ -551,8 +628,10 @@ __global__ void __launch_bounds__(kStatThreads)
   }
 }
 
-// y = relu(z scale + shift [+ residual image]) -> split image (and fp32 rows); one thread per (row, 8 channels)
-__global__ void bn_apply_kernel(const float *__restrict__ z, const float *__restrict__ stat,
+// y = relu(z scale + shift [+ residual image]) -> split image (and fp32 rows); one thread per (row, 8 channels).
+// F16: z, the residual and y are fp16 images; y is rounded once.
+template <bool F16>
+__global__ void bn_apply_kernel(const enc_row_t<F16> *__restrict__ z, const float *__restrict__ stat,
                                 const uint8_t *__restrict__ res_split, const int32_t *__restrict__ n_dev, int cap,
                                 int c, int relu, uint8_t *__restrict__ ysplit, float *__restrict__ yf32) {
   const int n = enc_rows(n_dev, cap);
@@ -562,14 +641,14 @@ __global__ void bn_apply_kernel(const float *__restrict__ z, const float *__rest
        t += (long long)gridDim.x * blockDim.x) {
     const int j = (int)(t % per_row), c0 = 8 * j;
     const long long r = t / per_row;
-    const float4 a = *reinterpret_cast<const float4 *>(z + r * c + c0);
-    const float4 b = *reinterpret_cast<const float4 *>(z + r * c + c0 + 4);
-    float y[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+    float y[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) y[e] = ld_f(z + r * c + c0 + e);
 #pragma unroll
     for (int e = 0; e < 8; ++e) y[e] = y[e] * __ldg(stat + 2 * c + c0 + e) + __ldg(stat + 3 * c + c0 + e);
     if (res_split) {
 #pragma unroll
-      for (int e = 0; e < 8; ++e) y[e] += split_value(res_split, r, c, c0 + e);
+      for (int e = 0; e < 8; ++e) y[e] += split_value<F16>(res_split, r, c, c0 + e);
     }
     if (relu) {
 #pragma unroll
@@ -579,17 +658,24 @@ __global__ void bn_apply_kernel(const float *__restrict__ z, const float *__rest
       *reinterpret_cast<float4 *>(yf32 + r * c + c0) = make_float4(y[0], y[1], y[2], y[3]);
       *reinterpret_cast<float4 *>(yf32 + r * c + c0 + 4) = make_float4(y[4], y[5], y[6], y[7]);
     }
-    uint32_t hi[4], lo[4];
+    if constexpr (F16) {
+      __half *dst = reinterpret_cast<__half *>(ysplit) + r * c + c0;
 #pragma unroll
-    for (int e = 0; e < 8; e += 2) split_pair(y[e], y[e + 1], hi[e / 2], lo[e / 2]);
-    uint8_t *dst = ysplit + r * (c * 4) + (j >> 1) * 64 + (j & 1) * 16;
-    *reinterpret_cast<uint4 *>(dst) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-    *reinterpret_cast<uint4 *>(dst + 32) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+      for (int e = 0; e < 8; ++e) dst[e] = __float2half_rn(y[e]);
+    } else {
+      uint32_t hi[4], lo[4];
+#pragma unroll
+      for (int e = 0; e < 8; e += 2) split_pair(y[e], y[e + 1], hi[e / 2], lo[e / 2]);
+      uint8_t *dst = ysplit + r * (c * 4) + (j >> 1) * 64 + (j & 1) * 16;
+      *reinterpret_cast<uint4 *>(dst) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+      *reinterpret_cast<uint4 *>(dst + 32) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+    }
   }
 }
 
 // rows of the last level from the dense gradient (the inverse of sparse_to_dense with z_major)
-__global__ void dense_gather_kernel(const float *__restrict__ dense, const int32_t *__restrict__ idx,
+template <typename T>
+__global__ void dense_gather_kernel(const T *__restrict__ dense, const int32_t *__restrict__ idx,
                                     const int32_t *__restrict__ n_dev, int cap, int c, int batch, int X, int Y, int Z,
                                     long long out_batch_stride, float *__restrict__ rows) {
   const int n = enc_rows(n_dev, cap);
@@ -601,15 +687,16 @@ __global__ void dense_gather_kernel(const float *__restrict__ dense, const int32
     float v = 0.f;
     if ((unsigned)p.x < (unsigned)batch && (unsigned)p.y < (unsigned)X && (unsigned)p.z < (unsigned)Y &&
         (unsigned)p.w < (unsigned)Z)
-      v = dense[p.x * out_batch_stride + ch * plane + ((long long)p.w * X + p.y) * Y + p.z];
+      v = ld_f(dense + p.x * out_batch_stride + ch * plane + ((long long)p.w * X + p.y) * Y + p.z);
     rows[(long long)i * c + ch] = v;
   }
 }
 
 // ReLU mask applied to g in place, then per-channel sums of g and g x^ (x^ = (z - mean) invstd) per chunk
+template <bool F16>
 __global__ void __launch_bounds__(kStatThreads)
     bn_bwd_partial_kernel(float *__restrict__ g, const uint8_t *__restrict__ ysplit, const float *__restrict__ yf32,
-                          int relu, const float *__restrict__ z, const float *__restrict__ stat,
+                          int relu, const enc_row_t<F16> *__restrict__ z, const float *__restrict__ stat,
                           const int32_t *__restrict__ n_dev, int cap, int c, double *__restrict__ partial) {
   __shared__ double sh[2][kStatThreads];
   STAT_THREAD(c);
@@ -623,12 +710,12 @@ __global__ void __launch_bounds__(kStatThreads)
       const long long e = (long long)r * c + ch;
       float gv = g[e];
       if (relu) {
-        const float y = yf32 ? yf32[e] : split_value(ysplit, r, c, ch);
+        const float y = yf32 ? yf32[e] : split_value<F16>(ysplit, r, c, ch);
         if (!(y > 0.f)) gv = 0.f;
         g[e] = gv;
       }
       s += gv;
-      sx += (double)gv * (double)((z[e] - mean) * invstd);
+      sx += (double)gv * (double)((ld_f(z + e) - mean) * invstd);
     }
   }
   sh[0][threadIdx.x] = s;
@@ -657,17 +744,18 @@ __global__ void __launch_bounds__(kStatThreads)
   coef[c + ch] = n > 0 ? (float)(sx / n) : 0.f;
 }
 
-// dz = gamma invstd (g - mean(g) - x^ mean(g x^))
-__global__ void bn_bwd_apply_kernel(const float *__restrict__ g, const float *__restrict__ z,
+// dz = gamma invstd (g - mean(g) - x^ mean(g x^)); F16: z16 in, dz rounded once to fp16
+template <bool F16>
+__global__ void bn_bwd_apply_kernel(const float *__restrict__ g, const enc_row_t<F16> *__restrict__ z,
                                     const float *__restrict__ stat, const float *__restrict__ coef,
-                                    const int32_t *__restrict__ n_dev, int cap, int c, float *__restrict__ dz) {
+                                    const int32_t *__restrict__ n_dev, int cap, int c, enc_row_t<F16> *__restrict__ dz) {
   const int n = enc_rows(n_dev, cap);
   const long long total = (long long)n * c;
   for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total;
        t += (long long)gridDim.x * blockDim.x) {
     const int ch = (int)(t % c);
-    const float xh = (z[t] - __ldg(stat + ch)) * __ldg(stat + c + ch);
-    dz[t] = __ldg(stat + 2 * c + ch) * (g[t] - __ldg(coef + ch) - xh * __ldg(coef + c + ch));
+    const float xh = (ld_f(z + t) - __ldg(stat + ch)) * __ldg(stat + c + ch);
+    st_f(dz + t, __ldg(stat + 2 * c + ch) * (g[t] - __ldg(coef + ch) - xh * __ldg(coef + c + ch)));
   }
 }
 
@@ -722,14 +810,15 @@ __global__ void enc_widen_image_kernel(const uint8_t *__restrict__ src, int c_sr
 }
 
 // input gradient rows [cap, c_eff] -> grad_voxel_features [rows, c_in]: the valid rows narrowed, the rest zero
+template <typename T>
 __global__ void enc_narrow_grad_kernel(const float *__restrict__ src, int c_eff, const int32_t *__restrict__ n_dev,
-                                       int cap, int rows, int c_in, float *__restrict__ dst) {
+                                       int cap, int rows, int c_in, T *__restrict__ dst) {
   const int n = enc_rows(n_dev, cap);
   const long long total = (long long)rows * c_in;
   for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total;
        t += (long long)gridDim.x * blockDim.x) {
     const long long r = t / c_in;
-    dst[t] = r < n ? src[r * c_eff + t % c_in] : 0.f;
+    st_f(dst + t, r < n ? src[r * c_eff + t % c_in] : 0.f);
   }
 }
 
@@ -737,11 +826,11 @@ __global__ void enc_narrow_grad_kernel(const float *__restrict__ src, int c_eff,
 struct ETrain {
   EWs w;
   char *params;
-  uint8_t *in_split;              // level-0 split image of the voxel features
-  std::vector<float *> z;         // pre-BN rows per conv
-  std::vector<uint8_t *> y;       // split image of every conv's output
+  uint8_t *in_split;              // level-0 split image (FP16: fp16 image) of the voxel features
+  std::vector<void *> z;          // pre-BN rows per conv: fp32 (FP16: z16 = fp16(acc))
+  std::vector<uint8_t *> y;       // split image (FP16: fp16 image) of every conv's output
   std::vector<float *> stat;      // per conv [mean | invstd | scale | shift][c_out]
-  float *y_last;                  // fp32 rows of the last conv (dense() and its ReLU mask)
+  float *y_last;                  // BF16x3: fp32 rows of the last conv (dense() and its ReLU mask)
   double *partial;
 };
 
@@ -750,25 +839,27 @@ static size_t train_layout(const bevb200_encoder *e, const std::vector<int> &cap
   Arena a(base, bytes);
   enc_layout_into(e, caps, batch, a, false, &t->w);
   t->params = a.take<char>(e->param_bytes);
-  t->in_split = a.take<uint8_t>((size_t)caps[0] * e->c0_eff * 4);
+  const size_t ib = enc_img_bytes(e);
+  t->in_split = a.take<uint8_t>((size_t)caps[0] * e->c0_eff * ib);
   const size_t n = e->convs.size();
   t->z.resize(n); t->y.resize(n); t->stat.resize(n);
   size_t part = 0;
   for (size_t i = 0; i < n; ++i) {
     const EConv &cv = e->convs[i];
     const size_t cap = caps[cv.level_out];
-    t->z[i] = a.take<float>(cap * cv.d.c_out);
-    t->y[i] = a.take<uint8_t>(cap * cv.d.c_out * 4);
+    t->z[i] = a.take<uint8_t>(cap * cv.d.c_out * (enc_f16(e) ? 2 : 4));
+    t->y[i] = a.take<uint8_t>(cap * cv.d.c_out * ib);
     t->stat[i] = a.take<float>(4 * (size_t)cv.d.c_out);
     part = std::max(part, (size_t)stat_chunks(caps[cv.level_out]) * 2 * cv.d.c_out);
   }
-  t->y_last = a.take<float>((size_t)caps.back() * e->convs.back().d.c_out);
+  t->y_last = enc_f16(e) ? nullptr : a.take<float>((size_t)caps.back() * e->convs.back().d.c_out);
   t->partial = a.take<double>(part);
   return a.off;
 }
 
 struct EBwd {
-  std::vector<float *> d[2], dz;  // per level: two gradient row buffers and the dz rows
+  std::vector<float *> d[2];      // per level: two gradient row buffers
+  std::vector<void *> dz;         // per level: the dz rows (FP16: the fp16 image of dz)
   int32_t *nbr_t;
   float *wt, *coef, *din0;
   char *packed, *wg;
@@ -785,18 +876,23 @@ static size_t bwd_layout(const bevb200_encoder *e, const std::vector<int> &caps,
     const size_t n = (size_t)caps[l] * e->levels[l].c_max;
     b->d[0][l] = a.take<float>(n);
     b->d[1][l] = a.take<float>(n);
-    b->dz[l] = a.take<float>(n);
+    b->dz[l] = a.take<uint8_t>(n * (enc_f16(e) ? 2 : 4));
   }
   size_t nbrt = 0, wt = 0, pk = 0, wg = 0, fw = 0, g16 = 0, part = 0, cmax = 0;
   for (const EConv &cv : e->convs) {
     const int li = cv.level_in, lo = cv.level_out, cip = spconv_v6_cin_eff(cv.d.c_in);
     if (!cv.d.subm) nbrt = std::max(nbrt, (size_t)cv.kvol * caps[li]);
     wt = std::max(wt, (size_t)cv.kvol * cv.d.c_out * cip);
-    pk = std::max(pk, spconv_v6_packed_bytes(cv.d.c_out, cip, cv.kvol));
-    wg = std::max(wg, spconv_wgrad_tc_split_workspace_bytes(caps[lo], cv.d.c_in, cv.d.c_out, cv.kvol));
-    const int wide = spconv_wgrad_tc_image_channels(cv.d.c_in);
-    if (wide != cip) fw = std::max(fw, (size_t)caps[li] * wide * 4);
-    if (cv.d.c_out == 16) g16 = std::max(g16, (size_t)caps[lo] * 64);
+    if (enc_f16(e)) {   // the fp16 images are read in place: no widened or second image of dz
+      pk = std::max(pk, spconv_v6_packed_bytes_f16(cv.d.c_out, cip, cv.kvol));
+      wg = std::max(wg, spconv_wgrad_tc_f16_workspace_bytes(caps[lo], cv.d.c_in, cv.d.c_out, cv.kvol));
+    } else {
+      pk = std::max(pk, spconv_v6_packed_bytes(cv.d.c_out, cip, cv.kvol));
+      wg = std::max(wg, spconv_wgrad_tc_split_workspace_bytes(caps[lo], cv.d.c_in, cv.d.c_out, cv.kvol));
+      const int wide = spconv_wgrad_tc_image_channels(cv.d.c_in);
+      if (wide != cip) fw = std::max(fw, (size_t)caps[li] * wide * 4);
+      if (cv.d.c_out == 16) g16 = std::max(g16, (size_t)caps[lo] * 64);
+    }
     part = std::max(part, (size_t)stat_chunks(caps[lo]) * 2 * cv.d.c_out);
     cmax = std::max(cmax, (size_t)cv.d.c_out);
   }
@@ -840,11 +936,17 @@ int bevb200_encoder_train_saved(const bevb200_encoder_t *e, int max_voxels, int 
   return BEVB200_OK;
 }
 
-int bevb200_encoder_forward_train(bevb200_encoder_t *e, const float *const *weights, const bevb200_encoder_bn_t *bn,
-                                  const float *voxel_features, const int32_t *coors, int max_voxels,
-                                  const int32_t *n_voxels_dev, int batch_size, const int32_t *user_caps,
-                                  float *dense_out, long long out_batch_stride, int32_t *status_dev, void *state,
-                                  size_t state_bytes, void *stream, void *rulebook_stream) {
+}  // extern "C"
+
+static int enc_forward_train(bevb200_encoder_t *e, bool f16, const float *const *weights, const bevb200_encoder_bn_t *bn,
+                             const void *voxel_features, const int32_t *coors, int max_voxels,
+                             const int32_t *n_voxels_dev, int batch_size, const int32_t *user_caps, void *dense_out,
+                             long long out_batch_stride, int32_t *status_dev, void *state, size_t state_bytes,
+                             void *stream, void *rulebook_stream) {
+  // the precision first: a call of the wrong family is refused before any other argument is looked at
+  BEVB200_REQUIRE(e, "null plan");
+  BEVB200_REQUIRE(enc_f16(e) == f16, f16 ? "the _f16 calls need a plan set to BEVB200_PREC_FP16"
+                                         : "an fp16 plan runs the _f16 calls");
   BEVB200_REQUIRE(e && weights && bn && dense_out && status_dev && max_voxels > 0 && batch_size > 0, "bad argument");
   BEVB200_REQUIRE(voxel_features && coors, "null input");
   const size_t nc = e->convs.size();
@@ -867,11 +969,13 @@ int bevb200_encoder_forward_train(bevb200_encoder_t *e, const float *const *weig
   if (rc) return rc;
   // the live weights, packed on every call (a graph replay after an in-place optimizer step sees the new values)
   for (size_t i = 0; i < nc; ++i) {
-    const EConv &cv = e->convs[i];
-    rc = spconv_v6_pack_weights(weights[i], cv.d.c_in, cv.d.c_out, cv.kvol, t.params + cv.packed_off, st);
+    rc = enc_pack(e, e->convs[i], weights[i], t.params, st);
     if (rc) return rc;
   }
-  rc = spconv_v6_split_rows(voxel_features, caps[0], n_voxels_dev, e->in_channels, e->c0_eff, t.in_split, st);
+  rc = f16 ? spconv_v6_f16_rows((const __half *)voxel_features, caps[0], n_voxels_dev, e->in_channels, e->c0_eff,
+                                t.in_split, st)
+           : spconv_v6_split_rows((const float *)voxel_features, caps[0], n_voxels_dev, e->in_channels, e->c0_eff,
+                                  t.in_split, st);
   if (rc) return rc;
   std::vector<char> rb_waited(nr, 0);
   const uint8_t *cur = t.in_split;
@@ -883,25 +987,65 @@ int bevb200_encoder_forward_train(bevb200_encoder_t *e, const float *const *weig
     }
     const int lo = cv.level_out, c = cv.d.c_out;
     const bool last = i + 1 == nc;
-    rc = spconv_v6_forward(cur, t.params + cv.packed_off, w.nbr[cv.rulebook], (long long)caps[lo], caps[cv.level_in],
-                           caps[lo], w.counts[lo], cv.c_in_eff, c, cv.kvol, nullptr, nullptr, nullptr, nullptr, 0,
-                           t.z[i], nullptr, st);
-    if (rc) return rc;
-    BEVB200_LAUNCH(bn_stats_partial_kernel, stat_chunks(caps[lo]), kStatThreads, 0, st, t.z[i], w.counts[lo], caps[lo],
-                   c, t.partial);
+    const uint8_t *res = cv.d.residual_from >= 0 ? t.y[cv.d.residual_from] : nullptr;
+    const int grid = grid_for((long long)caps[lo] * (c / 8), 256);
+    if (f16) {   // z16 = fp16(acc)
+      rc = spconv_v6_forward_f16(cur, t.params + cv.packed_off, w.nbr[cv.rulebook], (long long)caps[lo],
+                                 caps[cv.level_in], caps[lo], w.counts[lo], cv.c_in_eff, c, cv.kvol, nullptr, nullptr,
+                                 nullptr, nullptr, 0, nullptr, t.z[i], st);
+      if (rc) return rc;
+      BEVB200_LAUNCH(bn_stats_partial_kernel<__half>, stat_chunks(caps[lo]), kStatThreads, 0, st,
+                     (const __half *)t.z[i], w.counts[lo], caps[lo], c, t.partial);
+    } else {
+      rc = spconv_v6_forward(cur, t.params + cv.packed_off, w.nbr[cv.rulebook], (long long)caps[lo], caps[cv.level_in],
+                             caps[lo], w.counts[lo], cv.c_in_eff, c, cv.kvol, nullptr, nullptr, nullptr, nullptr, 0,
+                             (float *)t.z[i], nullptr, st);
+      if (rc) return rc;
+      BEVB200_LAUNCH(bn_stats_partial_kernel<float>, stat_chunks(caps[lo]), kStatThreads, 0, st, (const float *)t.z[i],
+                     w.counts[lo], caps[lo], c, t.partial);
+    }
     BEVB200_LAUNCH(bn_stats_reduce_kernel, 1, kStatThreads, 0, st, t.partial, w.counts[lo], caps[lo], c, bn[i],
                    t.stat[i], status_dev);
-    BEVB200_LAUNCH(bn_apply_kernel, grid_for((long long)caps[lo] * (c / 8), 256), 256, 0, st, t.z[i], t.stat[i],
-                   cv.d.residual_from >= 0 ? t.y[cv.d.residual_from] : nullptr, w.counts[lo], caps[lo], c, cv.d.relu,
-                   t.y[i], last ? t.y_last : nullptr);
+    if (f16)
+      BEVB200_LAUNCH(bn_apply_kernel<true>, grid, 256, 0, st, (const __half *)t.z[i], t.stat[i], res, w.counts[lo],
+                     caps[lo], c, cv.d.relu, t.y[i], (float *)nullptr);
+    else
+      BEVB200_LAUNCH(bn_apply_kernel<false>, grid, 256, 0, st, (const float *)t.z[i], t.stat[i], res, w.counts[lo],
+                     caps[lo], c, cv.d.relu, t.y[i], last ? t.y_last : nullptr);
     cur = t.y[i];
   }
   const size_t ll = nl - 1;
-  rc = sparse_to_dense(t.y_last, w.indices[ll] ? w.indices[ll] : coors, caps[ll], w.counts[ll], e->convs.back().d.c_out,
-                       batch_size, e->levels[ll].shape, 1, out_batch_stride, dense_out, st);
+  const int32_t *lidx = w.indices[ll] ? w.indices[ll] : coors;
+  rc = f16 ? sparse_to_dense((const __half *)cur, lidx, caps[ll], w.counts[ll], e->convs.back().d.c_out, batch_size,
+                             e->levels[ll].shape, 1, out_batch_stride, (__half *)dense_out, st)
+           : sparse_to_dense(t.y_last, lidx, caps[ll], w.counts[ll], e->convs.back().d.c_out, batch_size,
+                             e->levels[ll].shape, 1, out_batch_stride, (float *)dense_out, st);
   if (rc) return rc;
   if (forked) BEVB200_CUDA(cudaStreamWaitEvent(st, e->events[1 + nr], 0));
   return BEVB200_OK;
+}
+
+extern "C" {
+
+int bevb200_encoder_forward_train(bevb200_encoder_t *e, const float *const *weights, const bevb200_encoder_bn_t *bn,
+                                  const float *voxel_features, const int32_t *coors, int max_voxels,
+                                  const int32_t *n_voxels_dev, int batch_size, const int32_t *user_caps,
+                                  float *dense_out, long long out_batch_stride, int32_t *status_dev, void *state,
+                                  size_t state_bytes, void *stream, void *rulebook_stream) {
+  return enc_forward_train(e, false, weights, bn, voxel_features, coors, max_voxels, n_voxels_dev, batch_size,
+                           user_caps, dense_out, out_batch_stride, status_dev, state, state_bytes, stream,
+                           rulebook_stream);
+}
+
+int bevb200_encoder_forward_train_f16(bevb200_encoder_t *e, const float *const *weights,
+                                      const bevb200_encoder_bn_t *bn, const void *voxel_features,
+                                      const int32_t *coors, int max_voxels, const int32_t *n_voxels_dev,
+                                      int batch_size, const int32_t *user_caps, void *dense_out,
+                                      long long out_batch_stride, int32_t *status_dev, void *state,
+                                      size_t state_bytes, void *stream, void *rulebook_stream) {
+  return enc_forward_train(e, true, weights, bn, voxel_features, coors, max_voxels, n_voxels_dev, batch_size,
+                           user_caps, dense_out, out_batch_stride, status_dev, state, state_bytes, stream,
+                           rulebook_stream);
 }
 
 size_t bevb200_encoder_backward_workspace_bytes(const bevb200_encoder_t *e, int max_voxels, int batch_size,
@@ -913,11 +1057,17 @@ size_t bevb200_encoder_backward_workspace_bytes(const bevb200_encoder_t *e, int 
   return bwd_layout(e, caps, nullptr, 0, &b);
 }
 
-int bevb200_encoder_backward(const bevb200_encoder_t *e, const float *const *weights, const void *state,
-                             size_t state_bytes, int max_voxels, int batch_size, const int32_t *user_caps,
-                             const float *grad_dense, long long out_batch_stride, float *grad_voxel_features,
-                             float *const *grad_weights, float *const *grad_bn_weight, float *const *grad_bn_bias,
-                             void *workspace, size_t workspace_bytes, void *stream) {
+}  // extern "C"
+
+static int enc_backward(const bevb200_encoder_t *e, bool f16, const float *const *weights, const void *state,
+                        size_t state_bytes, int max_voxels, int batch_size, const int32_t *user_caps,
+                        const void *grad_dense, long long out_batch_stride, void *grad_voxel_features,
+                        float *const *grad_weights, float *const *grad_bn_weight, float *const *grad_bn_bias,
+                        void *workspace, size_t workspace_bytes, void *stream) {
+  // the precision first: a call of the wrong family is refused before any other argument is looked at
+  BEVB200_REQUIRE(e, "null plan");
+  BEVB200_REQUIRE(enc_f16(e) == f16, f16 ? "the _f16 calls need a plan set to BEVB200_PREC_FP16"
+                                         : "an fp16 plan runs the _f16 calls");
   BEVB200_REQUIRE(e && weights && state && grad_dense && grad_weights && grad_bn_weight && grad_bn_bias &&
                       max_voxels > 0 && batch_size > 0, "bad argument");
   const size_t nc = e->convs.size(), nl = e->levels.size();
@@ -946,8 +1096,14 @@ int bevb200_encoder_backward(const bevb200_encoder_t *e, const float *const *wei
   {
     const int *s = e->levels[ll].shape;
     const int c = e->convs.back().d.c_out;
-    BEVB200_LAUNCH(dense_gather_kernel, grid_for((long long)caps[ll] * c, 256), 256, 0, st, grad_dense, w.indices[ll],
-                   w.counts[ll], caps[ll], c, batch_size, s[0], s[1], s[2], out_batch_stride, b.d[0][ll]);
+    if (f16)
+      BEVB200_LAUNCH(dense_gather_kernel<__half>, grid_for((long long)caps[ll] * c, 256), 256, 0, st,
+                     (const __half *)grad_dense, w.indices[ll], w.counts[ll], caps[ll], c, batch_size, s[0], s[1], s[2],
+                     out_batch_stride, b.d[0][ll]);
+    else
+      BEVB200_LAUNCH(dense_gather_kernel<float>, grid_for((long long)caps[ll] * c, 256), 256, 0, st,
+                     (const float *)grad_dense, w.indices[ll], w.counts[ll], caps[ll], c, batch_size, s[0], s[1], s[2],
+                     out_batch_stride, b.d[0][ll]);
   }
   std::vector<int> cur(nl, 0), held(nl, -1);
   const float *pending = nullptr;   // a block's identity gradient, added to the input gradient of conv pending_for
@@ -959,12 +1115,22 @@ int bevb200_encoder_backward(const bevb200_encoder_t *e, const float *const *wei
     const bool last = i + 1 == (int)nc;
     float *g = b.d[cur[lo]][lo];
     // ReLU mask, BN backward
-    BEVB200_LAUNCH(bn_bwd_partial_kernel, stat_chunks(caps[lo]), kStatThreads, 0, st, g, t.y[i],
-                   last ? t.y_last : nullptr, cv.d.relu, t.z[i], t.stat[i], w.counts[lo], caps[lo], c, b.partial);
+    if (f16)
+      BEVB200_LAUNCH(bn_bwd_partial_kernel<true>, stat_chunks(caps[lo]), kStatThreads, 0, st, g, t.y[i],
+                     (const float *)nullptr, cv.d.relu, (const __half *)t.z[i], t.stat[i], w.counts[lo], caps[lo], c,
+                     b.partial);
+    else
+      BEVB200_LAUNCH(bn_bwd_partial_kernel<false>, stat_chunks(caps[lo]), kStatThreads, 0, st, g, t.y[i],
+                     last ? t.y_last : nullptr, cv.d.relu, (const float *)t.z[i], t.stat[i], w.counts[lo], caps[lo], c,
+                     b.partial);
     BEVB200_LAUNCH(bn_bwd_reduce_kernel, 1, kStatThreads, 0, st, b.partial, w.counts[lo], caps[lo], c,
                    grad_bn_weight[i], grad_bn_bias[i], b.coef);
-    BEVB200_LAUNCH(bn_bwd_apply_kernel, grid_for((long long)caps[lo] * c, 256), 256, 0, st, g, t.z[i], t.stat[i],
-                   b.coef, w.counts[lo], caps[lo], c, b.dz[lo]);
+    if (f16)
+      BEVB200_LAUNCH(bn_bwd_apply_kernel<true>, grid_for((long long)caps[lo] * c, 256), 256, 0, st, g,
+                     (const __half *)t.z[i], t.stat[i], b.coef, w.counts[lo], caps[lo], c, (__half *)b.dz[lo]);
+    else
+      BEVB200_LAUNCH(bn_bwd_apply_kernel<false>, grid_for((long long)caps[lo] * c, 256), 256, 0, st, g,
+                     (const float *)t.z[i], t.stat[i], b.coef, w.counts[lo], caps[lo], c, (float *)b.dz[lo]);
     if (cv.d.residual_from >= 0) {   // g (after the mask) is also the gradient of the identity
       BEVB200_REQUIRE(pending_for < 0, "two pending residual gradients");
       held[lo] = cur[lo];
@@ -974,23 +1140,31 @@ int bevb200_encoder_backward(const bevb200_encoder_t *e, const float *const *wei
     // filter gradient on the saved input image
     const int cip = spconv_v6_cin_eff(cv.d.c_in), wide = spconv_wgrad_tc_image_channels(cv.d.c_in);
     const uint8_t *fimg = i == 0 ? t.in_split : t.y[i - 1];
-    if (wide != cip) {
-      BEVB200_LAUNCH(enc_widen_image_kernel, grid_for((long long)caps[li] * (wide / 4), 256), 256, 0, st, fimg, cip,
-                     wide, w.counts[li], caps[li], b.fwide);
-      fimg = b.fwide;
-    }
-    rc = spconv_wgrad_tc_split(fimg, b.dz[lo], w.nbr[cv.rulebook], caps[li], caps[lo], w.counts[lo], cv.d.c_in, c,
+    if (f16) {
+      rc = spconv_wgrad_tc_f16(fimg, cip, b.dz[lo], w.nbr[cv.rulebook], caps[li], caps[lo], w.counts[lo], cv.d.c_in, c,
                                cv.kvol, grad_weights[i], b.wg, st);
+    } else {
+      if (wide != cip) {
+        BEVB200_LAUNCH(enc_widen_image_kernel, grid_for((long long)caps[li] * (wide / 4), 256), 256, 0, st, fimg, cip,
+                       wide, w.counts[li], caps[li], b.fwide);
+        fimg = b.fwide;
+      }
+      rc = spconv_wgrad_tc_split(fimg, (const float *)b.dz[lo], w.nbr[cv.rulebook], caps[li], caps[lo], w.counts[lo],
+                                 cv.d.c_in, c, cv.kvol, grad_weights[i], b.wg, st);
+    }
     if (rc) return rc;
     // input gradient
     if (i == 0 && grad_voxel_features == nullptr) break;
     BEVB200_LAUNCH(enc_weight_t_kernel, grid_for((long long)cv.kvol * c * cip, 256), 256, 0, st, weights[i], cv.kvol,
                    cv.d.c_in, c, cip, cv.d.subm, b.wt);
-    rc = spconv_v6_pack_weights(b.wt, c, cip, cv.kvol, b.packed, st);
+    rc = f16 ? spconv_v6_pack_weights_f16(b.wt, c, cip, cv.kvol, b.packed, st)
+             : spconv_v6_pack_weights(b.wt, c, cip, cv.kvol, b.packed, st);
     if (rc) return rc;
     const void *gimg = b.wg;   // c_out 32 / 64 / 128: the filter gradient's image of dz is the forward's row image
-    if (c == 16) {
-      rc = spconv_v6_split_rows(b.dz[lo], caps[lo], w.counts[lo], c, c, b.g16, st);
+    if (f16) {
+      gimg = b.dz[lo];         // the one fp16 image of dz
+    } else if (c == 16) {
+      rc = spconv_v6_split_rows((const float *)b.dz[lo], caps[lo], w.counts[lo], c, c, b.g16, st);
       if (rc) return rc;
       gimg = b.g16;
     }
@@ -1011,8 +1185,9 @@ int bevb200_encoder_backward(const bevb200_encoder_t *e, const float *const *wei
       oi = (li == lo && held[lo] == cur[lo]) ? cur[lo] ^ 1 : (li == lo ? cur[lo] : 0);
       out = b.d[oi][li];
     }
-    rc = spconv_v6_forward(gimg, b.packed, table, (long long)caps[li], caps[lo], caps[li], w.counts[li], c, cip,
-                           cv.kvol, nullptr, nullptr, res, nullptr, 0, out, nullptr, st);
+    rc = (f16 ? spconv_v6_forward_f16 : spconv_v6_forward)(gimg, b.packed, table, (long long)caps[li], caps[lo],
+                                                           caps[li], w.counts[li], c, cip, cv.kvol, nullptr, nullptr,
+                                                           res, nullptr, 0, out, nullptr, st);
     if (rc) return rc;
     if (res) {
       pending = nullptr;
@@ -1020,13 +1195,41 @@ int bevb200_encoder_backward(const bevb200_encoder_t *e, const float *const *wei
       held[lo] = -1;
     }
     if (i == 0) {
-      BEVB200_LAUNCH(enc_narrow_grad_kernel, grid_for((long long)max_voxels * e->in_channels, 256), 256, 0, st,
-                     b.din0, e->c0_eff, w.counts[0], caps[0], max_voxels, e->in_channels, grad_voxel_features);
+      if (f16)
+        BEVB200_LAUNCH(enc_narrow_grad_kernel<__half>, grid_for((long long)max_voxels * e->in_channels, 256), 256, 0,
+                       st, b.din0, e->c0_eff, w.counts[0], caps[0], max_voxels, e->in_channels,
+                       (__half *)grad_voxel_features);
+      else
+        BEVB200_LAUNCH(enc_narrow_grad_kernel<float>, grid_for((long long)max_voxels * e->in_channels, 256), 256, 0,
+                       st, b.din0, e->c0_eff, w.counts[0], caps[0], max_voxels, e->in_channels,
+                       (float *)grad_voxel_features);
     } else {
       cur[li] = oi;
     }
   }
   return BEVB200_OK;
+}
+
+extern "C" {
+
+int bevb200_encoder_backward(const bevb200_encoder_t *e, const float *const *weights, const void *state,
+                             size_t state_bytes, int max_voxels, int batch_size, const int32_t *user_caps,
+                             const float *grad_dense, long long out_batch_stride, float *grad_voxel_features,
+                             float *const *grad_weights, float *const *grad_bn_weight, float *const *grad_bn_bias,
+                             void *workspace, size_t workspace_bytes, void *stream) {
+  return enc_backward(e, false, weights, state, state_bytes, max_voxels, batch_size, user_caps, grad_dense,
+                      out_batch_stride, grad_voxel_features, grad_weights, grad_bn_weight, grad_bn_bias, workspace,
+                      workspace_bytes, stream);
+}
+
+int bevb200_encoder_backward_f16(const bevb200_encoder_t *e, const float *const *weights, const void *state,
+                                 size_t state_bytes, int max_voxels, int batch_size, const int32_t *user_caps,
+                                 const void *grad_dense, long long out_batch_stride, void *grad_voxel_features,
+                                 float *const *grad_weights, float *const *grad_bn_weight,
+                                 float *const *grad_bn_bias, void *workspace, size_t workspace_bytes, void *stream) {
+  return enc_backward(e, true, weights, state, state_bytes, max_voxels, batch_size, user_caps, grad_dense,
+                      out_batch_stride, grad_voxel_features, grad_weights, grad_bn_weight, grad_bn_bias, workspace,
+                      workspace_bytes, stream);
 }
 
 }  // extern "C"

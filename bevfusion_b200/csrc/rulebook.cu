@@ -232,10 +232,11 @@ __global__ void __launch_bounds__(256)
 }
 
 // dense() + permute(0,1,4,2,3) + view(N, C*D, H, W) (structure.py:49-59, sparse_encoder.py:126-130)
+template <typename T>
 __global__ void __launch_bounds__(256)
-    sparse_to_dense_kernel(const float *__restrict__ features, const int32_t *__restrict__ idx, int cap,
+    sparse_to_dense_kernel(const T *__restrict__ features, const int32_t *__restrict__ idx, int cap,
                            const int32_t *__restrict__ n_dev, int c, int batch, int X, int Y, int Z, int z_major,
-                           long long out_batch_stride, float *__restrict__ out) {
+                           long long out_batch_stride, T *__restrict__ out) {
   // grid (row tiles, channel groups): a thread handles one site and the channels ch0, ch0+gridDim.y, ..
   // (site fastest across the warp: neighbouring sites -> nearby stores; no per-element division)
   const int n = row_count(n_dev, cap);
@@ -246,7 +247,7 @@ __global__ void __launch_bounds__(256)
       continue;
     const long long site = z_major ? ((long long)p.w * X + p.y) * Y + p.z : ((long long)p.y * Y + p.z) * Z + p.w;
     const long long plane = (long long)X * Y * Z;
-    float *o = out + p.x * out_batch_stride + site;
+    T *o = out + p.x * out_batch_stride + site;
     for (int ch = blockIdx.y; ch < c; ch += gridDim.y) o[ch * plane] = features[(long long)i * c + ch];
   }
 }
@@ -349,23 +350,32 @@ int rb_gather(const int32_t *qidx, int qcap, const int32_t *nq_dev, const ConvGe
   return BEVB200_OK;
 }
 
-int sparse_to_dense(const float *features, const int32_t *idx, int cap, const int32_t *n_dev, int c, int batch,
-                    const int shape[3], int z_major, long long out_batch_stride, float *out, cudaStream_t st) {
+template <typename T>
+static int sparse_to_dense_t(const T *features, const int32_t *idx, int cap, const int32_t *n_dev, int c, int batch,
+                             const int shape[3], int z_major, long long out_batch_stride, T *out, cudaStream_t st) {
   const int X = shape[0], Y = shape[1], Z = shape[2];
   const long long per_batch = (long long)c * X * Y * Z;
   if (out_batch_stride == 0) out_batch_stride = per_batch;
   BEVB200_REQUIRE(out_batch_stride >= per_batch, "output batch stride too small");
   if (out_batch_stride == per_batch) {
-    BEVB200_CUDA(cudaMemsetAsync(out, 0, (size_t)batch * per_batch * sizeof(float), st));
+    BEVB200_CUDA(cudaMemsetAsync(out, 0, (size_t)batch * per_batch * sizeof(T), st));
   } else {  // channel slice of a wider [B, C_total, ...] buffer (the fuser's concatenated input)
-    BEVB200_CUDA(cudaMemset2DAsync(out, (size_t)out_batch_stride * sizeof(float), 0, (size_t)per_batch * sizeof(float),
+    BEVB200_CUDA(cudaMemset2DAsync(out, (size_t)out_batch_stride * sizeof(T), 0, (size_t)per_batch * sizeof(T),
                                    batch, st));
   }
   if (cap == 0) return BEVB200_OK;
   BEVB200_REQUIRE(features && idx, "null argument");
-  BEVB200_LAUNCH(sparse_to_dense_kernel, dim3(grid_for(cap, 256, kNumSMs), c < 32 ? c : 32), 256, 0, st, features, idx,
-                 cap, n_dev, c, batch, X, Y, Z, z_major, out_batch_stride, out);
+  BEVB200_LAUNCH(sparse_to_dense_kernel<T>, dim3(grid_for(cap, 256, kNumSMs), c < 32 ? c : 32), 256, 0, st, features,
+                 idx, cap, n_dev, c, batch, X, Y, Z, z_major, out_batch_stride, out);
   return BEVB200_OK;
+}
+int sparse_to_dense(const float *features, const int32_t *idx, int cap, const int32_t *n_dev, int c, int batch,
+                    const int shape[3], int z_major, long long out_batch_stride, float *out, cudaStream_t st) {
+  return sparse_to_dense_t(features, idx, cap, n_dev, c, batch, shape, z_major, out_batch_stride, out, st);
+}
+int sparse_to_dense(const __half *features, const int32_t *idx, int cap, const int32_t *n_dev, int c, int batch,
+                    const int shape[3], int z_major, long long out_batch_stride, __half *out, cudaStream_t st) {
+  return sparse_to_dense_t(features, idx, cap, n_dev, c, batch, shape, z_major, out_batch_stride, out, st);
 }
 
 // ---- per-conv rulebook: workspace = the bitmap of the output grid + rank2row -------------

@@ -4,6 +4,8 @@
 // Kernels that walk rows take a host-side cap and a nullable device-side count n_dev: they use
 // min(max(*n_dev, 0), cap) rows, or cap rows when n_dev is null.
 #pragma once
+#include <cuda_fp16.h>
+
 #include "common.cuh"
 
 namespace bevb200 {
@@ -61,5 +63,7 @@ int rb_gather(const int32_t *qidx, int qcap, const int32_t *nq_dev, const ConvGe
 // dense(): zero `out`, then scatter the rows (layout: bevb200_sparse_to_dense in the public header)
 int sparse_to_dense(const float *features, const int32_t *idx, int cap, const int32_t *n_dev, int c, int batch,
                     const int shape[3], int z_major, long long out_batch_stride, float *out, cudaStream_t st);
+int sparse_to_dense(const __half *features, const int32_t *idx, int cap, const int32_t *n_dev, int c, int batch,
+                    const int shape[3], int z_major, long long out_batch_stride, __half *out, cudaStream_t st);
 
 }  // namespace bevb200

@@ -6,6 +6,8 @@
 //   spconv_bwd.cu       backward C ABI, SIMT filter-gradient kernels, the ordered partial reduction
 //   spconv_wgrad_tc.cu  tensor-core filter gradient
 #pragma once
+#include <cuda_fp16.h>
+
 #include "common.cuh"
 
 namespace bevb200 {
@@ -49,6 +51,18 @@ int spconv_v6_forward(const void *features_split, const void *packed, const int3
                       int n_in, int n_out, const int32_t *n_out_dev, int c_in, int c_out, int kvol, const float *scale,
                       const float *shift, const float *residual, const void *residual_split, int relu, float *out,
                       void *out_split, cudaStream_t st);
+// FP16 (BEVB200_PREC_FP16): the weight image (K blocks of 64 fp16 channels), the fp16 row image [n, c_eff] of fp16
+// rows (zero padded; n as in split_rows) and the forward on it.  residual (fp32 rows) or
+// residual_f16 (an fp16 image [n_out, c_out]) is added before the ReLU; out and / or out_f16 receive the result, the
+// image rounded once to fp16.
+size_t spconv_v6_packed_bytes_f16(int c_in, int c_out, int kvol);
+int spconv_v6_pack_weights_f16(const float *weight, int c_in, int c_out, int kvol, void *packed, cudaStream_t st);
+int spconv_v6_f16_rows(const __half *rows, int n_cap, const int32_t *n_dev, int c_in, int c_eff, void *image,
+                       cudaStream_t st);
+int spconv_v6_forward_f16(const void *rows, const void *packed, const int32_t *nbr, long long nbr_stride, int n_in,
+                          int n_out, const int32_t *n_out_dev, int c_in, int c_out, int kvol, const float *scale,
+                          const float *shift, const float *residual, const void *residual_f16, int relu, float *out,
+                          void *out_f16, cudaStream_t st);
 // TF32 (tf32x3 = false) / 3xTF32 forward on fp32 rows [n_in][c_in], c_in a power of two 8 .. 128
 int spconv_v6_forward_tf32(const float *rows, const void *packed, const int32_t *nbr, int n_in, int n_out, int c_in,
                            int c_out, int kvol, bool tf32x3, const float *scale, const float *shift,
@@ -71,6 +85,13 @@ size_t spconv_wgrad_tc_split_workspace_bytes(int n_out, int c_in, int c_out, int
 int spconv_wgrad_tc_split(const void *features_split, const float *out_grad, const int32_t *nbr, int n_in, int n_out,
                           const int32_t *n_out_dev, int c_in, int c_out, int kvol, float *weight_grad,
                           void *workspace, cudaStream_t st);
+
+// FP16 form of the same filter gradient: features an fp16 image [n_in][f_channels] (c_in <= f_channels, a multiple of 8,
+// <= 128), out_grad an fp16 image [n_out][c_out]; the workspace holds the partials only.
+size_t spconv_wgrad_tc_f16_workspace_bytes(int n_out, int c_in, int c_out, int kvol);
+int spconv_wgrad_tc_f16(const void *features, int f_channels, const void *out_grad, const int32_t *nbr, int n_in,
+                        int n_out, const int32_t *n_out_dev, int c_in, int c_out, int kvol, float *weight_grad,
+                        void *workspace, cudaStream_t st);
 
 // ---- spconv_bwd.cu ---------------------------------------------------------------------------
 // weight_grad[e] = sum over the chunks, in ascending order, of partial[chunk][e]: bit-reproducible

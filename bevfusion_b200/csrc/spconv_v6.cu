@@ -1,5 +1,5 @@
-// Sparse convolution forward on the Hopper tensor cores, BF16x3 and TF32 precisions: a warp-specialised wgmma
-// kernel (spconv_wg_kernel, BF16x3 at Cout >= 64, described above it) and the mma.sync kernel below.
+// Sparse convolution forward on the Hopper tensor cores, BF16x3, FP16 and TF32 precisions: a warp-specialised wgmma
+// kernel (spconv_wg_kernel, BF16x3 / FP16 at Cout >= 64, described above it) and the mma.sync kernel below.
 //
 //   out[o, :] = epilogue( sum_k features[nbr[k, o], :] @ W[k] )          (spconv_ops.h:260-361)
 //
@@ -11,6 +11,10 @@
 //     needs them; a residual is read from a split image too), so the split is done once per row instead of once
 //     per (row, kernel offset) visit.  Per 16-channel step: lo*W_hi + hi*W_lo + hi*W_hi, fp32 accumulate.
 //   * TF32 (mode 1) and 3xTF32 (mode 2): zero-padded fp32 rows, split into tf32 hi / lo in registers.
+//   * FP16 (mode 3, the encoder plan's BEVB200_PREC_FP16): a row is c_eff fp16 channels, 2 B each.  The kernels see it
+//     as c_eff / 2 four-byte units, so a K block is 64 channels, the gather and the swizzle are those of the other
+//     modes, and a 16-channel step is one fp16 MMA (the products are exact in the fp32 accumulator).  The epilogue
+//     rounds once to fp16 (round to nearest, overflow to inf) and writes the fp16 image; a residual is read from one.
 // A CTA (8 warps, two CTAs per SM) owns 128-row output tiles, persistent over the tiles; per K block all 256
 // threads gather the 128 neighbour rows with 16-byte cp.async (zero fill for missing neighbours) into an XOR-
 // swizzled tile (16-byte chunk c of row r at (c ^ (r & 7)): conflict-free ldmatrix) and copy the weight block
@@ -47,7 +51,8 @@ struct V6Params {
 
 // Epilogue of NC (8 or 16) consecutive channels [c0, c0 + NC) of one row: folded BN, residual, ReLU,
 // then the fp32 row and / or its split image.  NC channels = NC/8 16-byte chunks of hi and of lo.
-template <int NC>
+// F16: residual_split and out_split are fp16 images [n, c_out] instead of split images.
+template <int NC, bool F16>
 __device__ __forceinline__ void v6_store_chunk(const V6Params &p, float (&acc)[NC], int orow, int c0) {
   const int c_out = p.c_out;
   float y[NC];
@@ -64,6 +69,20 @@ __device__ __forceinline__ void v6_store_chunk(const V6Params &p, float (&acc)[N
     for (int j = 0; j < NC / 4; ++j) {
       const float4 rv = __ldg(res + j);
       y[4 * j] += rv.x; y[4 * j + 1] += rv.y; y[4 * j + 2] += rv.z; y[4 * j + 3] += rv.w;
+    }
+  } else if (F16 && p.residual_split) {
+    // plain loads (the image may be this launch's own out_split, rewritten below by the same lane)
+    const uint4 *row = reinterpret_cast<const uint4 *>(p.residual_split + ((long long)orow * c_out + c0) * 2);
+#pragma unroll
+    for (int j = 0; j < NC / 8; ++j) {
+      const uint4 h = row[j];
+      const uint32_t hw[4] = {h.x, h.y, h.z, h.w};
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float2 f = __half22float2(*reinterpret_cast<const __half2 *>(&hw[e]));
+        y[8 * j + 2 * e] += f.x;
+        y[8 * j + 2 * e + 1] += f.y;
+      }
     }
   } else if (p.residual_split) {
     // plain loads (the image may be this launch's own out_split, rewritten below by the same lane)
@@ -89,7 +108,17 @@ __device__ __forceinline__ void v6_store_chunk(const V6Params &p, float (&acc)[N
 #pragma unroll
     for (int j = 0; j < NC / 4; ++j) dst[j] = make_float4(y[4 * j], y[4 * j + 1], y[4 * j + 2], y[4 * j + 3]);
   }
-  if (p.out_split) {
+  if (F16 && p.out_split) {
+    uint32_t h[NC / 2];
+#pragma unroll
+    for (int e = 0; e < NC; e += 2) {
+      const __half2 v = __floats2half2_rn(y[e], y[e + 1]);
+      h[e / 2] = *reinterpret_cast<const uint32_t *>(&v);
+    }
+    uint4 *row = reinterpret_cast<uint4 *>(p.out_split + ((long long)orow * c_out + c0) * 2);
+#pragma unroll
+    for (int j = 0; j < NC / 8; ++j) row[j] = make_uint4(h[4 * j], h[4 * j + 1], h[4 * j + 2], h[4 * j + 3]);
+  } else if (p.out_split) {
     uint32_t hi[NC / 2], lo[NC / 2];
 #pragma unroll
     for (int e = 0; e < NC; e += 2) split_pair(y[e], y[e + 1], hi[e / 2], lo[e / 2]);
@@ -235,6 +264,36 @@ __global__ void __launch_bounds__(kV6Threads, 2) spconv_v6_kernel(const V6Params
             }
           }
         }
+      } else if constexpr (MODE == 3) {
+        // four k16 steps of 16 fp16 channels: chunks 2 ks, 2 ks + 1 (not unrolled at Cout 128: it would spill)
+#pragma unroll(COUT == 128 ? 1 : 4)
+        for (int ks = 0; ks < 4; ++ks) {
+          uint32_t af[2][4];
+#pragma unroll
+          for (int mt = 0; mt < 2; ++mt) {
+            const int r = wm + 16 * mt + (lane & 15), lc = 2 * ks + (lane >> 4);
+            ldsm_x4(a + (uint32_t)(r * 128 + ((lc ^ (r & 7)) << 4)), af[mt]);
+          }
+          const int lc = 2 * ks + ((lane >> 3) & 1);
+          if constexpr (NT == 1) {
+            const int n = wn + (lane & 7);
+            uint32_t bf[2];
+            ldsm_x2(b + (uint32_t)(n * 128 + ((lc ^ (n & 7)) << 4)), bf);
+#pragma unroll
+            for (int mt = 0; mt < 2; ++mt) mma_f16_16816(acc[mt][0], af[mt], bf[0], bf[1]);
+          } else {
+#pragma unroll
+            for (int nt = 0; nt < NT; nt += 2) {
+              const int n = wn + nt * 8 + (lane & 7) + ((lane >> 4) << 3);
+              uint32_t bf[4];
+              ldsm_x4(b + (uint32_t)(n * 128 + ((lc ^ (n & 7)) << 4)), bf);
+#pragma unroll
+              for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) mma_f16_16816(acc[mt][nt + h], af[mt], bf[2 * h], bf[2 * h + 1]);
+            }
+          }
+        }
       } else {
 #pragma unroll
         for (int ks = 0; ks < 4; ++ks) {     // four k8 steps of 8 fp32 channels
@@ -309,7 +368,7 @@ __global__ void __launch_bounds__(kV6Threads, 2) spconv_v6_kernel(const V6Params
           const float4 q = *reinterpret_cast<const float4 *>(cs + r * LD + 16 * j + e);
           v[e] = q.x; v[e + 1] = q.y; v[e + 2] = q.z; v[e + 3] = q.w;
         }
-        v6_store_chunk<16>(p, v, orow, 16 * j);
+        v6_store_chunk<16, MODE == 3>(p, v, orow, 16 * j);
       }
     }
     __syncthreads();                         // the transpose area is the next tile's ring
@@ -326,7 +385,8 @@ __global__ void __launch_bounds__(kV6Threads, 2) spconv_v6_kernel(const V6Params
 //   * B: the K block's packed weight rows (Cout x 128 B, same swizzle), one bulk copy.
 // The producer gathers the rows with 16-byte cp.async (zero fill for missing neighbours), each thread arriving on
 // the stage's "full" barrier when its copies land (cp.async.mbarrier.arrive.noinc); one thread adds the weight
-// copy's bytes to the same barrier.  Consumers wait on "full", issue the 3 x 2 x kMT wgmmas of the block, keep one
+// copy's bytes to the same barrier.  Consumers wait on "full", issue the 3 x 2 x kMT wgmmas of the block (FP16, mode 3:
+// 4 x kMT, one per 16 channels of the 64-channel block), keep one
 // block in flight (wait_group 1) and then release the previous stage on its "empty" barrier.  The tile's epilogue
 // goes through a small per-warp transpose buffer, so the producer keeps filling the ring meanwhile.
 constexpr int kWgThreads = 384;
@@ -350,13 +410,14 @@ struct WgShape {
   static_assert(kStage % 1024 == 0 && kStages >= 2, "ring does not fit");
 };
 
-template <int COUT>
-__device__ __forceinline__ void wgmma_bf16(float (&d)[COUT / 2], uint64_t da, uint64_t db, int accumulate) {
-  if constexpr (COUT == 64) wgmma_bf16_n64(d, da, db, accumulate);
-  else wgmma_bf16_n128(d, da, db, accumulate);
+template <bool F16, int COUT>
+__device__ __forceinline__ void wgmma_nc(float (&d)[COUT / 2], uint64_t da, uint64_t db, int accumulate) {
+  if constexpr (COUT == 64) wgmma_n64<F16>(d, da, db, accumulate);
+  else wgmma_n128<F16>(d, da, db, accumulate);
 }
 
-template <int COUT>
+// MODE 0 (BF16x3) or 3 (FP16)
+template <int MODE, int COUT>
 __global__ void __launch_bounds__(kWgThreads, 1) spconv_wg_kernel(const V6Params p) {
   using Sh = WgShape<COUT>;
   constexpr int S = Sh::kStages, MT = Sh::kMT, TM = Sh::kTileM;
@@ -441,15 +502,25 @@ __global__ void __launch_bounds__(kWgThreads, 1) spconv_wg_kernel(const V6Params
         fence_proxy_async_smem();
         wgmma_fence();
         const uint32_t a = smem + s * Sh::kStage + cw * (MT * 64 * 128), b = smem + s * Sh::kStage + Sh::kA;
+        if constexpr (MODE == 3) {
 #pragma unroll
-        for (int g = 0; g < 2; ++g) {       // the two 16-channel groups of the K block: A [hi | lo], W [hi, hi | lo, lo]
-          const uint64_t bh = wgmma_desc_sw128(b + 32 * g), bl = wgmma_desc_sw128(b + 64 + 32 * g);
+          for (int ks = 0; ks < 4; ++ks) {  // the four k16 slices of the 64-channel K block, A and W alike
+            const uint64_t bd = wgmma_desc_sw128(b + 32 * ks);
 #pragma unroll
-          for (int m = 0; m < MT; ++m) {
-            const uint64_t ah = wgmma_desc_sw128(a + m * (64 * 128) + 64 * g), al = wgmma_desc_sw128(a + m * (64 * 128) + 64 * g + 32);
-            wgmma_bf16<COUT>(acc[m], al, bh, kb > 0 || g > 0);
-            wgmma_bf16<COUT>(acc[m], ah, bl, 1);
-            wgmma_bf16<COUT>(acc[m], ah, bh, 1);
+            for (int m = 0; m < MT; ++m)
+              wgmma_nc<true, COUT>(acc[m], wgmma_desc_sw128(a + m * (64 * 128) + 32 * ks), bd, kb > 0 || ks > 0);
+          }
+        } else {
+#pragma unroll
+          for (int g = 0; g < 2; ++g) {     // the two 16-channel groups of the K block: A [hi | lo], W [hi, hi | lo, lo]
+            const uint64_t bh = wgmma_desc_sw128(b + 32 * g), bl = wgmma_desc_sw128(b + 64 + 32 * g);
+#pragma unroll
+            for (int m = 0; m < MT; ++m) {
+              const uint64_t ah = wgmma_desc_sw128(a + m * (64 * 128) + 64 * g), al = wgmma_desc_sw128(a + m * (64 * 128) + 64 * g + 32);
+              wgmma_nc<false, COUT>(acc[m], al, bh, kb > 0 || g > 0);
+              wgmma_nc<false, COUT>(acc[m], ah, bl, 1);
+              wgmma_nc<false, COUT>(acc[m], ah, bh, 1);
+            }
           }
         }
         wgmma_commit();
@@ -485,7 +556,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) spconv_wg_kernel(const V6Params
               const float4 q = *reinterpret_cast<const float4 *>(buf + r * LD + 16 * j + e);
               v[e] = q.x; v[e + 1] = q.y; v[e + 2] = q.z; v[e + 3] = q.w;
             }
-            v6_store_chunk<16>(p, v, rbase + r, c0 + 16 * j);
+            v6_store_chunk<16, MODE == 3>(p, v, rbase + r, c0 + 16 * j);
           }
           __syncwarp();
         }
@@ -546,6 +617,46 @@ __global__ void spconv_v6_pack_rows_kernel(const float *__restrict__ w, int kvol
   }
 }
 
+// fp16 rows [n, c_in] -> fp16 image [n, c_eff] (zero padded, exact); one thread per (row, 8 channels)
+__global__ void spconv_v6_f16_rows_kernel(const __half *__restrict__ in, int n_cap, const int32_t *__restrict__ n_dev,
+                                          int c_in, int c_eff, uint8_t *__restrict__ out) {
+  int n = n_cap;
+  if (n_dev) n = min(n, max(__ldg(n_dev), 0));
+  const int per_row = c_eff >> 3;
+  const long long total = (long long)n * per_row;
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total;
+       t += (long long)gridDim.x * blockDim.x) {
+    const int j = (int)(t % per_row);
+    const long long r = t / per_row;
+    uint32_t h[4];
+#pragma unroll
+    for (int e = 0; e < 8; e += 2) {
+      const int c = 8 * j + e;
+      const __half2 v = __halves2half2(c < c_in ? in[r * c_in + c] : __ushort_as_half(0),
+                                       c + 1 < c_in ? in[r * c_in + c + 1] : __ushort_as_half(0));
+      h[e / 2] = *reinterpret_cast<const uint32_t *>(&v);
+    }
+    *reinterpret_cast<uint4 *>(out + (r * c_eff + 8 * j) * 2) = make_uint4(h[0], h[1], h[2], h[3]);
+  }
+}
+
+// Weight image of the fp16 form: one stage (Cout rows of 128 B) per 64-wide K block, row n = fp16(W) of kk 0-63,
+// SWIZZLE_128B (16-byte chunk kk / 8 at (kk / 8) ^ (n & 7)).
+__global__ void spconv_v6_pack_f16_kernel(const float *__restrict__ w, int kvol, int c_in, int c_in_eff, int c_out,
+                                          int nkb, __half *__restrict__ packed) {
+  const long long total = (long long)nkb * c_out * 64;
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total;
+       t += (long long)gridDim.x * blockDim.x) {
+    const int cc = (int)(t % 64);
+    const int n = (int)((t / 64) % c_out);
+    const int kb = (int)(t / (64ll * c_out));
+    const int kk = kb * 64 + cc;
+    const int k = kk / c_in_eff, ci = kk % c_in_eff;
+    const float v = (k < kvol && ci < c_in) ? w[((long long)k * c_in + ci) * c_out + n] : 0.f;
+    packed[((long long)kb * c_out + n) * 64 + ((((cc >> 3) ^ (n & 7)) << 3) | (cc & 7))] = __float2half_rn(v);
+  }
+}
+
 int spconv_v6_cin_eff(int c_in) {
   for (int e = 16; e <= 128; e <<= 1)
     if (c_in <= e) return e;
@@ -560,6 +671,30 @@ static int v6_nkb(int c_eff, int kvol) { return (kvol * c_eff + 31) / 32; }
 size_t spconv_v6_packed_bytes(int c_in, int c_out, int kvol) {
   if (!spconv_v6_shape_ok(c_in, c_out, kvol)) return 0;
   return (size_t)v6_nkb(spconv_v6_cin_eff(c_in), kvol) * c_out * 128;
+}
+// K blocks of 64 fp16 channels = 32 four-byte units
+static int v6_nkb_f16(int c_eff, int kvol) { return v6_nkb(c_eff / 2, kvol); }
+
+size_t spconv_v6_packed_bytes_f16(int c_in, int c_out, int kvol) {
+  if (!spconv_v6_shape_ok(c_in, c_out, kvol)) return 0;
+  return (size_t)v6_nkb_f16(spconv_v6_cin_eff(c_in), kvol) * c_out * 128;
+}
+
+int spconv_v6_pack_weights_f16(const float *weight, int c_in, int c_out, int kvol, void *packed, cudaStream_t st) {
+  const int ce = spconv_v6_cin_eff(c_in);
+  const int nkb = v6_nkb_f16(ce, kvol);
+  BEVB200_LAUNCH(spconv_v6_pack_f16_kernel, grid_for((long long)nkb * c_out * 64, 256), 256, 0, st, weight, kvol,
+                 c_in, ce, c_out, nkb, (__half *)packed);
+  return BEVB200_OK;
+}
+
+int spconv_v6_f16_rows(const __half *rows, int n_cap, const int32_t *n_dev, int c_in, int c_eff, void *image,
+                       cudaStream_t st) {
+  BEVB200_REQUIRE(c_eff >= c_in && c_eff % 16 == 0 && c_in >= 1, "bad padded channel count");
+  if (n_cap <= 0) return BEVB200_OK;
+  BEVB200_LAUNCH(spconv_v6_f16_rows_kernel, grid_for((long long)n_cap * (c_eff / 8), 256), 256, 0, st, rows, n_cap,
+                 n_dev, c_in, c_eff, (uint8_t *)image);
+  return BEVB200_OK;
 }
 
 int spconv_v6_pack_weights(const float *weight, int c_in, int c_out, int kvol, void *packed, cudaStream_t st) {
@@ -619,17 +754,19 @@ static int v6_launch(const V6Params &p, cudaStream_t st) {
   BEVB200_REQUIRE(false, "output channel count has no tensor-core form");
 }
 
-template <int COUT>
+template <int MODE, int COUT>
 static int wg_launch_one(const V6Params &p, cudaStream_t st) {
   using Sh = WgShape<COUT>;
   const int n_tiles = (p.n_out + Sh::kTileM - 1) / Sh::kTileM;
-  return v6_launch_kernel(spconv_wg_kernel<COUT>, n_tiles < kNumSMs ? n_tiles : kNumSMs, kWgThreads, Sh::kSmem, p, st);
+  return v6_launch_kernel(spconv_wg_kernel<MODE, COUT>, n_tiles < kNumSMs ? n_tiles : kNumSMs, kWgThreads, Sh::kSmem,
+                          p, st);
 }
 
+template <int MODE>
 static int wg_launch(const V6Params &p, cudaStream_t st) {
   switch (p.c_out) {
-    case 64: return wg_launch_one<64>(p, st);
-    case 128: return wg_launch_one<128>(p, st);
+    case 64: return wg_launch_one<MODE, 64>(p, st);
+    case 128: return wg_launch_one<MODE, 128>(p, st);
   }
   BEVB200_REQUIRE(false, "output channel count has no tensor-core form");
 }
@@ -672,7 +809,30 @@ int spconv_v6_forward(const void *features_split, const void *packed, const int3
   // The warpgroup-MMA kernel wins where the tensor work per gathered row is large (Cout >= 64) and a tile has K
   // blocks enough to amortise its pipeline fill and epilogue.  At Cout <= 32 the row gather bounds both kernels
   // and two mma.sync CTAs per SM keep more of it in flight; the k(1,1,3) conv_out (12 K blocks) is faster there too.
-  return p.c_out >= 64 && p.nkb >= kWgMinKBlocks ? wg_launch(p, st) : v6_launch<0>(p, st);
+  return p.c_out >= 64 && p.nkb >= kWgMinKBlocks ? wg_launch<0>(p, st) : v6_launch<0>(p, st);
+}
+
+int spconv_v6_forward_f16(const void *rows, const void *packed, const int32_t *nbr, long long nbr_stride, int n_in,
+                          int n_out, const int32_t *n_out_dev, int c_in, int c_out, int kvol, const float *scale,
+                          const float *shift, const float *residual, const void *residual_f16, int relu, float *out,
+                          void *out_f16, cudaStream_t st) {
+  BEVB200_REQUIRE(!(residual && residual_f16), "residual given twice");
+  BEVB200_REQUIRE(c_in == spconv_v6_cin_eff(c_in) && spconv_v6_shape_ok(c_in, c_out, kvol), "shape has no tensor-core form");
+  BEVB200_REQUIRE(rows && packed && nbr, "null argument");
+  BEVB200_REQUIRE((uintptr_t)rows % 16 == 0 && (out == nullptr || (uintptr_t)out % 16 == 0) &&
+                      (out_f16 == nullptr || (uintptr_t)out_f16 % 16 == 0) &&
+                      (residual == nullptr || (uintptr_t)residual % 16 == 0) &&
+                      (residual_f16 == nullptr || (uintptr_t)residual_f16 % 16 == 0) && (uintptr_t)packed % 16 == 0,
+                  "operands must be 16-byte aligned");
+  if (n_out <= 0) return BEVB200_OK;
+  V6Params p;
+  // the kernels address a row in four-byte units: c_in fp16 channels are c_in / 2 of them
+  v6_common(p, rows, packed, nbr, nbr_stride, n_in, n_out, n_out_dev, c_in / 2, c_out, kvol, scale, shift, residual,
+            relu, out);
+  p.residual_split = (const uint8_t *)residual_f16;
+  p.out_split = (uint8_t *)out_f16;
+  // the same layers as BF16x3 take the wgmma kernel: >= kWgMinKBlocks K blocks of 32 channels (half as many fp16 blocks)
+  return p.c_out >= 64 && v6_nkb(c_in, kvol) >= kWgMinKBlocks ? wg_launch<3>(p, st) : v6_launch<3>(p, st);
 }
 
 // TF32 (tf32x3 = false) / 3xTF32 forward on zero-padded fp32 rows [n_in][c_in] (c_in a power of two, 8 .. 128) and

@@ -15,6 +15,9 @@
 //     rows with 16-byte cp.async into XOR-swizzled tiles (chunk c of row r at c ^ (r & 7): conflict-free ldmatrix),
 //     in a ring of cp.async stages;
 //   * multiplies hi.hi + hi.lo + lo.hi per 16-row k step (the lo.lo term is below the fp32 rounding of the sum).
+// The FP16 form (the encoder plan's BEVB200_PREC_FP16 backward) runs the same kernel on fp16 images (a row: the
+// channels as fp16, 2 B each) with one MMA per k step.  Its tiles keep 128-byte lines, so rows of 64 or 128 channels;
+// narrower rows in memory (the 16 / 32-channel images of the forward) are zero filled in shared memory.
 #include <stdlib.h>
 
 #include "spconv.cuh"
@@ -27,8 +30,9 @@ constexpr int kWgtRows = 32;           // reduction rows per stage
 constexpr int kWgtStages = 3;
 
 struct WgtParams {
-  const uint8_t *fsplit;       // [n_in][ci_eff * 4 B]
-  const uint8_t *gsplit;       // [n_out][co_eff * 4 B]
+  const uint8_t *fsplit;       // [n_in][ci_eff * 4 B]; FP16: [n_in][f_row_bytes]
+  const uint8_t *gsplit;       // [n_out][co_eff * 4 B]; FP16: [n_out][g_row_bytes]
+  int f_row_bytes, g_row_bytes;   // FP16: bytes per row in memory (<= the tile's row; the rest reads as zeros)
   const int32_t *nbr;          // [kvol][n_out]
   const int32_t *n_out_dev;    // nullable device row count (<= n_out): rows past it count as missing
   float *partial;              // [n_chunks][kvol][c_in][c_out]
@@ -36,9 +40,10 @@ struct WgtParams {
   int n_chunks, tiles_per_chunk, n_tiles;   // tiles of kWgtRows rows
 };
 
-template <int CI, int CO>
+template <bool F16, int CI, int CO>
 struct WgtShape {
-  static constexpr int kFRow = CI * 4, kGRow = CO * 4;           // bytes per operand row
+  static constexpr int kFRow = CI * (F16 ? 2 : 4), kGRow = CO * (F16 ? 2 : 4);   // bytes per operand row
+  static_assert(kFRow % 128 == 0 && kGRow % 128 == 0, "tile rows are whole 128-byte lines");
   static constexpr int kStage = kWgtRows * (kFRow + kGRow);
   static constexpr int kSmem = kWgtStages * kStage;
 };
@@ -48,9 +53,9 @@ __device__ __forceinline__ uint32_t wgt_off(int r, int c, int row_bytes) {
   return (uint32_t)(r * row_bytes + ((c ^ (r & 7)) << 4));
 }
 
-template <int CI, int CO>
+template <bool F16, int CI, int CO>
 __global__ void __launch_bounds__(kWgtThreads, 1) spconv_wgrad_tc_kernel(const WgtParams p) {
-  using Sh = WgtShape<CI, CO>;
+  using Sh = WgtShape<F16, CI, CO>;
   constexpr int FR = Sh::kFRow, GR = Sh::kGRow;
   constexpr int MT = CI / 32;          // m16 tiles per warp (two warps along Cin)
   constexpr int NT = CO / 32;          // n8 tiles per warp (four warps along Cout)
@@ -81,13 +86,15 @@ __global__ void __launch_bounds__(kWgtThreads, 1) spconv_wgrad_tc_kernel(const W
       for (int u = tid; u < kWgtRows * FCH; u += kWgtThreads) {
         const int r = u / FCH, c = u - r * FCH;
         int src = o0 + r < n_valid ? __ldg(nbr_k + o0 + r) : -1;
-        if (src >= p.n_in) src = -1;
-        cp_async16_row(f + wgt_off(r, c, FR), fbase + (unsigned long long)(uint32_t)max(src, 0) * FR + c * 16, src);
+        if (src >= p.n_in || (F16 && c * 16 >= p.f_row_bytes)) src = -1;
+        cp_async16_row(f + wgt_off(r, c, FR),
+                       fbase + (unsigned long long)(uint32_t)max(src, 0) * (F16 ? p.f_row_bytes : FR) + c * 16, src);
       }
       for (int u = tid; u < kWgtRows * GCH; u += kWgtThreads) {
         const int r = u / GCH, c = u - r * GCH;
-        const int o = o0 + r < n_valid ? o0 + r : -1;
-        cp_async16_row(g + wgt_off(r, c, GR), gbase + (unsigned long long)(uint32_t)max(o, 0) * GR + c * 16, o);
+        const int o = o0 + r < n_valid && !(F16 && c * 16 >= p.g_row_bytes) ? o0 + r : -1;
+        cp_async16_row(g + wgt_off(r, c, GR),
+                       gbase + (unsigned long long)(uint32_t)max(o, 0) * (F16 ? p.g_row_bytes : GR) + c * 16, o);
       }
     };
     float acc[MT][NT][4];
@@ -109,7 +116,28 @@ __global__ void __launch_bounds__(kWgtThreads, 1) spconv_wgrad_tc_kernel(const W
       cp_async_commit();
       const uint32_t f = smem + (uint32_t)(i % kWgtStages) * Sh::kStage, g = f + kWgtRows * FR;
 #pragma unroll
-      for (int ks = 0; ks < kWgtRows / 16; ++ks) {
+      for (int ks = 0; ks < kWgtRows / 16 && F16; ++ks) {
+        // FP16: channel c of a row sits in chunk c / 8; matrices and lanes as in the BF16x3 loop below
+        uint32_t af[MT][4];
+#pragma unroll
+        for (int mt = 0; mt < MT; ++mt) {
+          const int m0 = wm + 16 * mt, q = lane >> 3;
+          ldsm_x4_t(f + wgt_off(ks * 16 + 8 * (q >> 1) + (lane & 7), (m0 >> 3) + (q & 1), FR), af[mt]);
+        }
+#pragma unroll
+        for (int nt = 0; nt < NT; nt += 2) {
+          static_assert(!F16 || NT >= 2, "fp16 tiles have >= 64 output channels");
+          const int q = lane >> 3;
+          uint32_t bf[4];
+          ldsm_x4_t(g + wgt_off(ks * 16 + 8 * (q & 1) + (lane & 7), (wn + 8 * nt + 8 * (q >> 1)) >> 3, GR), bf);
+#pragma unroll
+          for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) mma_f16_16816(acc[mt][nt + h], af[mt], bf[2 * h], bf[2 * h + 1]);
+        }
+      }
+#pragma unroll
+      for (int ks = 0; ks < kWgtRows / 16 && !F16; ++ks) {
         // A = F^T: m = input channel, k = row.  Matrix q of ldmatrix.x4.trans: rows k0 + 8 (q >> 1) .., channels
         // m0 + 8 (q & 1) ..; the channel group m0 / 16 keeps hi at chunk 4 (m0 / 16) + 0 / 1, lo at + 2 / 3.
         uint32_t ahi[MT][4], alo[MT][4];
@@ -179,8 +207,10 @@ bool spconv_wgrad_tc_ok(int c_in, int c_out, int kvol) {
          kvol >= 1 && kvol <= 27;
 }
 
-// channel count of an operand image: 128-byte slabs of 32 channels, 1 / 2 / 4 of them (zero padded)
+// channel count of an operand image: 128-byte slabs of 32 channels, 1 / 2 / 4 of them (zero padded); FP16 tiles:
+// slabs of 64 channels, 1 / 2 of them
 static int wgt_eff(int c) { return c <= 32 ? 32 : (c <= 64 ? 64 : 128); }
+static int wgt_eff_f16(int c) { return c <= 64 ? 64 : 128; }
 
 // The shape of a launch: row tiles and row chunks (~3 work items per SM, every chunk non-empty).
 struct WgtPlan {
@@ -213,13 +243,14 @@ size_t spconv_wgrad_tc_workspace_bytes(int n_in, int n_out, int c_in, int c_out,
          align_up((size_t)w.n_chunks * kvol * c_in * c_out * sizeof(float));
 }
 
-template <int CI, int CO>
+template <int CI, int CO, bool F16 = false>
 static int wgt_launch(const WgtParams &p, cudaStream_t st) {
-  constexpr int smem = WgtShape<CI, CO>::kSmem;
+  constexpr int smem = WgtShape<F16, CI, CO>::kSmem;
   const int n_items = p.n_chunks * p.kvol;
   const int grid = n_items < kNumSMs ? n_items : kNumSMs;
-  BEVB200_CUDA(cudaFuncSetAttribute(spconv_wgrad_tc_kernel<CI, CO>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  BEVB200_LAUNCH((spconv_wgrad_tc_kernel<CI, CO>), grid, kWgtThreads, smem, st, p);
+  BEVB200_CUDA(cudaFuncSetAttribute(spconv_wgrad_tc_kernel<F16, CI, CO>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    smem));
+  BEVB200_LAUNCH((spconv_wgrad_tc_kernel<F16, CI, CO>), grid, kWgtThreads, smem, st, p);
   return BEVB200_OK;
 }
 template <int CI>
@@ -265,6 +296,39 @@ int spconv_wgrad_tc(const float *features, const float *out_grad, const int32_t 
 }
 
 int spconv_wgrad_tc_image_channels(int c) { return wgt_eff(c); }
+
+size_t spconv_wgrad_tc_f16_workspace_bytes(int n_out, int c_in, int c_out, int kvol) {
+  if (!spconv_wgrad_tc_ok(c_in, c_out, kvol) || n_out <= 0) return 0;
+  const WgtPlan w = wgt_plan(n_out, c_in, c_out, kvol);
+  return align_up((size_t)w.n_chunks * kvol * c_in * c_out * sizeof(float));
+}
+
+int spconv_wgrad_tc_f16(const void *features, int f_channels, const void *out_grad, const int32_t *nbr, int n_in,
+                        int n_out, const int32_t *n_out_dev, int c_in, int c_out, int kvol, float *weight_grad,
+                        void *workspace, cudaStream_t st) {
+  BEVB200_REQUIRE(spconv_wgrad_tc_ok(c_in, c_out, kvol), "shape has no tensor-core filter gradient");
+  BEVB200_REQUIRE(n_out > 0 && n_in > 0, "empty operands");
+  BEVB200_REQUIRE(f_channels >= c_in && f_channels % 8 == 0 && c_out % 8 == 0 && f_channels <= wgt_eff_f16(c_in),
+                  "bad fp16 image width");
+  const WgtPlan w = wgt_plan(n_out, c_in, c_out, kvol);
+  WgtParams p;
+  memset(&p, 0, sizeof(p));
+  p.fsplit = (const uint8_t *)features;
+  p.gsplit = (const uint8_t *)out_grad;
+  p.f_row_bytes = f_channels * 2;
+  p.g_row_bytes = c_out * 2;
+  p.nbr = nbr;
+  p.n_out_dev = n_out_dev;
+  p.partial = (float *)workspace;
+  p.n_in = n_in; p.n_out = n_out; p.c_in = c_in; p.c_out = c_out; p.kvol = kvol;
+  p.n_tiles = w.n_tiles; p.n_chunks = w.n_chunks; p.tiles_per_chunk = w.tiles_per_chunk;
+  const int ci = wgt_eff_f16(c_in), co = wgt_eff_f16(c_out);
+  int rc;
+  if (ci == 64) rc = co == 64 ? wgt_launch<64, 64, true>(p, st) : wgt_launch<64, 128, true>(p, st);
+  else rc = co == 64 ? wgt_launch<128, 64, true>(p, st) : wgt_launch<128, 128, true>(p, st);
+  if (rc) return rc;
+  return spconv_wgrad_reduce(p.partial, (long long)kvol * c_in * c_out, p.n_chunks, weight_grad, st);
+}
 
 size_t spconv_wgrad_tc_split_workspace_bytes(int n_out, int c_in, int c_out, int kvol) {
   if (!spconv_wgrad_tc_ok(c_in, c_out, kvol) || n_out <= 0) return 0;

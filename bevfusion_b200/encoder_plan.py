@@ -4,13 +4,18 @@ a CUDA graph.  Replaces the python loop of mmdet3d/models/backbones/sparse_encod
 spconv/conv.py:114-223 (one rulebook build + ~80 launches + one device->host count per conv there).
 
 forward_train() is the same chain in training mode (batch-statistics BatchNorm, running statistics updated
-in place) with a native whole-encoder backward, also sync-free and capturable."""
+in place) with a native whole-encoder backward, also sync-free and capturable.
+
+A plan runs one precision: BF16x3 (the default, fp32 rows in and out) or FP16 (fp16 operands with fp32
+accumulation, half rows in and out; the numerical contract is in include/bevfusion_b200.h).  Each plan packs its
+own weight image, so a module keeps one plan per precision."""
 import ctypes
 
 import torch
 
 from . import _C
 from .sparse_block import SparseBasicBlock, bn_fold_key, bn_scale_shift
+from .spconv.ops import PREC_BF16X3, PREC_FP16
 
 
 class _ConvDesc(ctypes.Structure):
@@ -73,8 +78,13 @@ def supported(encoder):
 
 
 class EncoderPlan:
-    def __init__(self, encoder):
+    def __init__(self, encoder, precision=PREC_BF16X3):
+        if precision not in (PREC_BF16X3, PREC_FP16):
+            raise ValueError("an encoder plan runs the bf16x3 or the fp16 precision")
         self.encoder = encoder
+        self.precision = precision
+        self.f16 = precision == PREC_FP16
+        self.row_dtype = torch.float16 if self.f16 else torch.float32
         self.chain = _chain_of(encoder)
         L = _C.lib()
         descs = (_ConvDesc * len(self.chain))()
@@ -89,6 +99,8 @@ class EncoderPlan:
         _C.check(L.bevb200_encoder_create(int(encoder.in_channels), shape, descs, len(self.chain),
                                           ctypes.byref(handle)), "encoder_create")
         self._h = handle
+        if self.f16:
+            _C.check(L.bevb200_encoder_set_precision(self._h, PREC_FP16), "encoder_set_precision")
         self.n_levels = L.bevb200_encoder_num_levels(self._h)
         oshape = (ctypes.c_int32 * 3)()
         oc = ctypes.c_int32()
@@ -154,9 +166,10 @@ class EncoderPlan:
 
     def forward(self, voxel_features, coors, batch_size, n_voxels_dev=None, out=None, level_caps=None,
                 overlap_rulebooks=True):
-        """voxel_features [N, C] fp32, coors [N, 4] int32 (b, x, y, z); with n_voxels_dev (device
-        int32[1]) only the first n rows are valid -- nothing is read back.  Returns [B, C*D, H, W]."""
-        _C.require_cuda(voxel_features, "voxel_features", torch.float32)
+        """voxel_features [N, C] fp32 (an fp16 plan: fp16), coors [N, 4] int32 (b, x, y, z); with n_voxels_dev
+        (device int32[1]) only the first n rows are valid -- nothing is read back.  Returns [B, C*D, H, W] in the
+        rows' dtype."""
+        _C.require_cuda(voxel_features, "voxel_features", self.row_dtype)
         _C.require_cuda(coors, "coors", torch.int32)
         dev = voxel_features.device
         n = voxel_features.shape[0]
@@ -167,9 +180,11 @@ class EncoderPlan:
         L = _C.lib()
         with torch.cuda.device(dev):
             if out is None:
-                out = torch.empty(shape, dtype=torch.float32, device=dev)
+                out = torch.empty(shape, dtype=self.row_dtype, device=dev)
+            elif out.dtype != self.row_dtype:
+                raise ValueError("out= must have the plan's row dtype %s" % self.row_dtype)
             from .spconv.ops import _batch_stride_of
-            stride = _batch_stride_of(out, shape)
+            stride = _batch_stride_of(out, shape, self.row_dtype)
             if n == 0:
                 out.zero_()
                 return out
@@ -192,10 +207,10 @@ class EncoderPlan:
                 if self._side is None or self._side.device != dev:
                     self._side = torch.cuda.Stream(device=dev)
                 side = self._side.cuda_stream
-            rc = L.bevb200_encoder_forward(self._h, _C.ptr(self._params), _C.ptr(voxel_features), _C.ptr(coors),
-                                           n, _C.ptr(n_voxels_dev), B, caps, _C.ptr(out), stride,
-                                           _C.ptr(self.status), _C.ptr(self._ws), self._ws.numel(),
-                                           _C.current_stream(dev), side)
+            fwd = L.bevb200_encoder_forward_f16 if self.f16 else L.bevb200_encoder_forward
+            rc = fwd(self._h, _C.ptr(self._params), _C.ptr(voxel_features), _C.ptr(coors), n, _C.ptr(n_voxels_dev),
+                     B, caps, _C.ptr(out), stride, _C.ptr(self.status), _C.ptr(self._ws), self._ws.numel(),
+                     _C.current_stream(dev), side)
         _C.check(rc, "encoder_forward")
         return out
 
@@ -211,14 +226,17 @@ class EncoderPlan:
 
     def saved_rows(self, state, max_voxels, batch_size, conv, level_caps=None):
         """(pre-BN rows z, output rows y) of conv `conv` as saved by a training forward into `state`: fp32
-        [cap, c_out] each (y decoded from its split image); only the level's first status[1 + l] rows are
-        defined."""
+        [cap, c_out] each (y decoded from its split image; an fp16 plan: the saved z16 and y16, fp16 [cap, c_out]);
+        only the level's first status[1 + l] rows are defined."""
         zo, yo = ctypes.c_size_t(), ctypes.c_size_t()
         _C.check(_C.lib().bevb200_encoder_train_saved(self._h, int(max_voxels), int(batch_size),
                                                       self._caps_arg(level_caps), int(conv), ctypes.byref(zo),
                                                       ctypes.byref(yo)), "encoder_train_saved")
         c = self.chain[conv][0].out_channels
         cap = self.level_caps(max_voxels, batch_size, level_caps)[self.level_of(conv)]
+        if self.f16:
+            return (state[zo.value:zo.value + cap * c * 2].view(torch.float16).view(cap, c),
+                    state[yo.value:yo.value + cap * c * 2].view(torch.float16).view(cap, c))
         z = state[zo.value:zo.value + cap * c * 4].view(torch.float32).view(cap, c)
         img = state[yo.value:yo.value + cap * c * 4].view(torch.bfloat16).view(cap, c // 16, 2, 16).float()
         return z, (img[:, :, 0] + img[:, :, 1]).reshape(cap, c)
@@ -227,25 +245,31 @@ class EncoderPlan:
         """level of conv `conv`'s output rows (0 = the voxels)."""
         return sum(1 for cv, _, _, _ in self.chain[:conv + 1] if not cv.subm)
 
-    def _bn_descs(self, bn_weights, bn_biases):
+    def _bn_descs(self, bn_weights, bn_biases, running):
         descs = (_BNDesc * len(self.chain))()
-        for d, (_, bn, _, _), g, b in zip(descs, self.chain, bn_weights, bn_biases):
+        for d, (_, bn, _, _), g, b, (rm, rv) in zip(descs, self.chain, bn_weights, bn_biases, running):
             d.weight, d.bias = g.data_ptr(), b.data_ptr()
-            d.running_mean, d.running_var = bn.running_mean.data_ptr(), bn.running_var.data_ptr()
+            d.running_mean, d.running_var = rm.data_ptr(), rv.data_ptr()
             d.num_batches_tracked = _C.ptr(bn.num_batches_tracked)
             d.eps, d.momentum = float(bn.eps), float(bn.momentum)
         return descs
 
     def _forward_train_native(self, voxel_features, coors, batch_size, n_voxels_dev, level_caps, overlap_rulebooks,
                               weights, bn_weights, bn_biases):
-        """One training forward: returns (dense output, state).  Updates the running statistics in place."""
+        """One training forward: returns (dense output, state).  Updates the running statistics in place.
+        An fp16 plan takes half or fp32 features (rounded once to fp16) and widens half weights and BN tensors
+        for the call (the C ABI takes fp32 parameters); half running statistics are updated through fp32 copies."""
         dev = voxel_features.device
         n = voxel_features.shape[0]
         B = int(batch_size)
         X, Y, Z = self.out_shape
         L = _C.lib()
+        voxel_features = voxel_features.to(self.row_dtype).contiguous()
+        weights = [_f32(w) for w in weights]
+        bn_weights, bn_biases = [_f32(g) for g in bn_weights], [_f32(b) for b in bn_biases]
+        running = [(_f32(bn.running_mean), _f32(bn.running_var)) for _, bn, _, _ in self.chain]
         with torch.cuda.device(dev):
-            out = torch.empty((B, self.out_channels * Z, X, Y), dtype=torch.float32, device=dev)
+            out = torch.empty((B, self.out_channels * Z, X, Y), dtype=self.row_dtype, device=dev)
             caps = self._caps_arg(level_caps)
             state = torch.empty(L.bevb200_encoder_train_state_bytes(self._h, n, B, caps), dtype=torch.uint8,
                                 device=dev)
@@ -257,11 +281,15 @@ class EncoderPlan:
                     self._side = torch.cuda.Stream(device=dev)
                 side = self._side.cuda_stream
             wp = (ctypes.c_void_p * len(weights))(*[w.data_ptr() for w in weights])
-            rc = L.bevb200_encoder_forward_train(self._h, wp, self._bn_descs(bn_weights, bn_biases),
-                                                 _C.ptr(voxel_features), _C.ptr(coors), n, _C.ptr(n_voxels_dev), B,
-                                                 caps, _C.ptr(out), 0, _C.ptr(self.status), _C.ptr(state),
-                                                 state.numel(), _C.current_stream(dev), side)
+            fwd = L.bevb200_encoder_forward_train_f16 if self.f16 else L.bevb200_encoder_forward_train
+            rc = fwd(self._h, wp, self._bn_descs(bn_weights, bn_biases, running), _C.ptr(voxel_features),
+                     _C.ptr(coors), n, _C.ptr(n_voxels_dev), B, caps, _C.ptr(out), 0, _C.ptr(self.status),
+                     _C.ptr(state), state.numel(), _C.current_stream(dev), side)
         _C.check(rc, "encoder_forward_train")
+        for (_, bn, _, _), (rm, rv) in zip(self.chain, running):
+            if rm is not bn.running_mean:          # half running statistics: updated through fp32 copies
+                bn.running_mean.copy_(rm)
+                bn.running_var.copy_(rv)
         # torch's BatchNorm bumps num_batches_tracked's version (add_(1)); the eval plan's fold key reads it
         for _, bn, _, _ in self.chain:
             if bn.num_batches_tracked is not None:
@@ -269,13 +297,16 @@ class EncoderPlan:
         return out, state
 
     def _backward_native(self, state, n, batch_size, level_caps, grad_out, weights, need_input):
+        """Gradients in the native dtypes: features in the plan's row dtype, everything else fp32."""
         dev = grad_out.device
         L = _C.lib()
+        grad_out = grad_out.to(self.row_dtype).contiguous()
+        weights = [_f32(w) for w in weights]
         with torch.cuda.device(dev):
             caps = self._caps_arg(level_caps)
             ws = torch.empty(L.bevb200_encoder_backward_workspace_bytes(self._h, n, int(batch_size), caps),
                              dtype=torch.uint8, device=dev)
-            gfeat = (torch.empty((n, self.encoder.in_channels), dtype=torch.float32, device=dev)
+            gfeat = (torch.empty((n, self.encoder.in_channels), dtype=self.row_dtype, device=dev)
                      if need_input else None)
             gw = [torch.empty_like(w) for w in weights]
             gg = [torch.empty(cv.out_channels, dtype=torch.float32, device=dev) for cv, _, _, _ in self.chain]
@@ -284,9 +315,9 @@ class EncoderPlan:
             def arr(ts):
                 return (ctypes.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
 
-            rc = L.bevb200_encoder_backward(self._h, arr(weights), _C.ptr(state), state.numel(), n, int(batch_size),
-                                            caps, _C.ptr(grad_out), 0, _C.ptr(gfeat), arr(gw), arr(gg), arr(gb),
-                                            _C.ptr(ws), ws.numel(), _C.current_stream(dev))
+            bwd = L.bevb200_encoder_backward_f16 if self.f16 else L.bevb200_encoder_backward
+            rc = bwd(self._h, arr(weights), _C.ptr(state), state.numel(), n, int(batch_size), caps, _C.ptr(grad_out),
+                     0, _C.ptr(gfeat), arr(gw), arr(gg), arr(gb), _C.ptr(ws), ws.numel(), _C.current_stream(dev))
         _C.check(rc, "encoder_backward")
         return gfeat, gw, gg, gb
 
@@ -296,8 +327,13 @@ class EncoderPlan:
         voxel_features [N, C] fp32, coors [N, 4] int32, n_voxels_dev as in forward().  Differentiable in the
         features, every conv weight and every BN weight / bias; the backward is one native call on this
         forward's rulebooks.  Under torch.no_grad() it still normalises with batch statistics and updates the
-        running statistics, and keeps nothing for a backward."""
-        _C.require_cuda(voxel_features, "voxel_features", torch.float32)
+        running statistics, and keeps nothing for a backward.
+        An fp16 plan also takes half features, half conv weights and half BN modules; its output is half and the
+        gradients come back in each tensor's dtype."""
+        ok = (torch.float32, torch.float16) if self.f16 else (torch.float32,)
+        if voxel_features.dtype not in ok:
+            raise ValueError("voxel_features must be %s" % " or ".join(str(t) for t in ok))
+        _C.require_cuda(voxel_features, "voxel_features", voxel_features.dtype)
         _C.require_cuda(coors, "coors", torch.int32)
         n = voxel_features.shape[0]
         assert coors.shape[0] == n and coors.shape[1] == 4 and voxel_features.shape[1] == self.encoder.in_channels
@@ -305,7 +341,9 @@ class EncoderPlan:
             raise ValueError("a training forward needs at least one voxel (BatchNorm statistics)")
         weights = [conv.weight for conv, _, _, _ in self.chain]
         for w in weights:
-            _C.require_cuda(w, "conv weight", torch.float32)
+            if w.dtype not in ok:
+                raise ValueError("conv weights must be %s" % " or ".join(str(t) for t in ok))
+            _C.require_cuda(w, "conv weight", w.dtype)
         bn_w = [bn.weight for _, bn, _, _ in self.chain]
         bn_b = [bn.bias for _, bn, _, _ in self.chain]
         params = weights + bn_w + bn_b
@@ -322,6 +360,11 @@ class EncoderPlan:
         return self.status is not None and int(self.status[0].item()) != 0
 
 
+def _f32(t):
+    """t itself when fp32, else an fp32 copy (the C ABI takes fp32 parameters)."""
+    return t if t.dtype == torch.float32 else t.detach().float().contiguous()
+
+
 class _EncoderTrainFn(torch.autograd.Function):
     """EncoderPlan.forward_train with the native backward.  The conv and BN parameters are saved with
     save_for_backward, so an in-place update between forward and backward raises; the state (rulebooks,
@@ -334,6 +377,7 @@ class _EncoderTrainFn(torch.autograd.Function):
                                                 overlap_rulebooks, params[:nc], params[nc:2 * nc], params[2 * nc:])
         ctx.save_for_backward(state, *params)     # the state is freed with the graph's saved tensors
         ctx.plan, ctx.n, ctx.batch_size, ctx.level_caps = plan, voxel_features.shape[0], batch_size, level_caps
+        ctx.feature_dtype = voxel_features.dtype
         return out
 
     @staticmethod
@@ -343,4 +387,7 @@ class _EncoderTrainFn(torch.autograd.Function):
         nc = len(plan.chain)
         gfeat, gw, gg, gb = plan._backward_native(state, ctx.n, ctx.batch_size, ctx.level_caps,
                                                   grad_out.contiguous(), params[:nc], ctx.needs_input_grad[6])
-        return (None,) * 6 + (gfeat,) + tuple(gw) + tuple(gg) + tuple(gb)
+        if gfeat is not None:
+            gfeat = gfeat.to(ctx.feature_dtype)
+        grads = [g.to(p.dtype) for g, p in zip(gw + gg + gb, params)]     # each in its parameter's dtype
+        return (None,) * 6 + (gfeat,) + tuple(grads)

@@ -47,18 +47,21 @@ class SparseEncoder(nn.Module):
         # BEVB200_ENCODER_NATIVE=0 keeps the per-conv python loop below (A/B runs, other precisions)
         self.native_plan = os.environ.get("BEVB200_ENCODER_NATIVE", "1") != "0"
         self._plan = None
+        self._plan_f16 = None        # the fp16 plan: its own weight image, never shared with the bf16x3 one
         self.rulebook_lookahead = os.environ.get("BEVB200_RULEBOOK_LOOKAHEAD", "1") != "0"
         self.conv_out = make_sparse_convmodule(encoder_out_channels, self.output_channels,
                                                kernel_size=(1, 1, 3), stride=(1, 1, 2),
                                                norm_cfg=norm_cfg, padding=0,
                                                indice_key="spconv_down2", conv_type="SparseConv3d")
 
-    def plan(self):
-        """The native EncoderPlan of this module (built lazily), or None when a layer has no native form."""
-        if self._plan is None:
+    def plan(self, precision=sp_ops.PREC_BF16X3):
+        """The native EncoderPlan of this module for `precision` (bf16x3 or fp16, built lazily), or None when a
+        layer has no native form."""
+        attr = "_plan_f16" if precision == sp_ops.PREC_FP16 else "_plan"
+        if getattr(self, attr) is None:
             from . import encoder_plan
-            self._plan = encoder_plan.EncoderPlan(self) if encoder_plan.supported(self) else False
-        return self._plan or None
+            setattr(self, attr, encoder_plan.EncoderPlan(self, precision) if encoder_plan.supported(self) else False)
+        return getattr(self, attr) or None
 
     def forward(self, voxel_features, coors, batch_size, fused=None, precision=None, out=None,
                 num_voxels=None, **kwargs):
@@ -69,12 +72,18 @@ class SparseEncoder(nn.Module):
         fused=None picks the fused path (BN / ReLU / residual in the conv epilogues, dense()
         written directly in the output layout) whenever the module is in eval mode.  `out`
         (fused path) is an optional [B, C*D, H, W] view to write into, e.g. the LiDAR channels
-        of the fuser's concatenated input (fusers/conv.py:16)."""
+        of the fuser's concatenated input (fusers/conv.py:16).
+
+        precision=sp_ops.PREC_FP16 runs the native plan in fp16 (fp32 accumulation; the contract is in
+        include/bevfusion_b200.h) and returns half: in eval mode under no_grad, and in training mode with
+        `num_voxels=`.  Anything else raises a ValueError; there is no fp16 form of the per-conv path."""
         coors = coors.int()
         if fused is None:
             fused = not self.training and self.order == ("conv", "norm", "act")
         if precision is None:
             precision = sp_ops.default_precision()
+        if precision == sp_ops.PREC_FP16:
+            return self._forward_fp16(voxel_features, coors, batch_size, fused, out, num_voxels)
         if (fused and self.native_plan and precision == sp_ops.PREC_BF16X3 and not torch.is_grad_enabled()
                 and voxel_features.dtype == torch.float32 and self.conv_input[0].weight.dtype == torch.float32
                 and self.plan() is not None):
@@ -106,23 +115,48 @@ class SparseEncoder(nn.Module):
         sync-free and capturable.  What it does not cover raises instead of falling back."""
         def refuse(reason):
             raise ValueError("num_voxels= in training mode runs the native training plan, which needs " + reason)
-        if precision != sp_ops.PREC_BF16X3:
-            refuse("the bf16x3 precision")
-        if voxel_features.dtype != torch.float32 or any(p.dtype != torch.float32 for p in self.parameters()):
+        if precision == sp_ops.PREC_FP16:
+            if voxel_features.dtype not in (torch.float32, torch.float16):
+                refuse("fp32 or fp16 features")
+        elif precision != sp_ops.PREC_BF16X3:
+            refuse("the bf16x3 or the fp16 precision")
+        elif voxel_features.dtype != torch.float32 or any(p.dtype != torch.float32 for p in self.parameters()):
             refuse("fp32 features and weights (no half)")
         if out is not None:
             refuse("no out= (the output is a fresh tensor)")
-        if self.plan() is None:
+        plan = self.plan(precision)
+        if plan is None:
             refuse("a chain of (conv, norm, act) modules with tensor-core channel counts")
-        for conv, bn, _, _ in self.plan().chain:
+        for conv, bn, _, _ in plan.chain:
             if conv.bias is not None:
                 refuse("convs without bias")
             if bn is None or not bn.affine or not bn.track_running_stats:
                 refuse("an affine BatchNorm1d with running statistics after every conv")
             if bn.momentum is None:
                 refuse("a BatchNorm momentum (momentum=None, the cumulative average, is not covered)")
-        return self.plan().forward_train(voxel_features.contiguous(), coors.contiguous(), batch_size,
-                                         n_voxels_dev=num_voxels, overlap_rulebooks=self.overlap_rulebooks)
+        return plan.forward_train(voxel_features.contiguous(), coors.contiguous(), batch_size,
+                                  n_voxels_dev=num_voxels, overlap_rulebooks=self.overlap_rulebooks)
+
+    def _forward_fp16(self, voxel_features, coors, batch_size, fused, out, num_voxels):
+        """precision=PREC_FP16: the fp16 plan, or a ValueError before anything runs."""
+        if self.training:
+            if num_voxels is None:
+                raise ValueError("fp16 training runs the native training plan: pass num_voxels= (device int32[1])")
+            return self._forward_train_native(voxel_features, coors, batch_size, num_voxels, sp_ops.PREC_FP16, out)
+        if not fused:
+            raise ValueError("the fp16 precision runs on the native plan only (no per-conv path): fused must not be False")
+        if torch.is_grad_enabled():
+            raise ValueError("fp16 in eval mode runs the native plan under torch.no_grad() only")
+        if voxel_features.dtype not in (torch.float32, torch.float16):
+            raise ValueError("the fp16 plan takes fp32 or fp16 features")
+        plan = self.plan(sp_ops.PREC_FP16)
+        if plan is None:
+            raise ValueError("the fp16 precision needs a chain of (conv, norm, act) modules with tensor-core channel "
+                             "counts")
+        if out is not None and out.dtype != torch.float16:
+            raise ValueError("out= of an fp16 forward must be half")
+        return plan.forward(voxel_features.to(torch.float16).contiguous(), coors.contiguous(), batch_size,
+                            n_voxels_dev=num_voxels, out=out, overlap_rulebooks=self.overlap_rulebooks)
 
     @staticmethod
     def _convmodule_fused(seq, x, precision):

@@ -18,6 +18,9 @@ import torch
 from .. import _C
 
 PREC_FP32, PREC_TF32X3, PREC_TF32, PREC_BF16X3 = 0, 1, 2, 3
+# fp16 operands with fp32 accumulation: only the native encoder plan runs it (SparseEncoder.forward(precision=...));
+# it is not one of the BEVB200_SPCONV_PRECISION names, and the per-conv ops refuse it
+PREC_FP16 = 4
 _PREC_NAMES = {"fp32": PREC_FP32, "tf32x3": PREC_TF32X3, "tf32": PREC_TF32, "bf16x3": PREC_BF16X3}
 
 
@@ -390,11 +393,11 @@ class _SparseConvExt:
 sparse_conv_ext = _SparseConvExt()
 
 
-def _batch_stride_of(out, shape):
+def _batch_stride_of(out, shape, dtype=torch.float32):
     """`out` must be a [B, C, ...] view that is dense inside each batch item (a channel slice
     of a wider channels-first buffer qualifies); returns its batch stride in elements."""
-    if tuple(out.shape) != tuple(shape) or out.dtype != torch.float32:
-        raise ValueError(f"out must be float32 of shape {tuple(shape)}")
+    if tuple(out.shape) != tuple(shape) or out.dtype != dtype:
+        raise ValueError(f"out must be {dtype} of shape {tuple(shape)}")
     inner = 1
     for size, stride in zip(reversed(out.shape[1:]), reversed(out.stride()[1:])):
         if size != 1 and stride != inner:

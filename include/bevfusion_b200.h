@@ -932,6 +932,8 @@ BEVB200_API int bevb200_pairs_to_nbr(const int32_t *indice_pairs, const int32_t 
 #define BEVB200_PREC_TF32X3 1
 #define BEVB200_PREC_TF32 2
 #define BEVB200_PREC_BF16X3 3 /* bf16 MMAs: a = bf16 hi + bf16 lo, hi*hi + hi*lo + lo*hi (3 MMAs per 16 K) */
+#define BEVB200_PREC_FP16 4   /* fp16 operands, fp32 accumulation (1 MMA per 16 K): the encoder plan only
+                                 (bevb200_encoder_set_precision); the per-conv calls refuse it */
 BEVB200_API int bevb200_spconv_forward(const float *features, const float *weight, const int32_t *nbr,
                            int n_in, int n_out, int c_in, int c_out, int kernel_volume,
                            const float *scale, const float *shift, const float *residual,
@@ -1069,6 +1071,27 @@ typedef struct bevb200_encoder bevb200_encoder_t;
 BEVB200_API int bevb200_encoder_create(int in_channels, const int32_t *sparse_shape_host,
                            const bevb200_encoder_conv_t *convs, int n_convs, bevb200_encoder_t **out);
 BEVB200_API void bevb200_encoder_destroy(bevb200_encoder_t *enc);
+/* FP16 plans.  bevb200_encoder_set_precision(enc, BEVB200_PREC_FP16) makes a plan fp16 (BEVB200_PREC_BF16X3, the
+ * default, makes it BF16x3 again); call it before the size queries and set_conv, which then report and pack the fp16
+ * layout.  An fp16 plan runs only the _f16 calls below, a BF16x3 plan only the others: the wrong one returns
+ * BEVB200_EINVAL before it writes anything.  In the _f16 calls the row data is half (voxel_features, dense_out,
+ * grad_dense, grad_voxel_features); weights, BN parameters and weight / BN gradients stay fp32.
+ * Numerical contract (fp32 accumulation throughout; every conversion to fp16 rounds to nearest, overflows to +-inf
+ * and keeps NaN, so a loss scaler sees an overflow):
+ *   inputs     voxel features are rounded once to fp16 (half features pass exactly); the weights are rounded to fp16
+ *              when packed (set_conv; forward_train_f16 packs the live weights on every call)
+ *   eval       y16 = fp16(relu(acc * scale + shift [+ y16 of residual_from])), one rounding per conv
+ *   training   z16 = fp16(acc) is saved; the batch mean / variance are those of z16 (double partials over fixed
+ *              2048-row chunks, bit-reproducible); running statistics fp32, updated as in forward_train (and
+ *              BEVB200_ENCODER_FEW_ROWS likewise); y16 = fp16(relu(gamma (z16 - mean) invstd + beta [+ y16 res]))
+ *   output     dense_out [B, C*Z, X, Y] half holds the last conv's y16 exactly
+ *   backward   grad_dense half; the BN backward runs in fp32 on z16; dz is rounded once to an fp16 image that is the
+ *              MMA operand of the input gradient (forward kernel on W^T) and of the filter gradient; dW in fp32
+ *              with the ordered chunk reduce; grad_voxel_features rounded once to fp16; BN gradients fp32
+ * train_saved on an fp16 plan gives the offsets of z16 ([cap, c_out] half) and of the fp16 image y16 ([cap, c_out]
+ * half).  bevb200_encoder_precision returns the plan's precision. */
+BEVB200_API int bevb200_encoder_set_precision(bevb200_encoder_t *enc, int precision);
+BEVB200_API int bevb200_encoder_precision(const bevb200_encoder_t *enc);
 BEVB200_API size_t bevb200_encoder_param_bytes(const bevb200_encoder_t *enc);
 BEVB200_API int bevb200_encoder_num_levels(const bevb200_encoder_t *enc);
 BEVB200_API int bevb200_encoder_output_shape(const bevb200_encoder_t *enc, int32_t *shape_out, int32_t *channels_out);
@@ -1083,6 +1106,11 @@ BEVB200_API int bevb200_encoder_forward(bevb200_encoder_t *enc, const void *para
                             int batch_size, const int32_t *level_caps_host, float *dense_out,
                             long long out_batch_stride, int32_t *status_dev, void *workspace,
                             size_t workspace_bytes, void *stream, void *rulebook_stream);
+BEVB200_API int bevb200_encoder_forward_f16(bevb200_encoder_t *enc, const void *params, const void *voxel_features,
+                                const int32_t *coors, int max_voxels, const int32_t *n_voxels_dev,
+                                int batch_size, const int32_t *level_caps_host, void *dense_out,
+                                long long out_batch_stride, int32_t *status_dev, void *workspace,
+                                size_t workspace_bytes, void *stream, void *rulebook_stream);
 
 /* status_dev[0] bits of the encoder calls */
 #define BEVB200_ENCODER_TRUNCATED 1  /* a level cap truncated a level's rows */
@@ -1126,6 +1154,12 @@ BEVB200_API int bevb200_encoder_forward_train(bevb200_encoder_t *enc, const floa
                                   int batch_size, const int32_t *level_caps_host, float *dense_out,
                                   long long out_batch_stride, int32_t *status_dev, void *state,
                                   size_t state_bytes, void *stream, void *rulebook_stream);
+BEVB200_API int bevb200_encoder_forward_train_f16(bevb200_encoder_t *enc, const float *const *weights,
+                                      const bevb200_encoder_bn_t *bn, const void *voxel_features,
+                                      const int32_t *coors, int max_voxels, const int32_t *n_voxels_dev,
+                                      int batch_size, const int32_t *level_caps_host, void *dense_out,
+                                      long long out_batch_stride, int32_t *status_dev, void *state,
+                                      size_t state_bytes, void *stream, void *rulebook_stream);
 BEVB200_API size_t bevb200_encoder_backward_workspace_bytes(const bevb200_encoder_t *enc, int max_voxels,
                                                 int batch_size, const int32_t *level_caps_host);
 BEVB200_API int bevb200_encoder_backward(const bevb200_encoder_t *enc, const float *const *weights,
@@ -1135,6 +1169,13 @@ BEVB200_API int bevb200_encoder_backward(const bevb200_encoder_t *enc, const flo
                              float *const *grad_weights, float *const *grad_bn_weight,
                              float *const *grad_bn_bias, void *workspace, size_t workspace_bytes,
                              void *stream);
+BEVB200_API int bevb200_encoder_backward_f16(const bevb200_encoder_t *enc, const float *const *weights,
+                                 const void *state, size_t state_bytes, int max_voxels, int batch_size,
+                                 const int32_t *level_caps_host, const void *grad_dense,
+                                 long long out_batch_stride, void *grad_voxel_features,
+                                 float *const *grad_weights, float *const *grad_bn_weight,
+                                 float *const *grad_bn_bias, void *workspace, size_t workspace_bytes,
+                                 void *stream);
 
 /* ---- PointPillars pillar feature net, training mode (pillar_encoder.py:43-176, BatchNorm1d in train mode) ----
  * The net of bevb200_pillar_features (F 3..8, P 1..32, feat_channels [64, 64], no distance feature; anything else
