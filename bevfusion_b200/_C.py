@@ -37,6 +37,20 @@ _SIGNATURES = {
                                                + [c_int, _P, _P, _P, c_size_t, _P]),
     "bevb200_bev_pool_lift_backward_workspace_bytes": (c_size_t, [c_int] * 2),
     "bevb200_bev_pool_lift_backward": (c_int, [c_int] * 8 + [_P] * 3 + [c_int] * 2 + [_P] * 6 + [_P, c_size_t, _P]),
+    "bevb200_bev_pool_dev_workspace_bytes": (c_size_t, [c_int] * 2),
+    "bevb200_bev_pool_perm_dev": (c_int, [c_int] * 6 + [_P] * 8 + [c_size_t, _P]),
+    "bevb200_bev_pool_grad_perm_dev": (c_int, [c_int] * 6 + [_P] * 8),
+    "bevb200_bev_pool_lift_dev": (c_int, [c_int] * 6 + [_P, _P, c_int, c_int] + [_P] * 8 + [c_size_t, _P]),
+    "bevb200_bev_pool_lift_prepare_dev_workspace_bytes": (c_size_t, [c_int] * 2),
+    "bevb200_bev_pool_lift_prepare_dev": (c_int, [_P] * 3 + [c_int] * 6 + [_P] * 8 + [c_size_t, _P]),
+    "bevb200_bev_pool_lift_columns_dev_workspace_bytes": (c_size_t, [c_int] * 3),
+    "bevb200_bev_pool_lift_columns_dev": (c_int, [c_int] * 6 + [_P, _P] + [c_int] * 4 + [_P] * 7 + [c_int]
+                                          + [_P] * 4 + [c_size_t, _P]),
+    "bevb200_bev_pool_lift_columns_backward_dev_workspace_bytes": (c_size_t, [c_int] * 2),
+    "bevb200_bev_pool_lift_columns_backward_dev": (c_int, [c_int] * 6 + [_P] * 3 + [c_int] * 4 + [_P] * 5 + [c_int]
+                                                   + [_P] * 6 + [c_size_t, _P]),
+    "bevb200_bev_pool_lift_backward_dev_workspace_bytes": (c_size_t, [c_int] * 2),
+    "bevb200_bev_pool_lift_backward_dev": (c_int, [c_int] * 6 + [_P] * 3 + [c_int] * 2 + [_P] * 9 + [c_size_t, _P]),
     "bevb200_bev_pool_prepare_workspace_bytes": (c_size_t, [c_int]),
     "bevb200_bev_pool_prepare_geom": (c_int, [_P, c_int, c_int, _P, _P, _P, c_int] + [_P] * 7
                                       + [c_size_t, _P]),

@@ -21,6 +21,11 @@ from . import _C
 
 __all__ = ["bev_pool", "bev_pool_ext", "QuickCumsumCuda", "BEVPoolPlan", "gen_dx_bx"]
 
+# status word of a sync-free plan's fused lift (tables.lift_form; BEVB200_LIFT_* in include/bevfusion_b200.h)
+_LIFT_COLUMNS, _LIFT_ROWS = 0, 1
+# default column-table cap of a sync-free plan, per (camera, image column, depth bin): see DESIGN.md section 4.24
+_SEGMENTS_PER_COLUMN_BIN = 5
+
 
 def _ws(nbytes, device):
     return torch.empty(max(int(nbytes), 256), dtype=torch.uint8, device=device)
@@ -101,13 +106,35 @@ class QuickCumsumCuda(torch.autograd.Function):
 
 
 class _PoolTables:
-    """Device-resident rank / perm / interval tables of one (geometry, grid) pair."""
+    """Device-resident rank / perm / interval tables of one (geometry, grid) pair.
 
-    def __init__(self, ranks, perm, geom, starts, lengths, n_kept, n_intervals, n_total, dims):
+    Tables of a sync-free plan (BEVPoolPlan.from_cameras(..., sync=False)) are sized for all n_total points and carry
+    `counts`, int32 [4] on the device = {n_kept, n_intervals, n_segments, lift form}; n_kept, n_intervals, n_segments
+    and lift_form are then 0-d views of it, and only the leading n_kept / n_intervals entries of the tables are valid."""
+
+    def __init__(self, ranks, perm, geom, starts, lengths, n_kept, n_intervals, n_total, dims, counts=None):
         self.ranks, self.perm, self.geom = ranks, perm, geom
         self.starts, self.lengths = starts, lengths
         self.n_kept, self.n_intervals, self.n_total = n_kept, n_intervals, n_total
         self.dims = dims  # (B, D, H, W)
+        self.counts = counts
+        if counts is not None:
+            self.n_segments, self.lift_form = counts[2], counts[3]
+        self._ws_cache = {}
+
+    def counts_ptr(self, k):
+        """device address of counts[k]"""
+        return _C.ptr(self.counts) + 4 * k
+
+    def workspace(self, key, nbytes, device):
+        """A workspace kept with the tables (sync-free plans allocate once per channel count).  One asked for during a
+        CUDA-graph capture comes from the graph's pool and is not kept."""
+        if torch.cuda.is_current_stream_capturing():
+            return _ws(nbytes, device)
+        ws = self._ws_cache.get(key)
+        if ws is None or ws.numel() < nbytes:
+            ws = self._ws_cache[key] = _ws(nbytes, device)
+        return ws
 
 
 def _finish_tables(n_total, device, dims, call):
@@ -178,6 +205,23 @@ def prepare_from_geometry(geom_xyz, dx, bx, nx, B):
                                   ws.numel(), _C.current_stream(g.device)))
 
 
+def _camera_params(dev, B, N, camera2lidar_rots, camera2lidar_trans, intrins, post_rots, post_trans, extra_rots,
+                   extra_trans, inverse):
+    """cam_params [B*N, 24] and extra_params [B, 12] (or None) of bevb200_bev_pool_prepare_cameras; `inverse` computes
+    the batched 3x3 inverses"""
+    f32 = dict(dtype=torch.float32, device=dev)
+    inv_post = inverse(post_rots.to(**f32))
+    combine = camera2lidar_rots.to(**f32).matmul(inverse(intrins.to(**f32)))
+    cam = torch.cat([inv_post.reshape(B * N, 9), post_trans.to(**f32).reshape(B * N, 3), combine.reshape(B * N, 9),
+                     camera2lidar_trans.to(**f32).reshape(B * N, 3)], 1).contiguous()
+    extra = None
+    if extra_rots is not None or extra_trans is not None:
+        er = extra_rots.to(**f32) if extra_rots is not None else torch.eye(3, **f32).repeat(B, 1, 1)
+        et = extra_trans.to(**f32) if extra_trans is not None else torch.zeros(B, 3, **f32)
+        extra = torch.cat([er.reshape(B, 9), et.reshape(B, 3)], 1).contiguous()
+    return cam, extra
+
+
 def prepare_from_cameras(frustum, camera2lidar_rots, camera2lidar_trans, intrins, post_rots, post_trans, dx, bx, nx,
                          extra_rots=None, extra_trans=None, return_geometry=False):
     """get_geometry (base.py:92-135) + quantise / filter / rank / sort / intervals in one library call: the
@@ -188,15 +232,8 @@ def prepare_from_cameras(frustum, camera2lidar_rots, camera2lidar_trans, intrins
     dev = frustum.device
     B, N = camera2lidar_trans.shape[:2]
     f32 = dict(dtype=torch.float32, device=dev)
-    inv_post = torch.inverse(post_rots.to(**f32))
-    combine = camera2lidar_rots.to(**f32).matmul(torch.inverse(intrins.to(**f32)))
-    cam = torch.cat([inv_post.reshape(B * N, 9), post_trans.to(**f32).reshape(B * N, 3), combine.reshape(B * N, 9),
-                     camera2lidar_trans.to(**f32).reshape(B * N, 3)], 1).contiguous()
-    extra = None
-    if extra_rots is not None or extra_trans is not None:
-        er = extra_rots.to(**f32) if extra_rots is not None else torch.eye(3, **f32).repeat(B, 1, 1)
-        et = extra_trans.to(**f32) if extra_trans is not None else torch.zeros(B, 3, **f32)
-        extra = torch.cat([er.reshape(B, 9), et.reshape(B, 3)], 1).contiguous()
+    cam, extra = _camera_params(dev, B, N, camera2lidar_rots, camera2lidar_trans, intrins, post_rots, post_trans,
+                                extra_rots, extra_trans, torch.inverse)
     fr = frustum.reshape(-1, 3).contiguous()
     n_fr = fr.shape[0]
     n_total = n_fr * B * N
@@ -224,6 +261,16 @@ class _PoolPerm(torch.autograd.Function):
         c = x.shape[1]
         with torch.cuda.device(x.device):
             out = torch.empty((B, D, H, W, c), dtype=x.dtype, device=x.device)
+            if tables.counts is not None:       # sync-free tables: sizes from the device
+                L = _C.lib()
+                ws = tables.workspace(("pool", c), L.bevb200_bev_pool_dev_workspace_bytes(tables.n_total, c), x.device)
+                rc = L.bevb200_bev_pool_perm_dev(
+                    B, D, H, W, tables.n_total, c, _C.ptr(x), _C.ptr(tables.perm), _C.ptr(tables.geom),
+                    _C.ptr(tables.starts), _C.ptr(tables.lengths), _C.ptr(tables.counts), _C.ptr(out), _C.ptr(ws),
+                    ws.numel(), _C.current_stream(x.device))
+                _C.check(rc, "bev_pool_perm_dev")
+                ctx.tables, ctx.c = tables, c
+                return out
             ws = _ws(_C.lib().bevb200_bev_pool_workspace_bytes(tables.n_kept, c), x.device)
             rc = _C.lib().bevb200_bev_pool_perm(
                 B, D, H, W, tables.n_kept, c, tables.n_intervals, _C.ptr(x), _C.ptr(tables.perm),
@@ -241,6 +288,12 @@ class _PoolPerm(torch.autograd.Function):
         out_grad = out_grad.contiguous()
         with torch.cuda.device(out_grad.device):
             x_grad = torch.empty((t.n_total, ctx.c), dtype=out_grad.dtype, device=out_grad.device)
+            if t.counts is not None:
+                rc = _C.lib().bevb200_bev_pool_grad_perm_dev(
+                    B, D, H, W, t.n_total, ctx.c, _C.ptr(out_grad), _C.ptr(t.perm), _C.ptr(t.geom), _C.ptr(t.starts),
+                    _C.ptr(t.lengths), _C.ptr(t.counts), _C.ptr(x_grad), _C.current_stream(out_grad.device))
+                _C.check(rc, "bev_pool_grad_perm_dev")
+                return x_grad, None
             rc = _C.lib().bevb200_bev_pool_grad_perm(
                 B, D, H, W, t.n_kept, t.n_total, ctx.c, t.n_intervals, _C.ptr(out_grad),
                 _C.ptr(t.perm), _C.ptr(t.geom), _C.ptr(t.starts), _C.ptr(t.lengths),
@@ -297,14 +350,114 @@ class BEVPoolPlan:
 
     @classmethod
     def from_cameras(cls, frustum, camera2lidar_rots, camera2lidar_trans, intrins, post_rots, post_trans,
-                     xbound, ybound, zbound, extra_rots=None, extra_trans=None):
+                     xbound, ybound, zbound, extra_rots=None, extra_trans=None, sync=True, max_segments=None):
         """Plan straight from the calibration: get_geometry (base.py:92-135) runs inside the plan build, the
-        96 MB geometry tensor is never written (what a per-sample camera2lidar needs every frame)."""
+        96 MB geometry tensor is never written (what a per-sample camera2lidar needs every frame).
+
+        sync=False builds a sync-free plan for calibration that changes every step (training augmentation,
+        per-sample camera2lidar): every table, count and workspace is allocated once, at capacity for
+        (B, N, D, fH, fW); rebuild_() refills them from new calibration without a host round trip, and pool, lift,
+        lift_pool and their backward read the point, interval and segment counts from the device.  A step of
+        rebuild_ -> lift_pool -> backward can then be captured in a CUDA graph.  max_segments caps the column
+        tables of the fused lift (default: _SEGMENTS_PER_COLUMN_BIN per (camera, image column, depth bin)); a
+        calibration with more segments runs the row kernels instead, chosen on the device (tables.lift_form)."""
         self = cls.__new__(cls)
         self.dx, self.bx, self.nx = gen_dx_bx(xbound, ybound, zbound)
         self.B = int(camera2lidar_trans.shape[0])
+        if not sync:
+            self._init_sync_free(frustum, int(camera2lidar_trans.shape[1]), max_segments)
+            self.rebuild_(camera2lidar_rots, camera2lidar_trans, intrins, post_rots, post_trans, extra_rots, extra_trans)
+            return self
         self.tables = prepare_from_cameras(frustum, camera2lidar_rots, camera2lidar_trans, intrins, post_rots,
                                            post_trans, self.dx, self.bx, self.nx, extra_rots, extra_trans)
+        return self
+
+    def _init_sync_free(self, frustum, N, max_segments):
+        _C.require_cuda(frustum, "frustum", torch.float32)
+        if frustum.dim() != 4 or frustum.shape[3] != 3:
+            raise ValueError("frustum must be [D, fH, fW, 3], got %s" % (tuple(frustum.shape),))
+        D, fH, fW = (int(v) for v in frustum.shape[:3])
+        B, dev = self.B, frustum.device
+        self._frustum = frustum.reshape(-1, 3).contiguous()
+        n_total = self._frustum.shape[0] * B * N
+        self._grid = _grid_host(self.dx, self.bx, self.nx, B)
+        self._cams = (B, N, D, fH, fW)
+        L = _C.lib()
+        i32 = dict(dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            counts = torch.zeros(4, **i32)
+            self.tables = _PoolTables(torch.empty(n_total, **i32), torch.empty(n_total, **i32),
+                                      torch.empty((n_total, 4), **i32), torch.empty(n_total, **i32),
+                                      torch.empty(n_total, **i32), counts[0], counts[1], n_total, self._grid[3],
+                                      counts=counts)
+            self._prepare_ws = _ws(L.bevb200_bev_pool_prepare_workspace_bytes(n_total), dev)
+            self._columns = fH <= 64
+            if not self._columns:
+                # the segment mask holds 64 pixel rows: taller features always run the row kernels
+                counts[3] = _LIFT_ROWS
+                self.max_segments = 0
+                return
+            if max_segments is None:
+                max_segments = _SEGMENTS_PER_COLUMN_BIN * B * N * fW * D
+            self.max_segments = min(int(max_segments), n_total)
+            if self.max_segments <= 0:
+                raise ValueError("max_segments must be positive, got %d" % self.max_segments)
+            cap = self.max_segments
+            self._seg = dict(col_begin=torch.empty(B * N * fW + 1, **i32),
+                             seg_key=torch.empty(cap, dtype=torch.int64, device=dev),
+                             seg_mask=torch.empty(cap, dtype=torch.int64, device=dev),
+                             seg_slot=torch.empty(cap, **i32), ival_begin=torch.empty(n_total + 1, **i32),
+                             ws=_ws(L.bevb200_bev_pool_lift_prepare_dev_workspace_bytes(n_total, cap), dev))
+
+    def rebuild_(self, camera2lidar_rots, camera2lidar_trans, intrins, post_rots, post_trans, extra_rots=None,
+                 extra_trans=None):
+        """Refill a sync-free plan's tables (and the fused lift's column tables) from new calibration, in place and
+        without synchronising the host: [B, N, 3, 3] / [B, N, 3] fp32 tensors on the plan's device as for
+        from_cameras, extra_* [B, 3, 3] / [B, 3] or None.  Raises ValueError, before any launch and with the tables
+        untouched, on a wrong shape, dtype or device."""
+        if getattr(self, "_cams", None) is None:
+            raise ValueError("rebuild_ needs a plan built with BEVPoolPlan.from_cameras(..., sync=False)")
+        B, N, D, fH, fW = self._cams
+        t = self.tables
+        dev = t.perm.device
+        args = [("camera2lidar_rots", camera2lidar_rots, (B, N, 3, 3)),
+                ("camera2lidar_trans", camera2lidar_trans, (B, N, 3)), ("intrins", intrins, (B, N, 3, 3)),
+                ("post_rots", post_rots, (B, N, 3, 3)), ("post_trans", post_trans, (B, N, 3)),
+                ("extra_rots", extra_rots, (B, 3, 3)), ("extra_trans", extra_trans, (B, 3))]
+        for name, v, shape in args:
+            if v is None and name.startswith("extra"):
+                continue
+            if not isinstance(v, torch.Tensor):
+                raise ValueError("%s must be a tensor" % name)
+            if tuple(v.shape) != shape:
+                raise ValueError("%s has shape %s, the plan needs %s" % (name, tuple(v.shape), shape))
+            if v.dtype != torch.float32:
+                raise ValueError("%s must be float32, got %s" % (name, v.dtype))
+            if v.device != dev:
+                raise ValueError("%s is on %s, the plan on %s" % (name, v.device, dev))
+        # torch.linalg.inv_ex runs the factorisation of torch.inverse without reading its error flag back to the
+        # host: the same inverses, bit for bit, and capturable in a CUDA graph
+        cam, extra = _camera_params(dev, B, N, camera2lidar_rots, camera2lidar_trans, intrins, post_rots, post_trans,
+                                    extra_rots, extra_trans, lambda m: torch.linalg.inv_ex(m)[0])
+        lower_h, dx_h, nx_h, _ = self._grid
+        fr = self._frustum
+        L = _C.lib()
+        with torch.cuda.device(dev):
+            stream = _C.current_stream(dev)
+            rc = L.bevb200_bev_pool_prepare_cameras(
+                _C.ptr(fr), fr.shape[0], B * N, N, _C.ptr(cam), _C.ptr(extra), ctypes.cast(lower_h, ctypes.c_void_p),
+                ctypes.cast(dx_h, ctypes.c_void_p), ctypes.cast(nx_h, ctypes.c_void_p), B, None, _C.ptr(t.ranks),
+                _C.ptr(t.perm), _C.ptr(t.geom), _C.ptr(t.starts), _C.ptr(t.lengths), _C.ptr(t.counts),
+                _C.ptr(self._prepare_ws), self._prepare_ws.numel(), stream)
+            _C.check(rc, "bev_pool_prepare_cameras")
+            if self._columns:
+                sg = self._seg
+                rc = L.bevb200_bev_pool_lift_prepare_dev(
+                    _C.ptr(t.perm), _C.ptr(t.starts), _C.ptr(t.counts), t.n_total, self.max_segments, B * N, D, fH, fW,
+                    _C.ptr(sg["col_begin"]), _C.ptr(sg["seg_key"]), _C.ptr(sg["seg_mask"]), _C.ptr(sg["seg_slot"]),
+                    _C.ptr(sg["ival_begin"]), t.counts_ptr(2), t.counts_ptr(3), _C.ptr(sg["ws"]), sg["ws"].numel(),
+                    stream)
+                _C.check(rc, "bev_pool_lift_prepare_dev")
         return self
 
     def pool(self, x):
@@ -370,6 +523,8 @@ class BEVPoolPlan:
         t = self.tables
         assert depth.numel() == t.n_total
         Bq, Dq, Hq, Wq = t.dims
+        if t.counts is not None:
+            return self._lift_pool_forward_dev(depth, ctx)
         if fH <= 64 and os.environ.get("BEVB200_LIFT_VARIANT", "columns") != "rows":
             # column formulation: context rows and depth values of an image column are staged once in shared
             # memory and every (column, depth bin, cell) segment is evaluated from there
@@ -395,6 +550,38 @@ class BEVPoolPlan:
         _C.check(rc, "bev_pool_lift")
         return out
 
+    def _lift_pool_forward_dev(self, depth, ctx):
+        """sync-free plan: the column and the row form are both launched and the status word of the column-table
+        prepare (tables.lift_form) lets exactly one of them write `out`"""
+        B, N, D, fH, fW = self._cams
+        if tuple(depth.shape) != (B, N, D, fH, fW):
+            raise ValueError("depth has shape %s, the plan needs %s" % (tuple(depth.shape), self._cams))
+        c = ctx.shape[-1]
+        t = self.tables
+        Bq, Dq, Hq, Wq = t.dims
+        dev = depth.device
+        L = _C.lib()
+        with torch.cuda.device(dev):
+            stream = _C.current_stream(dev)
+            out = torch.empty((Bq, Dq, Hq, Wq, c), dtype=torch.float32, device=dev)
+            if self._columns:
+                sg = self._seg
+                ws = t.workspace(("columns", c), L.bevb200_bev_pool_lift_columns_dev_workspace_bytes(
+                    self.max_segments, t.n_total, c), dev)
+                rc = L.bevb200_bev_pool_lift_columns_dev(
+                    Bq, Dq, Hq, Wq, t.n_total, c, _C.ptr(depth), _C.ptr(ctx), B * N, D, fH, fW, _C.ptr(t.geom),
+                    _C.ptr(t.starts), _C.ptr(sg["col_begin"]), _C.ptr(sg["seg_key"]), _C.ptr(sg["seg_mask"]),
+                    _C.ptr(sg["seg_slot"]), _C.ptr(sg["ival_begin"]), self.max_segments, _C.ptr(t.counts),
+                    t.counts_ptr(3), _C.ptr(out), _C.ptr(ws), ws.numel(), stream)
+                _C.check(rc, "bev_pool_lift_columns_dev")
+            ws = t.workspace(("pool", c), L.bevb200_bev_pool_dev_workspace_bytes(t.n_total, c), dev)
+            rc = L.bevb200_bev_pool_lift_dev(
+                Bq, Dq, Hq, Wq, t.n_total, c, _C.ptr(depth), _C.ptr(ctx), D, fH * fW, _C.ptr(t.perm), _C.ptr(t.geom),
+                _C.ptr(t.starts), _C.ptr(t.lengths), _C.ptr(t.counts), t.counts_ptr(3), _C.ptr(out), _C.ptr(ws),
+                ws.numel(), stream)
+            _C.check(rc, "bev_pool_lift_dev")
+        return out
+
     def _lift_pool_backward(self, out_grad, depth, ctx, want_depth, want_ctx):
         """(ddepth, dctx) of lift_pool from the gradient of its output; a gradient not wanted is None.
         The column kernel runs wherever the column formulation can (fH <= 64), the pixel kernel otherwise."""
@@ -409,7 +596,28 @@ class BEVPoolPlan:
         with torch.cuda.device(dev):
             ddepth = torch.empty_like(depth) if want_depth else None
             dctx = torch.empty_like(ctx) if want_ctx else None
-            if fH <= 64:
+            if t.counts is not None:
+                # sync-free plan: both backwards are launched, the status word picks the one that writes
+                stream = _C.current_stream(dev)
+                nbytes = L.bevb200_bev_pool_lift_backward_dev_workspace_bytes(t.n_total, c)
+                if self._columns:
+                    nbytes = max(nbytes, L.bevb200_bev_pool_lift_columns_backward_dev_workspace_bytes(
+                        self.max_segments, c))
+                ws = t.workspace("backward", nbytes, dev)
+                if self._columns:
+                    sg = self._seg
+                    rc = L.bevb200_bev_pool_lift_columns_backward_dev(
+                        Bq, Dq, Hq, Wq, t.n_total, c, _C.ptr(out_grad), _C.ptr(depth), _C.ptr(ctx), B * N, D, fH, fW,
+                        _C.ptr(t.geom), _C.ptr(t.starts), _C.ptr(sg["col_begin"]), _C.ptr(sg["seg_key"]),
+                        _C.ptr(sg["seg_mask"]), self.max_segments, _C.ptr(t.counts), t.counts_ptr(2), t.counts_ptr(3),
+                        _C.ptr(ddepth), _C.ptr(dctx), _C.ptr(ws), ws.numel(), stream)
+                    _C.check(rc, "bev_pool_lift_columns_backward_dev")
+                rc = L.bevb200_bev_pool_lift_backward_dev(
+                    Bq, Dq, Hq, Wq, t.n_total, c, _C.ptr(out_grad), _C.ptr(depth), _C.ptr(ctx), D, fH * fW,
+                    _C.ptr(t.perm), _C.ptr(t.geom), _C.ptr(t.starts), _C.ptr(t.lengths), _C.ptr(t.counts),
+                    t.counts_ptr(3), _C.ptr(ddepth), _C.ptr(dctx), _C.ptr(ws), ws.numel(), stream)
+                _C.check(rc, "bev_pool_lift_backward_dev")
+            elif fH <= 64:
                 col_begin, seg_key, seg_mask, _, _, n_seg = self._lift_tables(B * N, D, fH, fW)
                 ws = _ws(L.bevb200_bev_pool_lift_columns_backward_workspace_bytes(n_seg, t.n_intervals, c), dev)
                 rc = L.bevb200_bev_pool_lift_columns_backward(

@@ -53,6 +53,12 @@ __device__ __forceinline__ int find_interval(const int32_t *__restrict__ starts,
 constexpr int kStageRows = 32;
 constexpr int kPoolStages = 3;
 
+// rows of the sorted stream per warp range when [0, n) is cut into at most `ranges_max` ranges (whole stages)
+__host__ __device__ __forceinline__ int tma_rows_per_warp(int n, int ranges_max) {
+  const int rpw = (int)(((long long)n + ranges_max - 1) / ranges_max);
+  return (rpw + kStageRows - 1) / kStageRows * kStageRows;
+}
+
 __device__ __forceinline__ uint32_t pool_smem_u32(const void *p) {
   return (uint32_t)__cvta_generic_to_shared(p);
 }
@@ -69,9 +75,36 @@ __device__ __forceinline__ void pool_mbar_wait(uint32_t bar, uint32_t parity) {
 
 __global__ void pool_interval_cells_kernel(const int32_t *__restrict__ geom_feats,
                                            const int32_t *__restrict__ starts, int n, int n_intervals,
-                                           PoolDims dm, int32_t *__restrict__ cells) {
+                                           PoolDims dm, int32_t *__restrict__ cells,
+                                           const int32_t *__restrict__ counts) {
+  device_counts(counts, n, n_intervals);
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_intervals; i += gridDim.x * blockDim.x)
     cells[i] = interval_cell(geom_feats, starts[i], n, dm);
+}
+
+__global__ void zero_fill_kernel(float *__restrict__ out, size_t n_floats, const int32_t *__restrict__ lift_form,
+                                 int32_t form, const int32_t *__restrict__ only_if_empty) {
+  if (form_off(lift_form, form)) return;
+  if (only_if_empty && __ldg(only_if_empty) > 0 && __ldg(only_if_empty + 1) > 0) return;
+  const size_t stride = (size_t)gridDim.x * blockDim.x, t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if ((uintptr_t)out % 16 == 0) {
+    float4 *o4 = reinterpret_cast<float4 *>(out);
+    for (size_t i = t; i < n_floats / 4; i += stride) o4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (size_t i = n_floats / 4 * 4 + t; i < n_floats; i += stride) out[i] = 0.f;
+  } else {
+    for (size_t i = t; i < n_floats; i += stride) out[i] = 0.f;
+  }
+}
+
+int zero_fill(float *out, size_t n_floats, const int32_t *lift_form, int32_t form, cudaStream_t st,
+              const int32_t *only_if_empty) {
+  if (lift_form == nullptr && only_if_empty == nullptr) {
+    BEVB200_CUDA(cudaMemsetAsync(out, 0, n_floats * sizeof(float), st));
+    return BEVB200_OK;
+  }
+  BEVB200_LAUNCH(zero_fill_kernel, grid_for((long long)(n_floats / 4 + 1), 256, kNumSMs * 8), 256, 0, st, out,
+                 n_floats, lift_form, form, only_if_empty);
+  return BEVB200_OK;
 }
 
 // MODE 0: rows already sorted (one TMA bulk copy per stage); MODE 1: rows gathered through perm;
@@ -87,7 +120,8 @@ __global__ void __launch_bounds__(256)
                            const int32_t *__restrict__ starts, const int32_t *__restrict__ cells,
                            int n, int n_intervals, int rows_per_warp, int zfill, int total_cells,
                            float4 *__restrict__ out, float4 *__restrict__ partial,
-                           const int32_t *__restrict__ lengths /* MODE 0 only */) {
+                           const int32_t *__restrict__ lengths /* MODE 0 only */,
+                           const int32_t *__restrict__ counts, int ranges_max, const int32_t *__restrict__ lift_form) {
   constexpr int QPL = (Q + 31) / 32;              // float4 columns per lane
   constexpr uint32_t kRowBytes = Q * 16;
   constexpr bool PERM = MODE == 1 || MODE == 2;   // cp.async gather with commit groups
@@ -95,6 +129,18 @@ __global__ void __launch_bounds__(256)
   extern __shared__ __align__(128) uint8_t pool_smem[];
   __shared__ uint64_t bars[8 * kPoolStages];
   const int warp = threadIdx.x >> 5, lane = lane_id(), nwarps = blockDim.x >> 5;
+  if (form_off(lift_form, BEVB200_LIFT_ROWS)) return;
+  if (counts) {   // sync-free tables: the grid covers ranges_max ranges; cut [0, n) exactly as the host-count call does
+    device_counts(counts, n, n_intervals);
+    if (n == 0 || n_intervals == 0) {              // nothing to pool: with zfill the grid is zeroed here
+      if (zfill)
+        for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < (long long)total_cells * Q;
+             e += (long long)gridDim.x * blockDim.x)
+          out[e] = make_float4(0.f, 0.f, 0.f, 0.f);
+      return;
+    }
+    rows_per_warp = tma_rows_per_warp(n, ranges_max);
+  }
   const int j = blockIdx.x * nwarps + warp;       // warp-range index
   const long long R0l = (long long)j * rows_per_warp;
   if (R0l >= n) return;
@@ -323,8 +369,17 @@ __global__ void bevpool_fwd_tma_fixup_kernel(const int32_t *__restrict__ starts,
                                              int n_intervals, int rows_per_warp, int n_ranges,
                                              float4 *__restrict__ out,
                                              const float4 *__restrict__ partial,
-                                             const int32_t *__restrict__ lengths /* MODE 0 only */) {
+                                             const int32_t *__restrict__ lengths /* MODE 0 only */,
+                                             const int32_t *__restrict__ counts, int ranges_max,
+                                             const int32_t *__restrict__ lift_form) {
   const int lane = lane_id();
+  if (form_off(lift_form, BEVB200_LIFT_ROWS)) return;
+  if (counts) {
+    device_counts(counts, n, n_intervals);
+    if (n == 0 || n_intervals == 0) return;
+    rows_per_warp = tma_rows_per_warp(n, ranges_max);
+    n_ranges = (n + rows_per_warp - 1) / rows_per_warp;
+  }
   const int wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
   for (int j = wid; j < n_ranges; j += nw) {
     const long long R0 = (long long)j * rows_per_warp, R1 = min((long long)n, R0 + rows_per_warp);
@@ -380,7 +435,9 @@ __global__ void bevpool_fwd_generic_kernel(const float *__restrict__ x,
                                            const int32_t *__restrict__ geom_feats,
                                            const int32_t *__restrict__ starts,
                                            const int32_t *__restrict__ lengths, int n, int c,
-                                           int n_intervals, PoolDims dm, float *__restrict__ out) {
+                                           int n_intervals, PoolDims dm, float *__restrict__ out,
+                                           const int32_t *__restrict__ counts) {
+  device_counts(counts, n, n_intervals);
   long long total = (long long)n_intervals * c;
   for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
        idx += (long long)gridDim.x * blockDim.x) {
@@ -418,8 +475,9 @@ __global__ void __launch_bounds__(kPoolWarps * 32)
                        const int32_t *__restrict__ geom_feats,
                        const int32_t *__restrict__ starts, const int32_t *__restrict__ lengths,
                        int n, int n_total, int n_intervals, PoolDims dm,
-                       float4 *__restrict__ x_grad) {
+                       float4 *__restrict__ x_grad, const int32_t *__restrict__ counts) {
   constexpr int T = PoolCfg<Q, G>::T;
+  device_counts(counts, n, n_intervals);   // n == 0 or no interval: every row is a gap and gets zeros
   const int lane = lane_id();
   int rig[T], qq[T];
 #pragma unroll
@@ -490,7 +548,8 @@ __global__ void bevpool_bwd_generic_kernel(const float *__restrict__ out_grad,
                                            const int32_t *__restrict__ starts,
                                            const int32_t *__restrict__ lengths, int n, int c,
                                            int n_intervals, PoolDims dm,
-                                           float *__restrict__ x_grad) {
+                                           float *__restrict__ x_grad, const int32_t *__restrict__ counts) {
+  device_counts(counts, n, n_intervals);
   long long total = (long long)n_intervals * c;
   for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
        idx += (long long)gridDim.x * blockDim.x) {
@@ -535,20 +594,22 @@ template <int Q>
 static int launch_fwd_tma(const float *x, const int32_t *perm, const int32_t *geom,
                           const int32_t *starts, const int32_t *lengths, int n, int n_intervals,
                           PoolDims dm, float *out, const PoolTmaWs &ws, int zfill, cudaStream_t st,
-                          const float *depth = nullptr, LiftDims lift = LiftDims{1, 1}) {
-  // MODE 1 / 2 tables tile [0, n): their interval ends are the next starts
+                          const float *depth = nullptr, LiftDims lift = LiftDims{1, 1},
+                          const int32_t *counts = nullptr, const int32_t *lift_form = nullptr) {
+  // MODE 1 / 2 tables tile [0, n): their interval ends are the next starts.  With `counts`, n and n_intervals are
+  // capacities: the grids cover them and the kernels read the true sizes from the device.
   const int32_t *mode0_lengths = (depth == nullptr && perm == nullptr) ? lengths : nullptr;
   BEVB200_LAUNCH(pool_interval_cells_kernel, grid_for(n_intervals, 256), 256, 0, st, geom, starts, n,
-                 n_intervals, dm, ws.cells);
+                 n_intervals, dm, ws.cells, counts);
   const size_t stage_bytes = (size_t)kStageRows * Q * 16 + (depth ? 128 : 0);
   int warps = (int)((200 * 1024) / (kPoolStages * stage_bytes));
   if (warps > 8) warps = 8;
   if (warps < 1) warps = 1;
   const size_t smem = (size_t)warps * kPoolStages * stage_bytes;
   const int n_ranges_max = kNumSMs * warps;
-  int rpw = (int)(((long long)n + n_ranges_max - 1) / n_ranges_max);
-  rpw = (rpw + kStageRows - 1) / kStageRows * kStageRows;
-  const int n_ranges = (n + rpw - 1) / rpw;
+  const int rpw = tma_rows_per_warp(n, n_ranges_max);
+  // the device count may cut [0, n_kept) into any number of ranges up to n_ranges_max
+  const int n_ranges = counts ? n_ranges_max : (n + rpw - 1) / rpw;
   const int grid = (n_ranges + warps - 1) / warps;
   const auto kernel = depth  ? &bevpool_fwd_tma_kernel<Q, 2>
                       : perm ? &bevpool_fwd_tma_kernel<Q, 1>
@@ -556,27 +617,30 @@ static int launch_fwd_tma(const float *x, const int32_t *perm, const int32_t *ge
   BEVB200_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   BEVB200_LAUNCH(kernel, grid, warps * 32, smem, st, (const float4 *)x, perm, depth, lift, starts, ws.cells, n,
                  n_intervals, rpw, zfill, dm.b * dm.d * dm.h * dm.w, (float4 *)out, (float4 *)ws.partial,
-                 mode0_lengths);
+                 mode0_lengths, counts, n_ranges_max, lift_form);
   BEVB200_LAUNCH((bevpool_fwd_tma_fixup_kernel<Q>), (n_ranges * 32 + 255) / 256, 256, 0, st, starts, ws.cells, n,
-                 n_intervals, rpw, n_ranges, (float4 *)out, (const float4 *)ws.partial, mode0_lengths);
+                 n_intervals, rpw, n_ranges, (float4 *)out, (const float4 *)ws.partial, mode0_lengths, counts,
+                 n_ranges_max, lift_form);
   return BEVB200_OK;
 }
 
 template <int Q>
 static int launch_bwd(const float *og, const int32_t *perm, const int32_t *geom,
                       const int32_t *starts, const int32_t *lengths, int n, int n_total,
-                      int n_intervals, PoolDims dm, float *xg, cudaStream_t st) {
+                      int n_intervals, PoolDims dm, float *xg, cudaStream_t st, const int32_t *counts) {
   int nchunks = (n_total + kChunkRows - 1) / kChunkRows;
   int grid = min((nchunks + kPoolWarps - 1) / kPoolWarps, kNumSMs * 4);
   BEVB200_LAUNCH((bevpool_bwd_kernel<Q, bwd_rows_per_step(Q)>), grid, kPoolWarps * 32, 0, st, (const float4 *)og,
-                 perm, geom, starts, lengths, n, n_total, n_intervals, dm, (float4 *)xg);
+                 perm, geom, starts, lengths, n, n_total, n_intervals, dm, (float4 *)xg, counts);
   return BEVB200_OK;
 }
 
+// With `counts` (sync-free tables) n and n_intervals are the capacities the tables were sized for, and the kernels read
+// the true sizes from counts = {n_kept, n_intervals} in device memory.
 static int pool_forward(int b, int d, int h, int w, int n, int c, int n_intervals, const float *x,
                         const int32_t *perm, const int32_t *geom, const int32_t *starts,
                         const int32_t *lengths, float *out, void *ws, size_t ws_bytes,
-                        void *stream, bool trust_tables) {
+                        void *stream, bool trust_tables, const int32_t *counts = nullptr) {
   BEVB200_REQUIRE(b > 0 && d > 0 && h > 0 && w > 0 && c > 0, "bad output shape");
   BEVB200_REQUIRE(n >= 0 && n_intervals >= 0, "negative size");
   BEVB200_REQUIRE(out != nullptr, "null out");
@@ -596,23 +660,26 @@ static int pool_forward(int b, int d, int h, int w, int n, int c, int n_interval
   }
   // plan tables (perm != null) with B*D == 1 are in ascending cell order: the pooling kernel
   // zero-fills the empty cells itself; every other case pre-zeroes the grid
+  // (with device counts the kernel zeroes the grid itself when there turns out to be no work)
   const int zfill = (perm != nullptr && b * d == 1 && work && tma && trust_tables) ? 1 : 0;
   if (!zfill) BEVB200_CUDA(cudaMemsetAsync(out, 0, out_bytes, st));
   if (!work) return BEVB200_OK;
   PoolDims dm{b, d, h, w};
   if (!tma) {
     BEVB200_LAUNCH(bevpool_fwd_generic_kernel, grid_for((long long)n_intervals * c, 256), 256, 0, st, x, perm, geom,
-                   starts, lengths, n, c, n_intervals, dm, out);
+                   starts, lengths, n, c, n_intervals, dm, out, counts);
     return BEVB200_OK;
   }
   return TunedWidths::dispatch(c, [&](auto q) {
-    return launch_fwd_tma<decltype(q)::value>(x, perm, geom, starts, lengths, n, n_intervals, dm, out, tws, zfill, st);
+    return launch_fwd_tma<decltype(q)::value>(x, perm, geom, starts, lengths, n, n_intervals, dm, out, tws, zfill, st,
+                                              nullptr, LiftDims{1, 1}, counts);
   });
 }
 
 static int pool_backward(int b, int d, int h, int w, int n, int n_total, int c, int n_intervals,
                          const float *og, const int32_t *perm, const int32_t *geom,
-                         const int32_t *starts, const int32_t *lengths, float *xg, void *stream) {
+                         const int32_t *starts, const int32_t *lengths, float *xg, void *stream,
+                         const int32_t *counts = nullptr) {
   BEVB200_REQUIRE(b > 0 && d > 0 && h > 0 && w > 0 && c > 0, "bad grid shape");
   BEVB200_REQUIRE(n >= 0 && n_total >= n && n_intervals >= 0, "bad sizes");
   if (n_total == 0) return BEVB200_OK;
@@ -627,11 +694,11 @@ static int pool_backward(int b, int d, int h, int w, int n, int n_total, int c, 
   if (!TunedWidths::has(c) || (uintptr_t)og % 16 != 0 || (uintptr_t)xg % 16 != 0) {
     BEVB200_CUDA(cudaMemsetAsync(xg, 0, (size_t)n_total * c * sizeof(float), st));
     BEVB200_LAUNCH(bevpool_bwd_generic_kernel, grid_for((long long)n_intervals * c, 256), 256, 0, st, og, perm, geom,
-                   starts, lengths, n, c, n_intervals, dm, xg);
+                   starts, lengths, n, c, n_intervals, dm, xg, counts);
     return BEVB200_OK;
   }
   return TunedWidths::dispatch(c, [&](auto q) {
-    return launch_bwd<decltype(q)::value>(og, perm, geom, starts, lengths, n, n_total, n_intervals, dm, xg, st);
+    return launch_bwd<decltype(q)::value>(og, perm, geom, starts, lengths, n, n_total, n_intervals, dm, xg, st, counts);
   });
 }
 
@@ -844,6 +911,42 @@ static int prepare_tables(const void *points, int n, int B, int D, int H, int W,
   return BEVB200_OK;
 }
 
+// the row form of the fused lift; with `counts` n / n_intervals are capacities (see pool_forward), with `lift_form`
+// the call does nothing unless *lift_form == BEVB200_LIFT_ROWS
+static int lift_rows_forward(int b, int d, int h, int w, int n, int c, int n_intervals, const float *depth,
+                             const float *ctx, int depth_bins, int pixels_per_camera, const int32_t *perm,
+                             const int32_t *geom_feats, const int32_t *interval_starts,
+                             const int32_t *interval_lengths, float *out, void *workspace,
+                             size_t workspace_bytes, void *stream, const int32_t *counts, const int32_t *lift_form) {
+  (void)interval_lengths;
+  BEVB200_REQUIRE(b > 0 && d > 0 && h > 0 && w > 0 && c > 0 && n >= 0 && n_intervals >= 0, "bad sizes");
+  BEVB200_REQUIRE(out != nullptr, "null out");
+  BEVB200_REQUIRE(depth_bins > 0 && pixels_per_camera > 0, "bad lift dims");
+  BEVB200_REQUIRE((long long)b * d * h * w < (1ll << 31), "grid has too many cells");
+  const bool work = n > 0 && n_intervals > 0;
+  // every argument is checked before `out` is written: a refused call leaves it untouched
+  PoolTmaWs ws;
+  if (work) {
+    BEVB200_REQUIRE(depth && ctx && perm && geom_feats && interval_starts, "null input");
+    BEVB200_REQUIRE(((uintptr_t)ctx % 16 == 0) && ((uintptr_t)out % 16 == 0), "ctx / out must be 16-byte aligned");
+    if (const int rc = workspace_check("bev_pool_lift", workspace, workspace_bytes, pool_tma_layout(n, c, workspace, &ws)))
+      return rc;
+    BEVB200_REQUIRE(TunedWidths::has(c), "no tuned kernel for this channel count");
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  // the tables tile [0, n) in ascending cell order: at B*D == 1 the kernel zero-fills the empty cells itself
+  const int zfill = (b * d == 1 && work) ? 1 : 0;
+  if (!zfill)
+    if (const int rc = zero_fill(out, (size_t)b * d * h * w * c, lift_form, BEVB200_LIFT_ROWS, st)) return rc;
+  if (!work) return BEVB200_OK;
+  PoolDims dm{b, d, h, w};
+  LiftDims lift{depth_bins, pixels_per_camera};
+  return TunedWidths::dispatch(c, [&](auto q) {
+    return launch_fwd_tma<decltype(q)::value>(ctx, perm, geom_feats, interval_starts, nullptr, n, n_intervals, dm, out,
+                                              ws, zfill, st, depth, lift, counts, lift_form);
+  });
+}
+
 }  // namespace bevb200
 
 using namespace bevb200;
@@ -894,32 +997,46 @@ int bevb200_bev_pool_lift(int b, int d, int h, int w, int n, int c, int n_interv
                           const int32_t *geom_feats, const int32_t *interval_starts,
                           const int32_t *interval_lengths, float *out, void *workspace,
                           size_t workspace_bytes, void *stream) {
-  (void)interval_lengths;
-  BEVB200_REQUIRE(b > 0 && d > 0 && h > 0 && w > 0 && c > 0 && n >= 0 && n_intervals >= 0, "bad sizes");
-  BEVB200_REQUIRE(out != nullptr, "null out");
-  BEVB200_REQUIRE(depth_bins > 0 && pixels_per_camera > 0, "bad lift dims");
-  BEVB200_REQUIRE((long long)b * d * h * w < (1ll << 31), "grid has too many cells");
-  const bool work = n > 0 && n_intervals > 0;
-  // every argument is checked before `out` is written: a refused call leaves it untouched
-  PoolTmaWs ws;
-  if (work) {
-    BEVB200_REQUIRE(depth && ctx && perm && geom_feats && interval_starts, "null input");
-    BEVB200_REQUIRE(((uintptr_t)ctx % 16 == 0) && ((uintptr_t)out % 16 == 0), "ctx / out must be 16-byte aligned");
-    if (const int rc = workspace_check("bev_pool_lift", workspace, workspace_bytes, pool_tma_layout(n, c, workspace, &ws)))
-      return rc;
-    BEVB200_REQUIRE(TunedWidths::has(c), "no tuned kernel for this channel count");
-  }
-  cudaStream_t st = (cudaStream_t)stream;
-  // the tables tile [0, n) in ascending cell order: at B*D == 1 the kernel zero-fills the empty cells itself
-  const int zfill = (b * d == 1 && work) ? 1 : 0;
-  if (!zfill) BEVB200_CUDA(cudaMemsetAsync(out, 0, (size_t)b * d * h * w * c * sizeof(float), st));
-  if (!work) return BEVB200_OK;
-  PoolDims dm{b, d, h, w};
-  LiftDims lift{depth_bins, pixels_per_camera};
-  return TunedWidths::dispatch(c, [&](auto q) {
-    return launch_fwd_tma<decltype(q)::value>(ctx, perm, geom_feats, interval_starts, nullptr, n, n_intervals, dm, out,
-                                              ws, zfill, st, depth, lift);
-  });
+  return lift_rows_forward(b, d, h, w, n, c, n_intervals, depth, ctx, depth_bins, pixels_per_camera, perm, geom_feats,
+                           interval_starts, interval_lengths, out, workspace, workspace_bytes, stream, nullptr, nullptr);
+}
+
+
+size_t bevb200_bev_pool_dev_workspace_bytes(int n_capacity, int c) {
+  if (n_capacity <= 0 || c <= 0) return 0;
+  return pool_tma_layout(n_capacity, c, nullptr, nullptr);
+}
+
+int bevb200_bev_pool_perm_dev(int b, int d, int h, int w, int n_capacity, int c, const float *x, const int32_t *perm,
+                              const int32_t *geom_feats, const int32_t *interval_starts,
+                              const int32_t *interval_lengths, const int32_t *counts_dev, float *out, void *workspace,
+                              size_t workspace_bytes, void *stream) {
+  BEVB200_REQUIRE(n_capacity > 0, "capacity must be positive");
+  BEVB200_REQUIRE(perm && counts_dev, "null perm / counts");
+  return pool_forward(b, d, h, w, n_capacity, c, n_capacity, x, perm, geom_feats, interval_starts, interval_lengths,
+                      out, workspace, workspace_bytes, stream, true, counts_dev);
+}
+
+int bevb200_bev_pool_grad_perm_dev(int b, int d, int h, int w, int n_total, int c, const float *out_grad,
+                                   const int32_t *perm, const int32_t *geom_feats, const int32_t *interval_starts,
+                                   const int32_t *interval_lengths, const int32_t *counts_dev, float *x_grad,
+                                   void *stream) {
+  BEVB200_REQUIRE(n_total > 0, "capacity must be positive");
+  BEVB200_REQUIRE(perm && counts_dev, "null perm / counts");
+  return pool_backward(b, d, h, w, n_total, n_total, c, n_total, out_grad, perm, geom_feats, interval_starts,
+                       interval_lengths, x_grad, stream, counts_dev);
+}
+
+int bevb200_bev_pool_lift_dev(int b, int d, int h, int w, int n_capacity, int c, const float *depth, const float *ctx,
+                              int depth_bins, int pixels_per_camera, const int32_t *perm, const int32_t *geom_feats,
+                              const int32_t *interval_starts, const int32_t *interval_lengths,
+                              const int32_t *counts_dev, const int32_t *lift_form, float *out, void *workspace,
+                              size_t workspace_bytes, void *stream) {
+  BEVB200_REQUIRE(n_capacity > 0, "capacity must be positive");
+  BEVB200_REQUIRE(counts_dev != nullptr, "null counts");
+  return lift_rows_forward(b, d, h, w, n_capacity, c, n_capacity, depth, ctx, depth_bins, pixels_per_camera, perm,
+                           geom_feats, interval_starts, interval_lengths, out, workspace, workspace_bytes, stream,
+                           counts_dev, lift_form);
 }
 
 int bevb200_bev_channels_first(const float *in, float *out, int batch, int nz, int rows, int c,

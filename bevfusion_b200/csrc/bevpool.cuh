@@ -30,10 +30,30 @@ __device__ __forceinline__ int32_t interval_cell(const int32_t *__restrict__ geo
   return (int32_t)(s >= 0 && s < n ? cell_of(geom_feats, s, dm) : -1);
 }
 
+// Sync-free plans (the *_dev entries): the kernels take a nullable `counts` = {n_kept, n_intervals} in device memory
+// that replaces the host n / n_intervals they were sized for, and the fused-lift kernels a nullable `lift_form`, the
+// status word of bevb200_bev_pool_lift_prepare_dev: a kernel whose form it does not name exits at once, so both forms
+// can be launched and the device picks one.
+__device__ __forceinline__ void device_counts(const int32_t *counts, int &n, int &n_intervals) {
+  if (counts) {
+    n = __ldg(counts);
+    n_intervals = __ldg(counts + 1);
+  }
+}
+__device__ __forceinline__ bool form_off(const int32_t *lift_form, int32_t form) {
+  return lift_form != nullptr && __ldg(lift_form) != form;
+}
+
 // cells[i] = interval_cell(starts[i]) for every interval (defined in bevpool.cu)
 __global__ void pool_interval_cells_kernel(const int32_t *__restrict__ geom_feats,
                                            const int32_t *__restrict__ starts, int n, int n_intervals,
-                                           PoolDims dm, int32_t *__restrict__ cells);
+                                           PoolDims dm, int32_t *__restrict__ cells,
+                                           const int32_t *__restrict__ counts);
+
+// out[0 .. n_floats) = 0 unless `lift_form` names another form or, given `only_if_empty` = device {n_kept,
+// n_intervals}, the tables are not empty (defined in bevpool.cu)
+int zero_fill(float *out, size_t n_floats, const int32_t *lift_form, int32_t form, cudaStream_t st,
+              const int32_t *only_if_empty = nullptr);
 
 // BEVB200_EWORKSPACE, with the error text, when the caller's workspace is smaller than `need` bytes
 inline int workspace_check(const char *who, const void *ws, size_t ws_bytes, size_t need) {

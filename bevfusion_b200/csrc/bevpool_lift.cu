@@ -33,17 +33,26 @@ struct LiftGeom {
 
 // sorted position s -> interval index (intervals tile [0, n_kept)); one thread per interval
 __global__ void lift_interval_ids_kernel(const int32_t *__restrict__ starts, int n_intervals, int n_kept,
-                                         int32_t *__restrict__ ival_of) {
+                                         int32_t *__restrict__ ival_of, const int32_t *__restrict__ counts) {
+  device_counts(counts, n_kept, n_intervals);
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_intervals; i += gridDim.x * blockDim.x) {
     const int s0 = starts[i], s1 = i + 1 < n_intervals ? starts[i + 1] : n_kept;
     for (int s = s0; s < s1; ++s) ival_of[s] = i;
   }
 }
 
-// key = ((column * D + d) << 32) | interval, value = h
+// key = ((column * D + d) << 32) | interval, value = h.  With device counts the keys cover the capacity n_items, and
+// the rows at or past n_kept get the key (ncols * D) << 32, which sorts after every real one.
 __global__ void lift_keys_kernel(const int32_t *__restrict__ perm, const int32_t *__restrict__ ival_of, int n_kept,
-                                 LiftGeom g, unsigned long long *__restrict__ keys, uint32_t *__restrict__ vals) {
-  for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < n_kept; s += gridDim.x * blockDim.x) {
+                                 LiftGeom g, unsigned long long *__restrict__ keys, uint32_t *__restrict__ vals,
+                                 const int32_t *__restrict__ counts, int n_items) {
+  if (counts) n_kept = __ldg(counts); else n_items = n_kept;
+  for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < n_items; s += gridDim.x * blockDim.x) {
+    if (s >= n_kept) {
+      keys[s] = ((unsigned long long)g.ncols * g.depth_bins) << 32;
+      vals[s] = 0u;
+      continue;
+    }
     long long p = perm[s];                         // ((cam * D + d) * fh + h) * fw + w,  cam = b * N + n
     const int w = (int)(p % g.fw); p /= g.fw;
     const int h = (int)(p % g.fh); p /= g.fh;
@@ -55,17 +64,31 @@ __global__ void lift_keys_kernel(const int32_t *__restrict__ perm, const int32_t
   }
 }
 
-__global__ void lift_heads_kernel(const unsigned long long *__restrict__ keys, int n, uint32_t *__restrict__ flags) {
-  for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < n; s += gridDim.x * blockDim.x)
-    flags[s] = (s == 0 || keys[s] != keys[s - 1]) ? 1u : 0u;
+// n_items flags; a run heads a segment only below the device n_kept (when `counts` is given)
+__global__ void lift_heads_kernel(const unsigned long long *__restrict__ keys, int n_items, uint32_t *__restrict__ flags,
+                                  const int32_t *__restrict__ counts) {
+  const int n = counts ? __ldg(counts) : n_items;
+  for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < n_items; s += gridDim.x * blockDim.x)
+    flags[s] = s < n && (s == 0 || keys[s] != keys[s - 1]) ? 1u : 0u;
+}
+
+// sync-free prepare: n_segments = the scan total; lift_form = BEVB200_LIFT_ROWS when it exceeds the cap of the column
+// tables
+__global__ void lift_form_kernel(const uint32_t *__restrict__ total, int max_segments, int32_t *__restrict__ n_segments,
+                                 int32_t *__restrict__ lift_form) {
+  const uint32_t n_seg = *total;
+  *n_segments = (int32_t)n_seg;
+  *lift_form = n_seg > (uint32_t)max_segments ? BEVB200_LIFT_ROWS : BEVB200_LIFT_COLUMNS;
 }
 
 // one thread per sorted element that heads a run: segment record
 __global__ void lift_segments_kernel(const unsigned long long *__restrict__ keys, const uint32_t *__restrict__ hs,
                                      const uint32_t *__restrict__ flags, const uint32_t *__restrict__ pos, int n,
-                                     unsigned long long *__restrict__ seg_key, unsigned long long *__restrict__ seg_mask) {
+                                     unsigned long long *__restrict__ seg_key, unsigned long long *__restrict__ seg_mask,
+                                     const int32_t *__restrict__ counts, uint32_t seg_cap) {
+  if (counts) n = __ldg(counts);
   for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < n; s += gridDim.x * blockDim.x) {
-    if (!flags[s]) continue;
+    if (!flags[s] || pos[s] >= seg_cap) continue;   // past the cap the column tables are not used
     const unsigned long long k = keys[s];
     unsigned long long m = 0;
     for (int e = s; e < n && keys[e] == k; ++e) m |= 1ull << hs[e];
@@ -74,10 +97,13 @@ __global__ void lift_segments_kernel(const unsigned long long *__restrict__ keys
   }
 }
 
-__global__ void lift_seg_ival_kernel(const unsigned long long *__restrict__ seg_key, int n_seg,
-                                     uint32_t *__restrict__ ival, uint32_t *__restrict__ idx) {
-  for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < n_seg; s += gridDim.x * blockDim.x) {
-    ival[s] = (uint32_t)(seg_key[s] & 0xffffffffull);
+// with a device segment count (n_seg_dev) the n_items entries past it get the key `beyond`, which sorts last
+__global__ void lift_seg_ival_kernel(const unsigned long long *__restrict__ seg_key, int n_items,
+                                     uint32_t *__restrict__ ival, uint32_t *__restrict__ idx,
+                                     const int32_t *__restrict__ n_seg_dev, uint32_t beyond) {
+  const int n_seg = n_seg_dev ? min(__ldg(n_seg_dev), n_items) : n_items;
+  for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < n_items; s += gridDim.x * blockDim.x) {
+    ival[s] = s < n_seg ? (uint32_t)(seg_key[s] & 0xffffffffull) : beyond;
     idx[s] = (uint32_t)s;
   }
 }
@@ -86,7 +112,16 @@ __global__ void lift_seg_ival_kernel(const unsigned long long *__restrict__ seg_
 // first segment of every column (segments are in (column, d, interval) order)
 __global__ void lift_slots_kernel(const uint32_t *__restrict__ ival_sorted, const uint32_t *__restrict__ seg_sorted,
                                   int n_seg, int n_intervals, int32_t *__restrict__ slot,
-                                  int32_t *__restrict__ ival_slot_begin) {
+                                  int32_t *__restrict__ ival_slot_begin, const int32_t *__restrict__ counts,
+                                  const int32_t *__restrict__ n_seg_dev, const int32_t *__restrict__ lift_form) {
+  if (form_off(lift_form, BEVB200_LIFT_COLUMNS)) return;
+  if (counts) {
+    n_intervals = __ldg(counts + 1);
+    n_seg = __ldg(n_seg_dev);
+    if (n_seg == 0)   // no kept point: an empty slot table, as the host-count prepare writes it
+      for (int j = blockIdx.x * blockDim.x + threadIdx.x; j <= n_intervals; j += gridDim.x * blockDim.x)
+        ival_slot_begin[j] = 0;
+  }
   for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < n_seg; s += gridDim.x * blockDim.x) {
     slot[seg_sorted[s]] = s;
     const uint32_t i = ival_sorted[s];
@@ -100,7 +135,10 @@ __global__ void lift_slots_kernel(const uint32_t *__restrict__ ival_sorted, cons
 }
 
 __global__ void lift_col_begin_kernel(const unsigned long long *__restrict__ seg_key, int n_seg, LiftGeom g,
-                                      int32_t *__restrict__ col_begin) {
+                                      int32_t *__restrict__ col_begin, const int32_t *__restrict__ n_seg_dev,
+                                      const int32_t *__restrict__ lift_form) {
+  if (form_off(lift_form, BEVB200_LIFT_COLUMNS)) return;
+  if (n_seg_dev) n_seg = __ldg(n_seg_dev);
   for (int c = blockIdx.x * blockDim.x + threadIdx.x; c <= g.ncols; c += gridDim.x * blockDim.x) {
     const unsigned long long want = ((unsigned long long)c * g.depth_bins) << 32;   // first key of column c
     int lo = 0, hi = n_seg;
@@ -120,8 +158,9 @@ __global__ void __launch_bounds__(256)
     lift_columns_kernel(const float *__restrict__ depth, const float4 *__restrict__ ctx, LiftGeom g,
                         const int32_t *__restrict__ col_begin, const unsigned long long *__restrict__ seg_key,
                         const unsigned long long *__restrict__ seg_mask, const int32_t *__restrict__ slot,
-                        float4 *__restrict__ partial) {
+                        float4 *__restrict__ partial, const int32_t *__restrict__ lift_form) {
   extern __shared__ __align__(16) uint8_t lift_smem[];
+  if (form_off(lift_form, BEVB200_LIFT_COLUMNS)) return;
   float4 *ctx_s = reinterpret_cast<float4 *>(lift_smem);                    // [fh][Q]
   float *dep_s = reinterpret_cast<float *>(lift_smem + (size_t)g.fh * Q * 16);   // [D][fh]
   const int col = blockIdx.x, cam = col / g.fw, w = col % g.fw;
@@ -199,13 +238,19 @@ __global__ void __launch_bounds__(256)
 }
 
 // kernel 2: one warp per interval; lane handles float4 columns lane, lane + 32, ...
-template <int Q>
+// DEV: sync-free tables (counts / lift_form); a separate instantiation keeps the host-count one as lean as before
+template <int Q, bool DEV>
 __global__ void __launch_bounds__(256)
     lift_cells_kernel(const float4 *__restrict__ partial, const int32_t *__restrict__ ival_slot_begin,
                       const int32_t *__restrict__ cells, int n_intervals, int zfill, int total_cells,
-                      float4 *__restrict__ out) {
+                      float4 *__restrict__ out, const int32_t *__restrict__ counts,
+                      const int32_t *__restrict__ lift_form) {
   constexpr int QPL = (Q + 31) / 32;
   const int lane = lane_id(), warps = (gridDim.x * blockDim.x) >> 5;
+  if constexpr (DEV) {
+    if (form_off(lift_form, BEVB200_LIFT_COLUMNS)) return;
+    n_intervals = __ldg(counts) > 0 ? __ldg(counts + 1) : 0;   // an empty grid is zeroed by zero_fill
+  }
   for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n_intervals; i += warps) {
     const int b0 = ival_slot_begin[i], b1 = ival_slot_begin[i + 1];
     const int cell = cells[i];
@@ -248,7 +293,13 @@ __global__ void __launch_bounds__(256)
 // cell of every segment (through its interval); -1 would mean "outside the grid" (cannot occur for prepared tables)
 __global__ void lift_seg_cells_kernel(const unsigned long long *__restrict__ seg_key, int n_seg,
                                       const int32_t *__restrict__ geom_feats, const int32_t *__restrict__ starts, int n,
-                                      PoolDims dm, int32_t *__restrict__ seg_cell) {
+                                      PoolDims dm, int32_t *__restrict__ seg_cell, const int32_t *__restrict__ counts,
+                                      const int32_t *__restrict__ n_seg_dev, const int32_t *__restrict__ lift_form) {
+  if (form_off(lift_form, BEVB200_LIFT_COLUMNS)) return;
+  if (counts) {
+    n = __ldg(counts);
+    n_seg = __ldg(n_seg_dev);
+  }
   for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < n_seg; s += gridDim.x * blockDim.x)
     seg_cell[s] = interval_cell(geom_feats, starts[(uint32_t)(seg_key[s] & 0xffffffffull)], n, dm);
 }
@@ -276,9 +327,11 @@ __global__ void __launch_bounds__(256)
                             const float4 *__restrict__ ctx, LiftGeom g, const int32_t *__restrict__ col_begin,
                             const unsigned long long *__restrict__ seg_key,
                             const unsigned long long *__restrict__ seg_mask, const int32_t *__restrict__ seg_cell,
-                            int smax, float *__restrict__ ddepth, float4 *__restrict__ dctx) {
+                            int smax, float *__restrict__ ddepth, float4 *__restrict__ dctx,
+                            const int32_t *__restrict__ lift_form) {
   constexpr int QP = Q + 1;
   extern __shared__ __align__(16) uint8_t lift_bwd_smem_raw[];
+  if (form_off(lift_form, BEVB200_LIFT_COLUMNS)) return;
   float4 *ctx_s = reinterpret_cast<float4 *>(lift_bwd_smem_raw);                  // [fh][QP]
   float4 *acc_s = ctx_s + g.fh * QP;                                               // [fh][Q]
   float4 *g_s = acc_s + g.fh * Q;                                                  // [smax][QP]
@@ -367,8 +420,11 @@ __global__ void __launch_bounds__(256)
 __global__ void lift_point_cells_kernel(const int32_t *__restrict__ perm, const int32_t *__restrict__ geom_feats,
                                         const int32_t *__restrict__ starts, const int32_t *__restrict__ lengths,
                                         int n, int n_total, int n_intervals, PoolDims dm,
-                                        int32_t *__restrict__ point_cell) {
+                                        int32_t *__restrict__ point_cell, const int32_t *__restrict__ counts,
+                                        const int32_t *__restrict__ lift_form) {
   const int lane = lane_id(), warps = (gridDim.x * blockDim.x) >> 5;
+  if (form_off(lift_form, BEVB200_LIFT_ROWS)) return;
+  device_counts(counts, n, n_intervals);
   for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n_intervals; i += warps) {   // warp per interval
     const int s0 = starts[i], len = lengths[i];
     const int32_t c = interval_cell(geom_feats, s0, n, dm);
@@ -384,9 +440,11 @@ template <int Q>
 __global__ void __launch_bounds__(256)
     lift_pixels_bwd_kernel(const float4 *__restrict__ out_grad, const float *__restrict__ depth,
                            const float4 *__restrict__ ctx, const int32_t *__restrict__ point_cell, int n_pixels,
-                           int depth_bins, int ppc, float *__restrict__ ddepth, float4 *__restrict__ dctx) {
+                           int depth_bins, int ppc, float *__restrict__ ddepth, float4 *__restrict__ dctx,
+                           const int32_t *__restrict__ lift_form) {
   constexpr int QPL = (Q + 31) / 32;
   const int lane = lane_id(), warps = (gridDim.x * blockDim.x) >> 5;
+  if (form_off(lift_form, BEVB200_LIFT_ROWS)) return;
   const bool want_dd = ddepth != nullptr, want_dc = dctx != nullptr;
   for (int px = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; px < n_pixels; px += warps) {
     const int cam = px / ppc, pix = px - cam * ppc;
@@ -500,29 +558,30 @@ static size_t lift_bwd_layout(int items, void *ws, int32_t **cells) {
 // the workspace queries of the column forward and both backwards report this much more than the calls require
 constexpr size_t kLiftQuerySlack = 256;
 
-}  // namespace bevb200
+// ---- host side ---------------------------------------------------------------------------------------------------
+// Each host-count entry and its *_dev twin share one body.  A twin passes `counts` = {n_kept, n_intervals} in device
+// memory (the host n_kept / n / n_intervals are then the capacity the tables were sized for), the device segment count
+// `n_seg_dev` and the status word `lift_form`; the host sizes every grid from the capacities and the kernels stop at the
+// device counts.  Every check comes before the first launch.
 
-using namespace bevb200;
-
-extern "C" {
-
-size_t bevb200_bev_pool_lift_prepare_workspace_bytes(int n_kept) {
-  if (n_kept < 0) return 0;
-  return lift_prepare_layout(n_kept, nullptr, 0, nullptr);
-}
-
-int bevb200_bev_pool_lift_prepare(const int32_t *perm, const int32_t *interval_starts, int n_kept, int n_intervals,
-                                  int cameras, int depth_bins, int feature_h, int feature_w, int32_t *col_begin,
-                                  uint64_t *seg_key, uint64_t *seg_mask, int32_t *seg_slot, int32_t *interval_slot_begin,
-                                  int32_t *n_segments, void *workspace, size_t workspace_bytes, void *stream) {
+static int lift_prepare(const int32_t *perm, const int32_t *interval_starts, int n_kept, int n_intervals, int cameras,
+                        int depth_bins, int feature_h, int feature_w, int32_t *col_begin, uint64_t *seg_key,
+                        uint64_t *seg_mask, int32_t *seg_slot, int32_t *interval_slot_begin, int32_t *n_segments,
+                        void *workspace, size_t workspace_bytes, cudaStream_t st, const int32_t *counts,
+                        int max_segments, int32_t *lift_form) {
+  const bool dev = counts != nullptr;
   BEVB200_REQUIRE(n_kept >= 0 && n_intervals >= 0 && cameras > 0 && depth_bins > 0 && feature_h > 0 && feature_w > 0,
                   "bad sizes");
   BEVB200_REQUIRE(feature_h <= 64, "feature height > 64: the per-segment pixel mask is 64 bits");
   BEVB200_REQUIRE((long long)cameras * feature_w * depth_bins < (1ll << 31), "too many (column, depth) pairs");
   BEVB200_REQUIRE(col_begin && seg_key && seg_mask && seg_slot && interval_slot_begin && n_segments, "null output");
-  cudaStream_t st = (cudaStream_t)stream;
+  if (dev) {
+    BEVB200_REQUIRE(n_kept > 0, "capacity must be positive");
+    BEVB200_REQUIRE(max_segments > 0 && max_segments <= n_kept, "max_segments must lie in [1, capacity]");
+    BEVB200_REQUIRE(lift_form != nullptr, "null lift_form");
+  }
   LiftGeom g{depth_bins, feature_h, feature_w, cameras * feature_w};
-  if (n_kept == 0 || n_intervals == 0) {
+  if (!dev && (n_kept == 0 || n_intervals == 0)) {
     BEVB200_CUDA(cudaMemsetAsync(n_segments, 0, sizeof(int32_t), st));
     BEVB200_CUDA(cudaMemsetAsync(col_begin, 0, (size_t)(g.ncols + 1) * sizeof(int32_t), st));
     BEVB200_CUDA(cudaMemsetAsync(interval_slot_begin, 0, (size_t)(n_intervals + 1) * sizeof(int32_t), st));
@@ -534,46 +593,67 @@ int bevb200_bev_pool_lift_prepare(const int32_t *perm, const int32_t *interval_s
                                      lift_prepare_layout(n_kept, workspace, workspace_bytes, &w)))
     return rc;
   BEVB200_LAUNCH(lift_interval_ids_kernel, grid_for(n_intervals, 128), 128, 0, st, interval_starts, n_intervals, n_kept,
-                 w.ival_of);
-  BEVB200_LAUNCH(lift_keys_kernel, grid_for(n_kept, 256), 256, 0, st, perm, w.ival_of, n_kept, g, w.keys_a, w.vals_a);
+                 w.ival_of, counts);
+  BEVB200_LAUNCH(lift_keys_kernel, grid_for(n_kept, 256), 256, 0, st, perm, w.ival_of, n_kept, g, w.keys_a, w.vals_a,
+                 counts, n_kept);
+  // cub takes a host item count: the sync-free prepare sorts all n_kept (capacity) keys, the rows past the device
+  // n_kept carrying the key (ncols * D) << 32, which the bit range must then hold.  A stable sort over more bits gives
+  // the same order.
+  const long long n_cd = (long long)g.ncols * depth_bins;
   int cd_bits = 1;
-  while ((1ll << cd_bits) < (long long)g.ncols * depth_bins) ++cd_bits;
+  while ((1ll << cd_bits) < n_cd + (dev ? 1 : 0)) ++cd_bits;
   size_t cub_bytes = w.cub_bytes;
   BEVB200_CUDA(cub::DeviceRadixSort::SortPairs(w.cub_tmp, cub_bytes, (const unsigned long long *)w.keys_a, w.keys_b,
                                                (const uint32_t *)w.vals_a, w.vals_b, n_kept, 0, 32 + cd_bits, st));
   g_launch_count += (32 + cd_bits + 7) / 8 + 2;
-  BEVB200_LAUNCH(lift_heads_kernel, grid_for(n_kept, 256), 256, 0, st, w.keys_b, n_kept, w.flags);
+  BEVB200_LAUNCH(lift_heads_kernel, grid_for(n_kept, 256), 256, 0, st, w.keys_b, n_kept, w.flags, counts);
   int rc = exclusive_scan_u32(w.flags, w.pos, n_kept, w.tiles, w.total, false, st);
   if (rc) return rc;
-  BEVB200_CUDA(cudaMemcpyAsync(n_segments, w.total, sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  // the segment records: all of them (host count), or the first max_segments (sync-free)
+  const uint32_t seg_cap = dev ? (uint32_t)max_segments : 0xffffffffu;
+  if (dev) {
+    BEVB200_LAUNCH(lift_form_kernel, 1, 1, 0, st, w.total, max_segments, n_segments, lift_form);
+  } else {
+    BEVB200_CUDA(cudaMemcpyAsync(n_segments, w.total, sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  }
   BEVB200_LAUNCH(lift_segments_kernel, grid_for(n_kept, 256), 256, 0, st, w.keys_b, w.vals_b, w.flags, w.pos, n_kept,
-                 (unsigned long long *)seg_key, (unsigned long long *)seg_mask);
-  // The slot pass needs the segment count on the host only for grid sizing: n_kept bounds it, and the kernels
-  // are bounded by the device count through `total` -- read it back once (this is a per-calibration call).
-  int32_t n_seg = 0;
-  BEVB200_CUDA(cudaMemcpyAsync(&n_seg, w.total, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  BEVB200_CUDA(cudaStreamSynchronize(st));
-  BEVB200_LAUNCH(lift_seg_ival_kernel, grid_for(n_seg, 256), 256, 0, st, (const unsigned long long *)seg_key, n_seg,
-                 w.ival_a, w.idx_a);
+                 (unsigned long long *)seg_key, (unsigned long long *)seg_mask, counts, seg_cap);
+  // The slot pass sorts the segments by interval.  The host-count prepare reads the segment count back once (this is
+  // a per-calibration call) and sorts exactly that many; the sync-free one sorts max_segments entries, those past the
+  // device count keyed after every interval, and its slot and column passes do nothing when the count is over the cap.
+  int n_items;
+  if (dev) {
+    n_items = max_segments;
+  } else {
+    int32_t n_seg = 0;
+    BEVB200_CUDA(cudaMemcpyAsync(&n_seg, w.total, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    BEVB200_CUDA(cudaStreamSynchronize(st));
+    n_items = n_seg;
+  }
+  const int32_t *n_seg_dev = dev ? n_segments : nullptr;
+  BEVB200_LAUNCH(lift_seg_ival_kernel, grid_for(n_items, 256), 256, 0, st, (const unsigned long long *)seg_key, n_items,
+                 w.ival_a, w.idx_a, n_seg_dev, (uint32_t)n_kept);
+  // interval ids are below n_intervals; the sync-free key past the count is n_kept (capacity) and must fit as well
+  const long long iv_bound = dev ? (long long)n_kept + 1 : (long long)n_intervals;
   int iv_bits = 1;
-  while ((1ll << iv_bits) < (long long)n_intervals) ++iv_bits;
+  while ((1ll << iv_bits) < iv_bound) ++iv_bits;
   cub_bytes = w.cub_bytes;
   BEVB200_CUDA(cub::DeviceRadixSort::SortPairs(w.cub_tmp, cub_bytes, (const uint32_t *)w.ival_a, w.ival_b,
-                                               (const uint32_t *)w.idx_a, w.idx_b, n_seg, 0, iv_bits, st));
+                                               (const uint32_t *)w.idx_a, w.idx_b, n_items, 0, iv_bits, st));
   g_launch_count += (iv_bits + 7) / 8 + 2;
-  BEVB200_LAUNCH(lift_slots_kernel, grid_for(n_seg, 256), 256, 0, st, w.ival_b, w.idx_b, n_seg, n_intervals, seg_slot,
-                 interval_slot_begin);
-  BEVB200_LAUNCH(lift_col_begin_kernel, grid_for(g.ncols + 1, 256), 256, 0, st, (const unsigned long long *)seg_key, n_seg,
-                 g, col_begin);
+  BEVB200_LAUNCH(lift_slots_kernel, grid_for(n_items, 256), 256, 0, st, w.ival_b, w.idx_b, n_items, n_intervals,
+                 seg_slot, interval_slot_begin, counts, n_seg_dev, lift_form);
+  BEVB200_LAUNCH(lift_col_begin_kernel, grid_for(g.ncols + 1, 256), 256, 0, st, (const unsigned long long *)seg_key,
+                 n_items, g, col_begin, n_seg_dev, lift_form);
   return BEVB200_OK;
 }
 
-int bevb200_bev_pool_lift_columns(int b, int d, int h, int w, int n, int c, int n_intervals, const float *depth,
-                                  const float *ctx, int cameras, int depth_bins, int feature_h, int feature_w,
-                                  const int32_t *geom_feats, const int32_t *interval_starts, const int32_t *col_begin,
-                                  const uint64_t *seg_key, const uint64_t *seg_mask, const int32_t *seg_slot,
-                                  const int32_t *interval_slot_begin, int n_segments, float *out, void *workspace,
-                                  size_t workspace_bytes, void *stream) {
+static int lift_columns(int b, int d, int h, int w, int n, int c, int n_intervals, const float *depth, const float *ctx,
+                        int cameras, int depth_bins, int feature_h, int feature_w, const int32_t *geom_feats,
+                        const int32_t *interval_starts, const int32_t *col_begin, const uint64_t *seg_key,
+                        const uint64_t *seg_mask, const int32_t *seg_slot, const int32_t *interval_slot_begin,
+                        int n_segments, float *out, void *workspace, size_t workspace_bytes, cudaStream_t st,
+                        const int32_t *counts, const int32_t *lift_form) {
   BEVB200_REQUIRE(b > 0 && d > 0 && h > 0 && w > 0 && c > 0 && n >= 0 && n_intervals >= 0 && n_segments >= 0, "bad sizes");
   BEVB200_REQUIRE(out != nullptr, "null out");
   BEVB200_REQUIRE(c % 4 == 0 && c <= 256, "channel count must be a multiple of 4, <= 256");
@@ -594,26 +674,148 @@ int bevb200_bev_pool_lift_columns(int b, int d, int h, int w, int n, int c, int 
     BEVB200_REQUIRE(smem <= 200 * 1024, "image column does not fit in shared memory");
     BEVB200_REQUIRE(TunedWidths::has(c), "no tuned kernel for this channel count");
   }
-  cudaStream_t st = (cudaStream_t)stream;
   const int zfill = (b * d == 1 && work) ? 1 : 0;
-  if (!zfill) BEVB200_CUDA(cudaMemsetAsync(out, 0, (size_t)b * d * h * w * c * sizeof(float), st));
+  // with zfill the cells kernel zeroes the empty cells; a grid with no kept point (known on the device only) is
+  // zeroed by zero_fill, which then does nothing unless the tables are empty
+  if (!zfill || counts)
+    if (const int rc = zero_fill(out, (size_t)b * d * h * w * c, lift_form, BEVB200_LIFT_COLUMNS, st,
+                                 zfill ? counts : nullptr))
+      return rc;
   if (!work) return BEVB200_OK;
   PoolDims dm{b, d, h, w};
   LiftGeom g{depth_bins, feature_h, feature_w, cameras * feature_w};
   BEVB200_LAUNCH(pool_interval_cells_kernel, grid_for(n_intervals, 256), 256, 0, st, geom_feats, interval_starts, n,
-                 n_intervals, dm, ws.cells);
+                 n_intervals, dm, ws.cells, counts);
   const int total_cells = b * d * h * w;
   return TunedWidths::dispatch(c, [&](auto q) {
     constexpr int Q = decltype(q)::value;
     BEVB200_CUDA(cudaFuncSetAttribute(lift_columns_kernel<Q>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     BEVB200_LAUNCH(lift_columns_kernel<Q>, g.ncols, 256, smem, st, depth, (const float4 *)ctx, g, col_begin,
                    (const unsigned long long *)seg_key, (const unsigned long long *)seg_mask, seg_slot,
-                   (float4 *)ws.partial);
-    BEVB200_LAUNCH(lift_cells_kernel<Q>, grid_for((long long)n_intervals * 32, 256, kNumSMs * 8), 256, 0, st,
+                   (float4 *)ws.partial, lift_form);
+    const auto cells = counts ? &lift_cells_kernel<Q, true> : &lift_cells_kernel<Q, false>;
+    BEVB200_LAUNCH(cells, grid_for((long long)n_intervals * 32, 256, kNumSMs * 8), 256, 0, st,
                    (const float4 *)ws.partial, interval_slot_begin, ws.cells, n_intervals, zfill, total_cells,
-                   (float4 *)out);
+                   (float4 *)out, counts, lift_form);
     return BEVB200_OK;
   });
+}
+
+static int lift_columns_backward(int b, int d, int h, int w, int n, int c, int n_intervals, const float *out_grad,
+                                 const float *depth, const float *ctx, int cameras, int depth_bins, int feature_h,
+                                 int feature_w, const int32_t *geom_feats, const int32_t *interval_starts,
+                                 const int32_t *col_begin, const uint64_t *seg_key, const uint64_t *seg_mask,
+                                 int n_segments, float *ddepth, float *dctx, void *workspace, size_t workspace_bytes,
+                                 cudaStream_t st, const int32_t *counts, const int32_t *n_seg_dev,
+                                 const int32_t *lift_form) {
+  BEVB200_REQUIRE(b > 0 && d > 0 && h > 0 && w > 0 && n >= 0 && n_intervals >= 0 && n_segments >= 0, "bad sizes");
+  BEVB200_REQUIRE(cameras > 0 && depth_bins > 0 && feature_h > 0 && feature_w > 0, "bad lift dims");
+  BEVB200_REQUIRE(feature_h <= 64, "feature height > 64: use bevb200_bev_pool_lift_backward");
+  BEVB200_REQUIRE(TunedWidths::has(c), "no tuned kernel for this channel count");
+  BEVB200_REQUIRE((long long)b * d * h * w < (1ll << 31), "grid has too many cells");
+  BEVB200_REQUIRE((long long)cameras * feature_w * depth_bins < (1ll << 31), "too many (column, depth) pairs");
+  if (ddepth == nullptr && dctx == nullptr) return BEVB200_OK;
+  BEVB200_REQUIRE(out_grad && col_begin && seg_key && seg_mask, "null input");
+  // the interval tables are read through the segments only: with no kept point (empty tables) they may be NULL
+  BEVB200_REQUIRE(n_segments == 0 || (geom_feats && interval_starts), "null interval tables");
+  BEVB200_REQUIRE(ctx || !ddepth, "ddepth needs ctx");
+  BEVB200_REQUIRE(depth || !dctx, "dctx needs depth");
+  BEVB200_REQUIRE(((uintptr_t)ctx % 16 == 0) && ((uintptr_t)dctx % 16 == 0) && ((uintptr_t)out_grad % 16 == 0),
+                  "ctx / dctx / out_grad must be 16-byte aligned");
+  int32_t *seg_cell;
+  if (const int rc = workspace_check("bev_pool_lift_columns_backward", workspace, workspace_bytes,
+                                     lift_bwd_layout(n_segments, workspace, &seg_cell)))
+    return rc;
+  const int q = c / 4;
+  const LiftBwdSmem sm = lift_bwd_smem(q, feature_h, depth_bins);
+  // chunk size: all of a column's segments at once when that stays within ~100 KB (two CTAs per SM), else as many
+  // as the 227 KB of one CTA allow
+  constexpr size_t kTwoPerSM = 100 * 1024, kMaxSmem = 220 * 1024;
+  long long smax = sm.fixed < kTwoPerSM ? (long long)((kTwoPerSM - sm.fixed) / sm.per_seg) : 0;
+  if (smax < 32 && sm.fixed < kMaxSmem) smax = (long long)((kMaxSmem - sm.fixed) / sm.per_seg);
+  if (smax > 256) smax = 256;
+  BEVB200_REQUIRE(smax >= 1, "image column does not fit in shared memory");
+  const size_t smem = sm.fixed + (size_t)smax * sm.per_seg;
+  LiftGeom g{depth_bins, feature_h, feature_w, cameras * feature_w};
+  if (n_segments > 0) {
+    PoolDims dm{b, d, h, w};
+    BEVB200_LAUNCH(lift_seg_cells_kernel, grid_for(n_segments, 256), 256, 0, st, (const unsigned long long *)seg_key,
+                   n_segments, geom_feats, interval_starts, n, dm, seg_cell, counts, n_seg_dev, lift_form);
+  }
+  return TunedWidths::dispatch(c, [&](auto q) {
+    constexpr int Q = decltype(q)::value;
+    BEVB200_CUDA(cudaFuncSetAttribute(lift_columns_bwd_kernel<Q>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    BEVB200_LAUNCH(lift_columns_bwd_kernel<Q>, g.ncols, 256, smem, st, (const float4 *)out_grad, depth,
+                   (const float4 *)ctx, g, col_begin, (const unsigned long long *)seg_key,
+                   (const unsigned long long *)seg_mask, seg_cell, (int)smax, ddepth, (float4 *)dctx, lift_form);
+    return BEVB200_OK;
+  });
+}
+
+static int lift_rows_backward(int b, int d, int h, int w, int n, int n_total, int c, int n_intervals,
+                              const float *out_grad, const float *depth, const float *ctx, int depth_bins,
+                              int pixels_per_camera, const int32_t *perm, const int32_t *geom_feats,
+                              const int32_t *interval_starts, const int32_t *interval_lengths, float *ddepth,
+                              float *dctx, void *workspace, size_t workspace_bytes, cudaStream_t st,
+                              const int32_t *counts, const int32_t *lift_form) {
+  BEVB200_REQUIRE(b > 0 && d > 0 && h > 0 && w > 0 && n >= 0 && n_total >= n && n_intervals >= 0, "bad sizes");
+  BEVB200_REQUIRE(depth_bins > 0 && pixels_per_camera > 0 && n_total % ((long long)depth_bins * pixels_per_camera) == 0,
+                  "bad lift dims");
+  BEVB200_REQUIRE(TunedWidths::has(c), "no tuned kernel for this channel count");
+  BEVB200_REQUIRE((long long)b * d * h * w < (1ll << 31), "grid has too many cells");
+  if (ddepth == nullptr && dctx == nullptr) return BEVB200_OK;
+  BEVB200_REQUIRE(out_grad && perm && geom_feats && interval_starts && interval_lengths, "null input");
+  BEVB200_REQUIRE(ctx || !ddepth, "ddepth needs ctx");
+  BEVB200_REQUIRE(depth || !dctx, "dctx needs depth");
+  BEVB200_REQUIRE(((uintptr_t)ctx % 16 == 0) && ((uintptr_t)dctx % 16 == 0) && ((uintptr_t)out_grad % 16 == 0),
+                  "ctx / dctx / out_grad must be 16-byte aligned");
+  int32_t *point_cell;
+  if (const int rc = workspace_check("bev_pool_lift_backward", workspace, workspace_bytes,
+                                     lift_bwd_layout(n_total, workspace, &point_cell)))
+    return rc;
+  if (n_total == 0) return BEVB200_OK;
+  PoolDims dm{b, d, h, w};
+  BEVB200_LAUNCH(lift_point_cells_kernel, grid_for((long long)n_total, 256), 256, 0, st, perm, geom_feats,
+                 interval_starts, interval_lengths, n, n_total, n_intervals, dm, point_cell, counts, lift_form);
+  const int n_pixels = (int)(n_total / depth_bins);
+  const int grid = grid_for((long long)n_pixels * 32, 256, kNumSMs * 16);
+  return TunedWidths::dispatch(c, [&](auto q) {
+    BEVB200_LAUNCH(lift_pixels_bwd_kernel<decltype(q)::value>, grid, 256, 0, st, (const float4 *)out_grad, depth,
+                   (const float4 *)ctx, point_cell, n_pixels, depth_bins, pixels_per_camera, ddepth, (float4 *)dctx,
+                   lift_form);
+    return BEVB200_OK;
+  });
+}
+
+}  // namespace bevb200
+
+using namespace bevb200;
+
+extern "C" {
+
+size_t bevb200_bev_pool_lift_prepare_workspace_bytes(int n_kept) {
+  if (n_kept < 0) return 0;
+  return lift_prepare_layout(n_kept, nullptr, 0, nullptr);
+}
+
+int bevb200_bev_pool_lift_prepare(const int32_t *perm, const int32_t *interval_starts, int n_kept, int n_intervals,
+                                  int cameras, int depth_bins, int feature_h, int feature_w, int32_t *col_begin,
+                                  uint64_t *seg_key, uint64_t *seg_mask, int32_t *seg_slot, int32_t *interval_slot_begin,
+                                  int32_t *n_segments, void *workspace, size_t workspace_bytes, void *stream) {
+  return lift_prepare(perm, interval_starts, n_kept, n_intervals, cameras, depth_bins, feature_h, feature_w, col_begin,
+                      seg_key, seg_mask, seg_slot, interval_slot_begin, n_segments, workspace, workspace_bytes,
+                      (cudaStream_t)stream, nullptr, 0, nullptr);
+}
+
+int bevb200_bev_pool_lift_columns(int b, int d, int h, int w, int n, int c, int n_intervals, const float *depth,
+                                  const float *ctx, int cameras, int depth_bins, int feature_h, int feature_w,
+                                  const int32_t *geom_feats, const int32_t *interval_starts, const int32_t *col_begin,
+                                  const uint64_t *seg_key, const uint64_t *seg_mask, const int32_t *seg_slot,
+                                  const int32_t *interval_slot_begin, int n_segments, float *out, void *workspace,
+                                  size_t workspace_bytes, void *stream) {
+  return lift_columns(b, d, h, w, n, c, n_intervals, depth, ctx, cameras, depth_bins, feature_h, feature_w, geom_feats,
+                      interval_starts, col_begin, seg_key, seg_mask, seg_slot, interval_slot_begin, n_segments, out,
+                      workspace, workspace_bytes, (cudaStream_t)stream, nullptr, nullptr);
 }
 
 size_t bevb200_bev_pool_lift_columns_workspace_bytes(int n_segments, int n_intervals, int c) {
@@ -633,47 +835,9 @@ int bevb200_bev_pool_lift_columns_backward(int b, int d, int h, int w, int n, in
                                            const uint64_t *seg_key, const uint64_t *seg_mask, int n_segments,
                                            float *ddepth, float *dctx, void *workspace, size_t workspace_bytes,
                                            void *stream) {
-  BEVB200_REQUIRE(b > 0 && d > 0 && h > 0 && w > 0 && n >= 0 && n_intervals >= 0 && n_segments >= 0, "bad sizes");
-  BEVB200_REQUIRE(cameras > 0 && depth_bins > 0 && feature_h > 0 && feature_w > 0, "bad lift dims");
-  BEVB200_REQUIRE(feature_h <= 64, "feature height > 64: use bevb200_bev_pool_lift_backward");
-  BEVB200_REQUIRE(TunedWidths::has(c), "no tuned kernel for this channel count");
-  BEVB200_REQUIRE((long long)b * d * h * w < (1ll << 31), "grid has too many cells");
-  BEVB200_REQUIRE((long long)cameras * feature_w * depth_bins < (1ll << 31), "too many (column, depth) pairs");
-  if (ddepth == nullptr && dctx == nullptr) return BEVB200_OK;
-  BEVB200_REQUIRE(out_grad && col_begin && seg_key && seg_mask && geom_feats && interval_starts, "null input");
-  BEVB200_REQUIRE(ctx || !ddepth, "ddepth needs ctx");
-  BEVB200_REQUIRE(depth || !dctx, "dctx needs depth");
-  BEVB200_REQUIRE(((uintptr_t)ctx % 16 == 0) && ((uintptr_t)dctx % 16 == 0) && ((uintptr_t)out_grad % 16 == 0),
-                  "ctx / dctx / out_grad must be 16-byte aligned");
-  int32_t *seg_cell;
-  if (const int rc = workspace_check("bev_pool_lift_columns_backward", workspace, workspace_bytes,
-                                     lift_bwd_layout(n_segments, workspace, &seg_cell)))
-    return rc;
-  const int q = c / 4;
-  const LiftBwdSmem sm = lift_bwd_smem(q, feature_h, depth_bins);
-  // chunk size: all of a column's segments at once when that stays within ~100 KB (two CTAs per SM), else as many
-  // as the 227 KB of one CTA allow
-  constexpr size_t kTwoPerSM = 100 * 1024, kMaxSmem = 220 * 1024;
-  long long smax = sm.fixed < kTwoPerSM ? (long long)((kTwoPerSM - sm.fixed) / sm.per_seg) : 0;
-  if (smax < 32 && sm.fixed < kMaxSmem) smax = (long long)((kMaxSmem - sm.fixed) / sm.per_seg);
-  if (smax > 256) smax = 256;
-  BEVB200_REQUIRE(smax >= 1, "image column does not fit in shared memory");
-  const size_t smem = sm.fixed + (size_t)smax * sm.per_seg;
-  cudaStream_t st = (cudaStream_t)stream;
-  LiftGeom g{depth_bins, feature_h, feature_w, cameras * feature_w};
-  if (n_segments > 0) {
-    PoolDims dm{b, d, h, w};
-    BEVB200_LAUNCH(lift_seg_cells_kernel, grid_for(n_segments, 256), 256, 0, st, (const unsigned long long *)seg_key,
-                   n_segments, geom_feats, interval_starts, n, dm, seg_cell);
-  }
-  return TunedWidths::dispatch(c, [&](auto q) {
-    constexpr int Q = decltype(q)::value;
-    BEVB200_CUDA(cudaFuncSetAttribute(lift_columns_bwd_kernel<Q>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    BEVB200_LAUNCH(lift_columns_bwd_kernel<Q>, g.ncols, 256, smem, st, (const float4 *)out_grad, depth,
-                   (const float4 *)ctx, g, col_begin, (const unsigned long long *)seg_key,
-                   (const unsigned long long *)seg_mask, seg_cell, (int)smax, ddepth, (float4 *)dctx);
-    return BEVB200_OK;
-  });
+  return lift_columns_backward(b, d, h, w, n, c, n_intervals, out_grad, depth, ctx, cameras, depth_bins, feature_h,
+                               feature_w, geom_feats, interval_starts, col_begin, seg_key, seg_mask, n_segments, ddepth,
+                               dctx, workspace, workspace_bytes, (cudaStream_t)stream, nullptr, nullptr, nullptr);
 }
 
 size_t bevb200_bev_pool_lift_backward_workspace_bytes(int n_total, int c) {
@@ -686,33 +850,85 @@ int bevb200_bev_pool_lift_backward(int b, int d, int h, int w, int n, int n_tota
                                    int pixels_per_camera, const int32_t *perm, const int32_t *geom_feats,
                                    const int32_t *interval_starts, const int32_t *interval_lengths, float *ddepth,
                                    float *dctx, void *workspace, size_t workspace_bytes, void *stream) {
-  BEVB200_REQUIRE(b > 0 && d > 0 && h > 0 && w > 0 && n >= 0 && n_total >= n && n_intervals >= 0, "bad sizes");
-  BEVB200_REQUIRE(depth_bins > 0 && pixels_per_camera > 0 && n_total % ((long long)depth_bins * pixels_per_camera) == 0,
-                  "bad lift dims");
-  BEVB200_REQUIRE(TunedWidths::has(c), "no tuned kernel for this channel count");
-  BEVB200_REQUIRE((long long)b * d * h * w < (1ll << 31), "grid has too many cells");
-  if (ddepth == nullptr && dctx == nullptr) return BEVB200_OK;
-  BEVB200_REQUIRE(out_grad && perm && geom_feats && interval_starts && interval_lengths, "null input");
-  BEVB200_REQUIRE(ctx || !ddepth, "ddepth needs ctx");
-  BEVB200_REQUIRE(depth || !dctx, "dctx needs depth");
-  BEVB200_REQUIRE(((uintptr_t)ctx % 16 == 0) && ((uintptr_t)dctx % 16 == 0) && ((uintptr_t)out_grad % 16 == 0),
-                  "ctx / dctx / out_grad must be 16-byte aligned");
-  int32_t *point_cell;
-  if (const int rc = workspace_check("bev_pool_lift_backward", workspace, workspace_bytes,
-                                     lift_bwd_layout(n_total, workspace, &point_cell)))
-    return rc;
-  if (n_total == 0) return BEVB200_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  PoolDims dm{b, d, h, w};
-  BEVB200_LAUNCH(lift_point_cells_kernel, grid_for((long long)n_total, 256), 256, 0, st, perm, geom_feats,
-                 interval_starts, interval_lengths, n, n_total, n_intervals, dm, point_cell);
-  const int n_pixels = (int)(n_total / depth_bins);
-  const int grid = grid_for((long long)n_pixels * 32, 256, kNumSMs * 16);
-  return TunedWidths::dispatch(c, [&](auto q) {
-    BEVB200_LAUNCH(lift_pixels_bwd_kernel<decltype(q)::value>, grid, 256, 0, st, (const float4 *)out_grad, depth,
-                   (const float4 *)ctx, point_cell, n_pixels, depth_bins, pixels_per_camera, ddepth, (float4 *)dctx);
-    return BEVB200_OK;
-  });
+  return lift_rows_backward(b, d, h, w, n, n_total, c, n_intervals, out_grad, depth, ctx, depth_bins,
+                            pixels_per_camera, perm, geom_feats, interval_starts, interval_lengths, ddepth, dctx,
+                            workspace, workspace_bytes, (cudaStream_t)stream, nullptr, nullptr);
+}
+
+// ---- sync-free twins ------------------------------------------------------------------------------------------------
+
+size_t bevb200_bev_pool_lift_prepare_dev_workspace_bytes(int n_capacity, int max_segments) {
+  if (n_capacity <= 0 || max_segments <= 0 || max_segments > n_capacity) return 0;
+  return lift_prepare_layout(n_capacity, nullptr, 0, nullptr);
+}
+
+int bevb200_bev_pool_lift_prepare_dev(const int32_t *perm, const int32_t *interval_starts, const int32_t *counts_dev,
+                                      int n_capacity, int max_segments, int cameras, int depth_bins, int feature_h,
+                                      int feature_w, int32_t *col_begin, uint64_t *seg_key, uint64_t *seg_mask,
+                                      int32_t *seg_slot, int32_t *interval_slot_begin, int32_t *n_segments,
+                                      int32_t *lift_form, void *workspace, size_t workspace_bytes, void *stream) {
+  BEVB200_REQUIRE(counts_dev != nullptr, "null counts");
+  return lift_prepare(perm, interval_starts, n_capacity, n_capacity, cameras, depth_bins, feature_h, feature_w,
+                      col_begin, seg_key, seg_mask, seg_slot, interval_slot_begin, n_segments, workspace,
+                      workspace_bytes, (cudaStream_t)stream, counts_dev, max_segments, lift_form);
+}
+
+size_t bevb200_bev_pool_lift_columns_dev_workspace_bytes(int max_segments, int n_capacity, int c) {
+  if (max_segments <= 0 || n_capacity <= 0 || c <= 0) return 0;
+  return lift_columns_layout(max_segments, n_capacity, c, nullptr, nullptr) + kLiftQuerySlack;
+}
+
+int bevb200_bev_pool_lift_columns_dev(int b, int d, int h, int w, int n_capacity, int c, const float *depth,
+                                      const float *ctx, int cameras, int depth_bins, int feature_h, int feature_w,
+                                      const int32_t *geom_feats, const int32_t *interval_starts,
+                                      const int32_t *col_begin, const uint64_t *seg_key, const uint64_t *seg_mask,
+                                      const int32_t *seg_slot, const int32_t *interval_slot_begin, int max_segments,
+                                      const int32_t *counts_dev, const int32_t *lift_form, float *out,
+                                      void *workspace, size_t workspace_bytes, void *stream) {
+  BEVB200_REQUIRE(n_capacity > 0 && max_segments > 0, "capacities must be positive");
+  BEVB200_REQUIRE(counts_dev && lift_form, "null counts / lift_form");
+  return lift_columns(b, d, h, w, n_capacity, c, n_capacity, depth, ctx, cameras, depth_bins, feature_h, feature_w,
+                      geom_feats, interval_starts, col_begin, seg_key, seg_mask, seg_slot, interval_slot_begin,
+                      max_segments, out, workspace, workspace_bytes, (cudaStream_t)stream, counts_dev, lift_form);
+}
+
+size_t bevb200_bev_pool_lift_columns_backward_dev_workspace_bytes(int max_segments, int c) {
+  if (max_segments <= 0 || !TunedWidths::has(c)) return 0;
+  return lift_bwd_layout(max_segments, nullptr, nullptr) + kLiftQuerySlack;
+}
+
+int bevb200_bev_pool_lift_columns_backward_dev(int b, int d, int h, int w, int n_capacity, int c,
+                                               const float *out_grad, const float *depth, const float *ctx,
+                                               int cameras, int depth_bins, int feature_h, int feature_w,
+                                               const int32_t *geom_feats, const int32_t *interval_starts,
+                                               const int32_t *col_begin, const uint64_t *seg_key,
+                                               const uint64_t *seg_mask, int max_segments, const int32_t *counts_dev,
+                                               const int32_t *n_segments_dev, const int32_t *lift_form, float *ddepth,
+                                               float *dctx, void *workspace, size_t workspace_bytes, void *stream) {
+  BEVB200_REQUIRE(n_capacity > 0 && max_segments > 0, "capacities must be positive");
+  BEVB200_REQUIRE(counts_dev && n_segments_dev && lift_form, "null counts / n_segments / lift_form");
+  return lift_columns_backward(b, d, h, w, n_capacity, c, n_capacity, out_grad, depth, ctx, cameras, depth_bins,
+                               feature_h, feature_w, geom_feats, interval_starts, col_begin, seg_key, seg_mask,
+                               max_segments, ddepth, dctx, workspace, workspace_bytes, (cudaStream_t)stream,
+                               counts_dev, n_segments_dev, lift_form);
+}
+
+size_t bevb200_bev_pool_lift_backward_dev_workspace_bytes(int n_total, int c) {
+  if (n_total <= 0 || !TunedWidths::has(c)) return 0;
+  return lift_bwd_layout(n_total, nullptr, nullptr) + kLiftQuerySlack;
+}
+
+int bevb200_bev_pool_lift_backward_dev(int b, int d, int h, int w, int n_total, int c, const float *out_grad,
+                                       const float *depth, const float *ctx, int depth_bins, int pixels_per_camera,
+                                       const int32_t *perm, const int32_t *geom_feats, const int32_t *interval_starts,
+                                       const int32_t *interval_lengths, const int32_t *counts_dev,
+                                       const int32_t *lift_form, float *ddepth, float *dctx, void *workspace,
+                                       size_t workspace_bytes, void *stream) {
+  BEVB200_REQUIRE(n_total > 0, "capacity must be positive");
+  BEVB200_REQUIRE(counts_dev != nullptr, "null counts");
+  return lift_rows_backward(b, d, h, w, n_total, n_total, c, n_total, out_grad, depth, ctx, depth_bins,
+                            pixels_per_camera, perm, geom_feats, interval_starts, interval_lengths, ddepth, dctx,
+                            workspace, workspace_bytes, (cudaStream_t)stream, counts_dev, lift_form);
 }
 
 }  // extern "C"

@@ -59,6 +59,57 @@ def camera_rig(n_cam=6, image_size=(256, 704), batch=1):
                 post_rots=st(prot), post_trans=st(ptr))
 
 
+def augmented_rig(n_cam=6, image_size=(256, 704), batch=1, seed=0):
+    """camera_rig under one seeded draw of the reference's training augmentation (configs/nuscenes/default.yaml):
+    ImageAug3D per image (resize 0.38-0.55 of 1600x900 -- scaled with the image width, as camera_rig's 0.48 is --,
+    bottom crop, random horizontal crop, flip with p = 0.5, rotation +-5.4 deg about the image centre) and, per sample,
+    GlobalRotScaleTrans (scale 0.9-1.1, z rotation +-45 deg, translation N(0, 0.5 m)) followed by RandomFlip3D (x and
+    y flips, p = 0.5 each).  Returns camera_rig's dict with post_rots / post_trans replaced and extra_rots [B, 3, 3] /
+    extra_trans [B, 3] (the lidar augmentation) added; fp32 on the host."""
+    rig = camera_rig(n_cam, image_size, batch)
+    rng = np.random.RandomState(seed)
+    fH, fW = image_size
+    width_scale = fW / 704.0
+    post_rots = torch.eye(3).repeat(batch, n_cam, 1, 1)
+    post_trans = torch.zeros(batch, n_cam, 3)
+    for b in range(batch):
+        for n in range(n_cam):
+            resize = rng.uniform(0.38, 0.55) * width_scale
+            new_w, new_h = int(1600 * resize), int(900 * resize)
+            crop_h = new_h - fH
+            crop_w = int(rng.uniform(0, max(0, new_w - fW)))
+            flip = bool(rng.choice([0, 1]))
+            theta = math.radians(rng.uniform(-5.4, 5.4))
+            rot = resize * np.eye(2)
+            tran = -np.array([crop_w, crop_h], dtype=np.float64)
+            if flip:
+                A = np.array([[-1.0, 0.0], [0.0, 1.0]])
+                rot, tran = A @ rot, A @ tran + np.array([fW, 0.0])
+            A = np.array([[math.cos(theta), math.sin(theta)], [-math.sin(theta), math.cos(theta)]])
+            centre = np.array([fW, fH], dtype=np.float64) / 2.0
+            rot, tran = A @ rot, A @ tran + (A @ -centre + centre)
+            post_rots[b, n, :2, :2] = torch.from_numpy(rot).float()
+            post_trans[b, n, :2] = torch.from_numpy(tran).float()
+    extra_rots = torch.zeros(batch, 3, 3)
+    extra_trans = torch.zeros(batch, 3)
+    for b in range(batch):
+        scale = rng.uniform(0.9, 1.1)
+        theta = rng.uniform(-0.78539816, 0.78539816)
+        t = rng.normal(0.0, 0.5, 3)
+        R = np.array([[math.cos(theta), -math.sin(theta), 0.0], [math.sin(theta), math.cos(theta), 0.0],
+                      [0.0, 0.0, 1.0]])
+        M = np.concatenate([R.T * scale, (t * scale)[:, None]], 1)
+        if rng.choice([0, 1]):
+            M = np.diag([1.0, -1.0, 1.0]) @ M
+        if rng.choice([0, 1]):
+            M = np.diag([-1.0, 1.0, 1.0]) @ M
+        extra_rots[b] = torch.from_numpy(M[:, :3]).float()
+        extra_trans[b] = torch.from_numpy(M[:, 3]).float()
+    rig.update(post_rots=post_rots.contiguous(), post_trans=post_trans.contiguous(),
+               extra_rots=extra_rots.contiguous(), extra_trans=extra_trans.contiguous())
+    return rig
+
+
 def lidar_camera_matrices(n_cam=6, image_size=(256, 704), batch=1, augment=True):
     """4x4 matrices the depth-aware lift consumes (base.py:237-262), consistent with camera_rig:
     lidar2image = K @ inverse(camera2lidar), img_aug_matrix from the resize / crop, and a

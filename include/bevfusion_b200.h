@@ -195,6 +195,76 @@ BEVB200_API int bevb200_bev_pool_lift_backward(int b, int d, int h, int w, int n
                                   const int32_t *interval_lengths, float *ddepth, float *dctx, void *workspace,
                                   size_t workspace_bytes, void *stream);
 
+/* Sync-free twins (*_dev) of the pooling, lift and lift-prepare calls above, for tables rebuilt every step without a
+ * host round trip (augmented training, per-sample calibration) and for CUDA-graph capture of that rebuild.  Each twin
+ * runs the same kernels as its host-count call, but reads the sizes from device memory:
+ *   counts_dev   int32[2] = {n_kept, n_intervals} as bevb200_bev_pool_prepare_* writes them
+ *   n_capacity   the size every table was allocated for (n_total, the frustum points of the plan): grids are sized from
+ *                it and the kernels stop at the device counts, so n_kept and n_intervals never reach the host
+ *   max_segments the capacity of the column tables (seg_key / seg_mask / seg_slot); 1 <= max_segments <= n_capacity
+ *   lift_form    int32[1] status word written by bevb200_bev_pool_lift_prepare_dev: BEVB200_LIFT_COLUMNS when the
+ *                device segment count fits under max_segments, BEVB200_LIFT_ROWS when it does not.  A lift call of a
+ *                form the word does not name launches its kernels, which exit at once: a caller launches both forms
+ *                (columns, then rows) and exactly one writes the output.  The column twins require it; the row twins
+ *                take NULL for "always run".
+ * Results are bit-identical to the host-count call on the same tables, including the zero-filled cells and rows for
+ * n_kept == 0 or n_intervals == 0.  Every argument is checked before the first write; a capacity <= 0 is refused.  The
+ * workspace queries take capacities and return 0 for a capacity <= 0 (or an unsupported channel count where the
+ * host-count query does).  None of these calls synchronises the host.
+ *   bevb200_bev_pool_perm_dev / _grad_perm_dev            bevb200_bev_pool_perm / _grad_perm; tables [n_capacity]
+ *   bevb200_bev_pool_lift_dev / _lift_backward_dev        the row lift (any feature_h) and its backward
+ *   bevb200_bev_pool_lift_prepare_dev                     column tables from device n_kept / n_intervals: sorts all
+ *       n_capacity keys (rows past n_kept sort last), writes n_segments[1] and lift_form[1]; interval_slot_begin
+ *       int32[n_capacity + 1], seg_* [max_segments].  Past the cap the column tables are not filled.
+ *   bevb200_bev_pool_lift_columns_dev / _columns_backward_dev   the column lift and its backward (feature_h <= 64) */
+#define BEVB200_LIFT_COLUMNS 0
+#define BEVB200_LIFT_ROWS 1
+BEVB200_API size_t bevb200_bev_pool_dev_workspace_bytes(int n_capacity, int c);
+BEVB200_API int bevb200_bev_pool_perm_dev(int b, int d, int h, int w, int n_capacity, int c, const float *x,
+                                  const int32_t *perm, const int32_t *geom_feats, const int32_t *interval_starts,
+                                  const int32_t *interval_lengths, const int32_t *counts_dev, float *out,
+                                  void *workspace, size_t workspace_bytes, void *stream);
+BEVB200_API int bevb200_bev_pool_grad_perm_dev(int b, int d, int h, int w, int n_total, int c, const float *out_grad,
+                                  const int32_t *perm, const int32_t *geom_feats, const int32_t *interval_starts,
+                                  const int32_t *interval_lengths, const int32_t *counts_dev, float *x_grad,
+                                  void *stream);
+BEVB200_API int bevb200_bev_pool_lift_dev(int b, int d, int h, int w, int n_capacity, int c, const float *depth,
+                                  const float *ctx, int depth_bins, int pixels_per_camera, const int32_t *perm,
+                                  const int32_t *geom_feats, const int32_t *interval_starts,
+                                  const int32_t *interval_lengths, const int32_t *counts_dev,
+                                  const int32_t *lift_form, float *out, void *workspace, size_t workspace_bytes,
+                                  void *stream);
+BEVB200_API size_t bevb200_bev_pool_lift_prepare_dev_workspace_bytes(int n_capacity, int max_segments);
+BEVB200_API int bevb200_bev_pool_lift_prepare_dev(const int32_t *perm, const int32_t *interval_starts,
+                                  const int32_t *counts_dev, int n_capacity, int max_segments, int cameras,
+                                  int depth_bins, int feature_h, int feature_w, int32_t *col_begin, uint64_t *seg_key,
+                                  uint64_t *seg_mask, int32_t *seg_slot, int32_t *interval_slot_begin,
+                                  int32_t *n_segments, int32_t *lift_form, void *workspace, size_t workspace_bytes,
+                                  void *stream);
+BEVB200_API size_t bevb200_bev_pool_lift_columns_dev_workspace_bytes(int max_segments, int n_capacity, int c);
+BEVB200_API int bevb200_bev_pool_lift_columns_dev(int b, int d, int h, int w, int n_capacity, int c,
+                                  const float *depth, const float *ctx, int cameras, int depth_bins, int feature_h,
+                                  int feature_w, const int32_t *geom_feats, const int32_t *interval_starts,
+                                  const int32_t *col_begin, const uint64_t *seg_key, const uint64_t *seg_mask,
+                                  const int32_t *seg_slot, const int32_t *interval_slot_begin, int max_segments,
+                                  const int32_t *counts_dev, const int32_t *lift_form, float *out, void *workspace,
+                                  size_t workspace_bytes, void *stream);
+BEVB200_API size_t bevb200_bev_pool_lift_columns_backward_dev_workspace_bytes(int max_segments, int c);
+BEVB200_API int bevb200_bev_pool_lift_columns_backward_dev(int b, int d, int h, int w, int n_capacity, int c,
+                                  const float *out_grad, const float *depth, const float *ctx, int cameras,
+                                  int depth_bins, int feature_h, int feature_w, const int32_t *geom_feats,
+                                  const int32_t *interval_starts, const int32_t *col_begin, const uint64_t *seg_key,
+                                  const uint64_t *seg_mask, int max_segments, const int32_t *counts_dev,
+                                  const int32_t *n_segments_dev, const int32_t *lift_form, float *ddepth, float *dctx,
+                                  void *workspace, size_t workspace_bytes, void *stream);
+BEVB200_API size_t bevb200_bev_pool_lift_backward_dev_workspace_bytes(int n_total, int c);
+BEVB200_API int bevb200_bev_pool_lift_backward_dev(int b, int d, int h, int w, int n_total, int c,
+                                  const float *out_grad, const float *depth, const float *ctx, int depth_bins,
+                                  int pixels_per_camera, const int32_t *perm, const int32_t *geom_feats,
+                                  const int32_t *interval_starts, const int32_t *interval_lengths,
+                                  const int32_t *counts_dev, const int32_t *lift_form, float *ddepth, float *dctx,
+                                  void *workspace, size_t workspace_bytes, void *stream);
+
 
 /* bev_pool precompute.  Replaces, on device and in one call, the index glue of
  * BaseTransform.bev_pool (mmdet3d/models/vtransforms/base.py:149-169: quantise, batch
