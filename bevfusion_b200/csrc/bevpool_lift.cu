@@ -425,6 +425,7 @@ __global__ void lift_point_cells_kernel(const int32_t *__restrict__ perm, const 
   const int lane = lane_id(), warps = (gridDim.x * blockDim.x) >> 5;
   if (form_off(lift_form, BEVB200_LIFT_ROWS)) return;
   device_counts(counts, n, n_intervals);
+  if (n_intervals == 0) n = 0;   // no interval pools anything: every point is filtered (no cell left unset)
   for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n_intervals; i += warps) {   // warp per interval
     const int s0 = starts[i], len = lengths[i];
     const int32_t c = interval_cell(geom_feats, s0, n, dm);
@@ -886,6 +887,7 @@ int bevb200_bev_pool_lift_columns_dev(int b, int d, int h, int w, int n_capacity
                                       const int32_t *counts_dev, const int32_t *lift_form, float *out,
                                       void *workspace, size_t workspace_bytes, void *stream) {
   BEVB200_REQUIRE(n_capacity > 0 && max_segments > 0, "capacities must be positive");
+  BEVB200_REQUIRE(max_segments <= n_capacity, "max_segments must lie in [1, capacity]");
   BEVB200_REQUIRE(counts_dev && lift_form, "null counts / lift_form");
   return lift_columns(b, d, h, w, n_capacity, c, n_capacity, depth, ctx, cameras, depth_bins, feature_h, feature_w,
                       geom_feats, interval_starts, col_begin, seg_key, seg_mask, seg_slot, interval_slot_begin,
@@ -906,6 +908,7 @@ int bevb200_bev_pool_lift_columns_backward_dev(int b, int d, int h, int w, int n
                                                const int32_t *n_segments_dev, const int32_t *lift_form, float *ddepth,
                                                float *dctx, void *workspace, size_t workspace_bytes, void *stream) {
   BEVB200_REQUIRE(n_capacity > 0 && max_segments > 0, "capacities must be positive");
+  BEVB200_REQUIRE(max_segments <= n_capacity, "max_segments must lie in [1, capacity]");
   BEVB200_REQUIRE(counts_dev && n_segments_dev && lift_form, "null counts / n_segments / lift_form");
   return lift_columns_backward(b, d, h, w, n_capacity, c, n_capacity, out_grad, depth, ctx, cameras, depth_bins,
                                feature_h, feature_w, geom_feats, interval_starts, col_begin, seg_key, seg_mask,
