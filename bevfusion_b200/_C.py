@@ -151,6 +151,7 @@ _SIGNATURES = {
     "bevb200_encoder_num_levels": (c_int, [_P]),
     "bevb200_encoder_output_shape": (c_int, [_P, _P, _P]),
     "bevb200_encoder_set_conv": (c_int, [_P, c_int, _P, _P, _P, _P, c_size_t, _P]),
+    "bevb200_encoder_set_conv_int8": (c_int, [_P, c_int, _P, _P, _P, c_float, c_float, c_float, _P, c_size_t, _P]),
     "bevb200_encoder_level_caps": (c_int, [_P, c_int, c_int, _P, _P]),
     "bevb200_encoder_workspace_bytes": (c_size_t, [_P, c_int, c_int, _P]),
     "bevb200_encoder_forward": (c_int, [_P, _P, _P, _P, c_int, _P, c_int, _P, _P, ctypes.c_longlong, _P, _P,

@@ -36,6 +36,7 @@ struct EConv {
   int level_in, level_out, rulebook;
   bool want_fp32;
   size_t packed_off, scale_off, shift_off;   // offsets into the parameter buffer
+  size_t q_off;                              // INT8: [r_out, s_res, s_w[c_out]]
   bool has_scale, has_shift;
 };
 struct ELevel {
@@ -54,7 +55,7 @@ using namespace bevb200;
 
 struct bevb200_encoder {
   int in_channels, c0_eff;
-  int precision;                     // BEVB200_PREC_BF16X3 (default) or BEVB200_PREC_FP16
+  int precision;                     // BEVB200_PREC_BF16X3 (default), BEVB200_PREC_FP16 or BEVB200_PREC_INT8
   std::vector<EConv> convs;
   std::vector<ELevel> levels;
   std::vector<ERulebook> rulebooks;
@@ -66,18 +67,36 @@ struct bevb200_encoder {
 namespace bevb200 {
 
 static bool enc_f16(const bevb200_encoder *e) { return e->precision == BEVB200_PREC_FP16; }
-// bytes per channel of the plan's operand images: BF16x3 split images 4, fp16 images 2
+static bool enc_i8(const bevb200_encoder *e) { return e->precision == BEVB200_PREC_INT8; }
+// bytes per channel of the plan's operand images: BF16x3 split images 4, fp16 images 2 (INT8: enc_level_row_bytes)
 static size_t enc_img_bytes(const bevb200_encoder *e) { return enc_f16(e) ? 2 : 4; }
 
-// offsets of every conv's packed weights, scale and shift in the parameter buffer (the weight image of the precision)
+// bytes per row of a level's two images.  INT8: the widest of the level-0 fp16 feature image and the u8 outputs of
+// the level's convs; the last conv writes its fp16 image into a buffer of its own (EWs::out16).
+static size_t enc_level_row_bytes(const bevb200_encoder *e, size_t l) {
+  if (!enc_i8(e)) return (size_t)e->levels[l].c_max * enc_img_bytes(e);
+  size_t b = l == 0 ? (size_t)e->c0_eff * 2 : 0;
+  for (size_t i = 0; i + 1 < e->convs.size(); ++i)
+    if ((size_t)e->convs[i].level_out == l) b = std::max(b, (size_t)e->convs[i].d.c_out);
+  return b;
+}
+
+// offsets of every conv's packed weights, scale and shift in the parameter buffer (the weight image of the precision).
+// INT8: the first conv keeps the fp16 image (it reads the fp16 features), the others take the s8 image; `scale` holds
+// the epilogue's factor a[c], and a block [r_out, s_res, s_w[c_out]] follows the shift.
 static void enc_param_layout(bevb200_encoder *e) {
   size_t poff = 0;
-  for (EConv &cv : e->convs) {
+  for (size_t i = 0; i < e->convs.size(); ++i) {
+    EConv &cv = e->convs[i];
     cv.packed_off = poff;
-    poff += align_up(enc_f16(e) ? spconv_v6_packed_bytes_f16(cv.d.c_in, cv.d.c_out, cv.kvol)
-                                : spconv_v6_packed_bytes(cv.d.c_in, cv.d.c_out, cv.kvol));
+    size_t pk = spconv_v6_packed_bytes(cv.d.c_in, cv.d.c_out, cv.kvol);
+    if (enc_f16(e) || (enc_i8(e) && i == 0)) pk = spconv_v6_packed_bytes_f16(cv.d.c_in, cv.d.c_out, cv.kvol);
+    else if (enc_i8(e)) pk = spconv_v6_packed_bytes_i8(cv.d.c_in, cv.d.c_out, cv.kvol);
+    poff += align_up(pk);
     cv.scale_off = poff; poff += align_up((size_t)cv.d.c_out * 4);
     cv.shift_off = poff; poff += align_up((size_t)cv.d.c_out * 4);
+    cv.q_off = poff;
+    if (enc_i8(e)) poff += align_up((size_t)(2 + cv.d.c_out) * 4);
   }
   e->param_bytes = poff;
 }
@@ -116,6 +135,7 @@ struct EWs {
   std::vector<int32_t *> nbr;
   std::vector<uint8_t *> split[2];
   std::vector<float *> f32[2];
+  uint8_t *out16;                  // INT8: the last conv's fp16 image, which dense() scatters
   char *zero_begin, *zero_end;
   size_t bytes;
 };
@@ -142,12 +162,12 @@ static void enc_layout_into(const bevb200_encoder *e, const std::vector<int> &ca
     w->f32[s].assign(nl, nullptr);
     if (!feature_buffers) continue;
     for (size_t l = 0; l < nl; ++l) {
-      const size_t row = (size_t)e->levels[l].c_max * enc_img_bytes(e);
-      w->split[s][l] = a.take<uint8_t>((size_t)caps[l] * row);
-      // FP16: dense() scatters the last conv's fp16 image, and residuals are read from images: no fp32 rows
-      if (!enc_f16(e)) w->f32[s][l] = a.take<float>((size_t)caps[l] * e->levels[l].c_max);
+      w->split[s][l] = a.take<uint8_t>((size_t)caps[l] * enc_level_row_bytes(e, l));
+      // FP16, INT8: dense() scatters the last conv's fp16 image, and residuals are read from images: no fp32 rows
+      if (!enc_f16(e) && !enc_i8(e)) w->f32[s][l] = a.take<float>((size_t)caps[l] * e->levels[l].c_max);
     }
   }
+  w->out16 = feature_buffers && enc_i8(e) ? a.take<uint8_t>((size_t)caps[nl - 1] * e->convs.back().d.c_out * 2) : nullptr;
   w->bytes = a.off;
 }
 
@@ -343,8 +363,10 @@ void bevb200_encoder_destroy(bevb200_encoder_t *e) {
 
 int bevb200_encoder_set_precision(bevb200_encoder_t *e, int precision) {
   BEVB200_REQUIRE(e, "null plan");
-  BEVB200_REQUIRE(precision == BEVB200_PREC_BF16X3 || precision == BEVB200_PREC_FP16,
-                  "an encoder plan runs BEVB200_PREC_BF16X3 or BEVB200_PREC_FP16");
+  BEVB200_REQUIRE(precision == BEVB200_PREC_BF16X3 || precision == BEVB200_PREC_FP16 || precision == BEVB200_PREC_INT8,
+                  "an encoder plan runs BEVB200_PREC_BF16X3, BEVB200_PREC_FP16 or BEVB200_PREC_INT8");
+  if (precision == BEVB200_PREC_INT8)   // every stored activation is >= 0: the u8 images
+    for (const EConv &cv : e->convs) BEVB200_REQUIRE(cv.d.relu, "an INT8 plan needs a ReLU after every conv");
   e->precision = precision;
   enc_param_layout(e);
   return BEVB200_OK;
@@ -366,6 +388,7 @@ int bevb200_encoder_output_shape(const bevb200_encoder_t *e, int32_t *shape_out,
 int bevb200_encoder_set_conv(bevb200_encoder_t *e, int conv, const float *weight, const float *scale,
                              const float *shift, void *params, size_t params_bytes, void *stream) {
   BEVB200_REQUIRE(e && conv >= 0 && conv < (int)e->convs.size(), "bad conv index");
+  BEVB200_REQUIRE(!enc_i8(e), "an INT8 plan packs its convs with bevb200_encoder_set_conv_int8");
   BEVB200_REQUIRE(weight && params && params_bytes >= e->param_bytes, "null argument / parameter buffer too small");
   EConv &cv = e->convs[conv];
   cudaStream_t st = (cudaStream_t)stream;
@@ -378,6 +401,49 @@ int bevb200_encoder_set_conv(bevb200_encoder_t *e, int conv, const float *weight
     BEVB200_CUDA(cudaMemcpyAsync(base + cv.scale_off, scale, (size_t)cv.d.c_out * 4, cudaMemcpyDeviceToDevice, st));
   if (shift)
     BEVB200_CUDA(cudaMemcpyAsync(base + cv.shift_off, shift, (size_t)cv.d.c_out * 4, cudaMemcpyDeviceToDevice, st));
+  return BEVB200_OK;
+}
+
+}  // extern "C"
+
+// INT8 epilogue parameters of one conv: a[c] = bn_scale[c] (the first conv) or fl(fl(s_in * s_w[c]) * bn_scale[c])
+// (bn_scale = 1 when absent), the shift (0 when absent), r_out = fl(1 / s_out) and s_res
+__global__ void enc_i8_epilogue_kernel(const float *__restrict__ bn_scale, const float *__restrict__ shift, int c_out,
+                                       int first, float s_in, float s_out, float s_res, float *__restrict__ a,
+                                       float *__restrict__ shift_out, float *__restrict__ q) {
+  const float *s_w = q + 2;
+  for (int c = threadIdx.x; c < c_out; c += blockDim.x) {
+    const float sc = bn_scale ? bn_scale[c] : 1.f;
+    a[c] = first ? sc : __fmul_rn(__fmul_rn(s_in, s_w[c]), sc);
+    shift_out[c] = shift ? shift[c] : 0.f;
+  }
+  if (threadIdx.x == 0) {
+    q[0] = __fdiv_rn(1.f, s_out);
+    q[1] = s_res;
+  }
+}
+
+extern "C" {
+
+int bevb200_encoder_set_conv_int8(bevb200_encoder_t *e, int conv, const float *weight, const float *scale,
+                                  const float *shift, float s_in, float s_out, float s_res, void *params,
+                                  size_t params_bytes, void *stream) {
+  BEVB200_REQUIRE(e && conv >= 0 && conv < (int)e->convs.size(), "bad conv index");
+  BEVB200_REQUIRE(enc_i8(e), "bevb200_encoder_set_conv_int8 needs a plan set to BEVB200_PREC_INT8");
+  BEVB200_REQUIRE(weight && params && params_bytes >= e->param_bytes, "null argument / parameter buffer too small");
+  EConv &cv = e->convs[conv];
+  auto scale_ok = [](float s) { return s > 0.f && s <= 3.4e38f; };
+  BEVB200_REQUIRE(scale_ok(s_out) && (conv == 0 || scale_ok(s_in)) && (cv.d.residual_from < 0 || scale_ok(s_res)),
+                  "activation scales must be finite and > 0");
+  cudaStream_t st = (cudaStream_t)stream;
+  char *base = (char *)params;
+  float *q = (float *)(base + cv.q_off);
+  int rc = conv == 0 ? spconv_v6_pack_weights_f16(weight, cv.d.c_in, cv.d.c_out, cv.kvol, base + cv.packed_off, st)
+                     : spconv_v6_pack_weights_i8(weight, cv.d.c_in, cv.d.c_out, cv.kvol, q + 2, base + cv.packed_off, st);
+  if (rc) return rc;
+  BEVB200_LAUNCH(enc_i8_epilogue_kernel, 1, 128, 0, st, scale, shift, cv.d.c_out, conv == 0 ? 1 : 0, s_in, s_out,
+                 cv.d.residual_from >= 0 ? s_res : 0.f, (float *)(base + cv.scale_off), (float *)(base + cv.shift_off), q);
+  cv.has_scale = cv.has_shift = true;
   return BEVB200_OK;
 }
 
@@ -401,15 +467,17 @@ size_t bevb200_encoder_workspace_bytes(const bevb200_encoder_t *e, int max_voxel
 
 }  // extern "C"
 
-// bevb200_encoder_forward(_f16): voxel_features and dense_out are fp32 (BF16x3 plan) or fp16 (FP16 plan)
+// bevb200_encoder_forward(_f16): voxel_features and dense_out are fp32 (BF16x3 plan) or fp16 (FP16 and INT8 plans)
 static int enc_forward(bevb200_encoder_t *e, bool f16, const void *params, const void *voxel_features,
                        const int32_t *coors, int max_voxels, const int32_t *n_voxels_dev, int batch_size,
                        const int32_t *user_caps, void *dense_out, long long out_batch_stride, int32_t *status_dev,
                        void *workspace, size_t workspace_bytes, void *stream, void *rulebook_stream) {
   // the precision first: a call of the wrong family is refused before any other argument is looked at
   BEVB200_REQUIRE(e, "null plan");
-  BEVB200_REQUIRE(enc_f16(e) == f16, f16 ? "the _f16 calls need a plan set to BEVB200_PREC_FP16"
-                                         : "an fp16 plan runs the _f16 calls");
+  BEVB200_REQUIRE((enc_f16(e) || enc_i8(e)) == f16,
+                  f16 ? "the _f16 calls need a plan set to BEVB200_PREC_FP16 or BEVB200_PREC_INT8"
+                      : "fp16 and INT8 plans run the _f16 calls");
+  const bool i8 = enc_i8(e);
   BEVB200_REQUIRE(e && params && dense_out && status_dev && max_voxels > 0 && batch_size > 0, "bad argument");
   BEVB200_REQUIRE(voxel_features && coors, "null input");
   cudaStream_t st = (cudaStream_t)stream, ss = rulebook_stream ? (cudaStream_t)rulebook_stream : st;
@@ -451,7 +519,9 @@ static int enc_forward(bevb200_encoder_t *e, bool f16, const void *params, const
     const size_t lo = cv.level_out;
     const bool last = i + 1 == e->convs.size();
     uint8_t *osplit = nullptr;
-    if (!last || f16) {   // FP16: the last conv's image is what dense() scatters
+    if (i8 && last) {
+      osplit = w.out16;
+    } else if (!last || f16) {   // FP16: the last conv's image is what dense() scatters
       osplit = w.split[split_turn[lo]][lo];
       split_turn[lo] ^= 1;
     }
@@ -466,7 +536,13 @@ static int enc_forward(bevb200_encoder_t *e, bool f16, const void *params, const
     const float *res = cv.d.residual_from >= 0 ? f32_of[cv.d.residual_from] : nullptr;
     const uint8_t *res_split = (cv.d.residual_from >= 0 && res == nullptr) ? split_of[cv.d.residual_from] : nullptr;
     BEVB200_REQUIRE(cv.d.residual_from < 0 || res || res_split, "residual source has no rows");
-    rc = (f16 ? spconv_v6_forward_f16 : spconv_v6_forward)(
+    if (i8)
+      rc = spconv_v6_forward_i8(cur_split, i == 0, pbase + cv.packed_off, w.nbr[cv.rulebook], (long long)caps[lo],
+                                caps[cv.level_in], caps[lo], w.counts[lo], cv.c_in_eff, cv.d.c_out, cv.kvol,
+                                (const float *)(pbase + cv.scale_off), (const float *)(pbase + cv.shift_off),
+                                (const float *)(pbase + cv.q_off), res_split, cv.d.relu, last, osplit, st);
+    else
+      rc = (f16 ? spconv_v6_forward_f16 : spconv_v6_forward)(
         cur_split, pbase + cv.packed_off, w.nbr[cv.rulebook], (long long)caps[lo], caps[cv.level_in], caps[lo],
         w.counts[lo], cv.c_in_eff, cv.d.c_out, cv.kvol, cv.has_scale ? (const float *)(pbase + cv.scale_off) : nullptr,
         cv.has_shift ? (const float *)(pbase + cv.shift_off) : nullptr, res, res_split, cv.d.relu, of32, osplit, st);
@@ -914,7 +990,7 @@ extern "C" {
 
 size_t bevb200_encoder_train_state_bytes(const bevb200_encoder_t *e, int max_voxels, int batch_size,
                                          const int32_t *user_caps) {
-  if (!e || max_voxels <= 0 || batch_size <= 0) return 0;
+  if (!e || enc_i8(e) || max_voxels <= 0 || batch_size <= 0) return 0;
   std::vector<int> caps;
   level_caps(e, max_voxels, batch_size, user_caps, &caps);
   ETrain t;
@@ -923,7 +999,9 @@ size_t bevb200_encoder_train_state_bytes(const bevb200_encoder_t *e, int max_vox
 
 int bevb200_encoder_train_saved(const bevb200_encoder_t *e, int max_voxels, int batch_size, const int32_t *user_caps,
                                 int conv, size_t *pre_bn_offset, size_t *out_image_offset) {
-  BEVB200_REQUIRE(e && max_voxels > 0 && batch_size > 0 && pre_bn_offset && out_image_offset, "bad argument");
+  BEVB200_REQUIRE(e, "null plan");
+  BEVB200_REQUIRE(!enc_i8(e), "an INT8 plan has no training path (eval forward only)");
+  BEVB200_REQUIRE(max_voxels > 0 && batch_size > 0 && pre_bn_offset && out_image_offset, "bad argument");
   BEVB200_REQUIRE(conv >= 0 && conv < (int)e->convs.size(), "bad conv index");
   std::vector<int> caps;
   level_caps(e, max_voxels, batch_size, user_caps, &caps);
@@ -945,6 +1023,7 @@ static int enc_forward_train(bevb200_encoder_t *e, bool f16, const float *const 
                              void *stream, void *rulebook_stream) {
   // the precision first: a call of the wrong family is refused before any other argument is looked at
   BEVB200_REQUIRE(e, "null plan");
+  BEVB200_REQUIRE(!enc_i8(e), "an INT8 plan has no training path (eval forward only)");
   BEVB200_REQUIRE(enc_f16(e) == f16, f16 ? "the _f16 calls need a plan set to BEVB200_PREC_FP16"
                                          : "an fp16 plan runs the _f16 calls");
   BEVB200_REQUIRE(e && weights && bn && dense_out && status_dev && max_voxels > 0 && batch_size > 0, "bad argument");
@@ -1050,7 +1129,7 @@ int bevb200_encoder_forward_train_f16(bevb200_encoder_t *e, const float *const *
 
 size_t bevb200_encoder_backward_workspace_bytes(const bevb200_encoder_t *e, int max_voxels, int batch_size,
                                                 const int32_t *user_caps) {
-  if (!e || max_voxels <= 0 || batch_size <= 0) return 0;
+  if (!e || enc_i8(e) || max_voxels <= 0 || batch_size <= 0) return 0;
   std::vector<int> caps;
   level_caps(e, max_voxels, batch_size, user_caps, &caps);
   EBwd b;
@@ -1066,6 +1145,7 @@ static int enc_backward(const bevb200_encoder_t *e, bool f16, const float *const
                         void *workspace, size_t workspace_bytes, void *stream) {
   // the precision first: a call of the wrong family is refused before any other argument is looked at
   BEVB200_REQUIRE(e, "null plan");
+  BEVB200_REQUIRE(!enc_i8(e), "an INT8 plan has no training path (eval forward only)");
   BEVB200_REQUIRE(enc_f16(e) == f16, f16 ? "the _f16 calls need a plan set to BEVB200_PREC_FP16"
                                          : "an fp16 plan runs the _f16 calls");
   BEVB200_REQUIRE(e && weights && state && grad_dense && grad_weights && grad_bn_weight && grad_bn_bias &&

@@ -63,6 +63,18 @@ int spconv_v6_forward_f16(const void *rows, const void *packed, const int32_t *n
                           int n_out, const int32_t *n_out_dev, int c_in, int c_out, int kvol, const float *scale,
                           const float *shift, const float *residual, const void *residual_f16, int relu, float *out,
                           void *out_f16, cudaStream_t st);
+// INT8 (BEVB200_PREC_INT8, the encoder plan only): the weight image (K blocks of 128 s8 channels; the per-output-channel
+// scales s_w [c_out] are written to s_w) and the forward on a u8 row image [n, c_in] (f16_rows: an fp16 image, read by
+// the FP16 MMA).  The epilogue (spconv_v6.cu: v6_store_chunk_q8) takes a = the per-channel factor of the accumulator,
+// shift, qparams = device [r_out, s_res] and a u8 residual image [n_out, c_out]; it writes a u8 image or, out_half,
+// the fp16 image [n_out, c_out].
+size_t spconv_v6_packed_bytes_i8(int c_in, int c_out, int kvol);
+int spconv_v6_pack_weights_i8(const float *weight, int c_in, int c_out, int kvol, float *s_w, void *packed,
+                              cudaStream_t st);
+int spconv_v6_forward_i8(const void *rows, bool f16_rows, const void *packed, const int32_t *nbr, long long nbr_stride,
+                         int n_in, int n_out, const int32_t *n_out_dev, int c_in, int c_out, int kvol, const float *a,
+                         const float *shift, const float *qparams, const void *residual_u8, int relu, bool out_half,
+                         void *out_image, cudaStream_t st);
 // TF32 (tf32x3 = false) / 3xTF32 forward on fp32 rows [n_in][c_in], c_in a power of two 8 .. 128
 int spconv_v6_forward_tf32(const float *rows, const void *packed, const int32_t *nbr, int n_in, int n_out, int c_in,
                            int c_out, int kvol, bool tf32x3, const float *scale, const float *shift,

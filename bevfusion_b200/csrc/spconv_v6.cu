@@ -15,6 +15,11 @@
 //     as c_eff / 2 four-byte units, so a K block is 64 channels, the gather and the swizzle are those of the other
 //     modes, and a 16-channel step is one fp16 MMA (the products are exact in the fp32 accumulator).  The epilogue
 //     rounds once to fp16 (round to nearest, overflow to inf) and writes the fp16 image; a residual is read from one.
+//   * INT8 (modes 4 and 5, the encoder plan's BEVB200_PREC_INT8): a row is c_eff u8 channels, c_eff / 4 four-byte
+//     units, so a K block is 128 channels and a k32 step of 8-bit values is the 32 B a k16 step of fp16 reads: the
+//     fragments, the ldmatrix loads (no .trans: the weight image is K-major) and the wgmma descriptors are those of
+//     FP16.  Mode 4 multiplies u8 rows by s8 weights into exact int32 accumulators; mode 5 is the FP16 MMA on fp16
+//     rows (the chain's first conv).  Both end in the quantising epilogue of v6_store_chunk_q8.
 // A CTA (8 warps, two CTAs per SM) owns 128-row output tiles, persistent over the tiles; per K block all 256
 // threads gather the 128 neighbour rows with 16-byte cp.async (zero fill for missing neighbours) into an XOR-
 // swizzled tile (16-byte chunk c of row r at (c ^ (r & 7)): conflict-free ldmatrix) and copy the weight block
@@ -24,6 +29,8 @@
 // rows and / or the split image) runs once through a shared-memory transpose.  The number of output rows may be
 // read from device memory (n_out_dev), so a strided conv needs no host round trip and the whole encoder can be
 // captured in a CUDA graph.
+#include <type_traits>
+
 #include "spconv.cuh"
 #include "tc_ptx.cuh"
 
@@ -48,6 +55,68 @@ struct V6Params {
   int c_in, c_out, kvol, relu;
   int nkb, cin_shift;
 };
+// The INT8 instances' parameters (a separate type: the other instances' parameter block, and so their code, is unchanged)
+struct V6ParamsQ8 : V6Params {
+  const float *qparams;         // [r_out, s_res] on the device
+  int out_half;                 // out_split is an fp16 image (the chain's last conv), not u8
+};
+
+// MMA mode of an instance: 0 BF16x3, 1 TF32, 2 3xTF32, 3 FP16, 4 u8 x s8 (INT8), 5 FP16 with the INT8 epilogue
+template <int MODE>
+using v6_acc_t = typename std::conditional<MODE == 4, int, float>::type;
+template <int MODE>
+using v6_params_t = typename std::conditional<MODE >= 4, V6ParamsQ8, V6Params>::type;
+
+// INT8 epilogue of 16 channels [c0, c0 + 16) of one row; fl() is one fp32 round-to-nearest op (no contraction):
+//   v = fl(fl(acc * a[c]) + shift[c]);  v = fl(v + fl(float(res_u8) * s_res));  v = max(v, 0)
+//   u8 image: q = clamp(rint(fl(v * r_out)), 0, 255) (NaN -> 0, +inf -> 255);  fp16 image: half(v)
+// The residual image may be this launch's own out_split (a lane reads its 16 bytes before it writes them).
+__device__ __forceinline__ void v6_store_chunk_q8(const V6ParamsQ8 &p, const float (&acc)[16], int orow, int c0) {
+  const int c_out = p.c_out;
+  float y[16];
+#pragma unroll
+  for (int e = 0; e < 16; ++e) y[e] = __fadd_rn(__fmul_rn(acc[e], __ldg(p.scale + c0 + e)), __ldg(p.shift + c0 + e));
+  if (p.residual_split) {
+    const float s_res = __ldg(p.qparams + 1);
+    const uint4 h = *reinterpret_cast<const uint4 *>(p.residual_split + (long long)orow * c_out + c0);
+    const uint32_t hw[4] = {h.x, h.y, h.z, h.w};
+#pragma unroll
+    for (int e = 0; e < 16; ++e)
+      y[e] = __fadd_rn(y[e], __fmul_rn((float)((hw[e >> 2] >> (8 * (e & 3))) & 0xffu), s_res));
+  }
+  if (p.relu) {
+#pragma unroll
+    for (int e = 0; e < 16; ++e) y[e] = fmaxf(y[e], 0.f);
+  }
+  if (p.out_half) {
+    uint32_t h[8];
+#pragma unroll
+    for (int e = 0; e < 16; e += 2) {
+      const __half2 v = __floats2half2_rn(y[e], y[e + 1]);
+      h[e / 2] = *reinterpret_cast<const uint32_t *>(&v);
+    }
+    uint4 *row = reinterpret_cast<uint4 *>(p.out_split + ((long long)orow * c_out + c0) * 2);
+    row[0] = make_uint4(h[0], h[1], h[2], h[3]);
+    row[1] = make_uint4(h[4], h[5], h[6], h[7]);
+  } else {
+    const float r_out = __ldg(p.qparams);
+    uint32_t q[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+    for (int e = 0; e < 16; ++e) {
+      // fmaxf first: NaN -> 0; the clamp to [0, 255] commutes with rint at these integer bounds
+      const float t = fminf(fmaxf(__fmul_rn(y[e], r_out), 0.f), 255.f);
+      q[e >> 2] |= (uint32_t)__float2int_rn(t) << (8 * (e & 3));
+    }
+    *reinterpret_cast<uint4 *>(p.out_split + (long long)orow * c_out + c0) = make_uint4(q[0], q[1], q[2], q[3]);
+  }
+}
+
+// one 16-bit k16 / 8-bit k32 MMA of the FP16 (3, 5) and INT8 (4) modes
+template <int MODE>
+__device__ __forceinline__ void v6_mma_k32b(v6_acc_t<MODE> (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  if constexpr (MODE == 4) mma_u8s8_16832(d, a, b0, b1);
+  else mma_f16_16816(d, a, b0, b1);
+}
 
 // Epilogue of NC (8 or 16) consecutive channels [c0, c0 + NC) of one row: folded BN, residual, ReLU,
 // then the fp32 row and / or its split image.  NC channels = NC/8 16-byte chunks of hi and of lo.
@@ -145,7 +214,7 @@ struct V6Shape {
 };
 
 template <int MODE, int COUT>
-__global__ void __launch_bounds__(kV6Threads, 2) spconv_v6_kernel(const V6Params p) {
+__global__ void __launch_bounds__(kV6Threads, 2) spconv_v6_kernel(const v6_params_t<MODE> p) {
   using Sh = V6Shape<MODE, COUT>;
   constexpr int S = Sh::kStages, kB = Sh::kB, kStage = Sh::kStage;
   constexpr int NT = COUT / 16;                   // n8 tiles per warp (the two warp halves split the columns)
@@ -197,13 +266,13 @@ __global__ void __launch_bounds__(kV6Threads, 2) spconv_v6_kernel(const V6Params
       for (int i = tid; i < kB / 16; i += kV6Threads) cp_async16(b + (uint32_t)i * 16u, src + (size_t)i * 16);
     };
 
-    float acc[2][NT][4];
+    v6_acc_t<MODE> acc[2][NT][4];
 #pragma unroll
     for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
       for (int nt = 0; nt < NT; ++nt)
 #pragma unroll
-        for (int e = 0; e < 4; ++e) acc[mt][nt][e] = 0.f;
+        for (int e = 0; e < 4; ++e) acc[mt][nt][e] = 0;
 
     int nidx[4];
 #pragma unroll
@@ -264,8 +333,9 @@ __global__ void __launch_bounds__(kV6Threads, 2) spconv_v6_kernel(const V6Params
             }
           }
         }
-      } else if constexpr (MODE == 3) {
-        // four k16 steps of 16 fp16 channels: chunks 2 ks, 2 ks + 1 (not unrolled at Cout 128: it would spill)
+      } else if constexpr (MODE >= 3) {
+        // four k16 steps of 16 fp16 channels (INT8: k32 steps of 32 u8 channels): chunks 2 ks, 2 ks + 1 (not
+        // unrolled at Cout 128: it would spill)
 #pragma unroll(COUT == 128 ? 1 : 4)
         for (int ks = 0; ks < 4; ++ks) {
           uint32_t af[2][4];
@@ -280,7 +350,7 @@ __global__ void __launch_bounds__(kV6Threads, 2) spconv_v6_kernel(const V6Params
             uint32_t bf[2];
             ldsm_x2(b + (uint32_t)(n * 128 + ((lc ^ (n & 7)) << 4)), bf);
 #pragma unroll
-            for (int mt = 0; mt < 2; ++mt) mma_f16_16816(acc[mt][0], af[mt], bf[0], bf[1]);
+            for (int mt = 0; mt < 2; ++mt) v6_mma_k32b<MODE>(acc[mt][0], af[mt], bf[0], bf[1]);
           } else {
 #pragma unroll
             for (int nt = 0; nt < NT; nt += 2) {
@@ -290,7 +360,7 @@ __global__ void __launch_bounds__(kV6Threads, 2) spconv_v6_kernel(const V6Params
 #pragma unroll
               for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
-                for (int h = 0; h < 2; ++h) mma_f16_16816(acc[mt][nt + h], af[mt], bf[2 * h], bf[2 * h + 1]);
+                for (int h = 0; h < 2; ++h) v6_mma_k32b<MODE>(acc[mt][nt + h], af[mt], bf[2 * h], bf[2 * h + 1]);
             }
           }
         }
@@ -352,9 +422,10 @@ __global__ void __launch_bounds__(kV6Threads, 2) spconv_v6_kernel(const V6Params
     for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
       for (int nt = 0; nt < NT; ++nt) {
+        // INT8: float(acc), rounded to nearest (exact below 2^24)
         const int r = wm + 16 * mt + (lane >> 2), c = wn + nt * 8 + 2 * (lane & 3);
-        *reinterpret_cast<float2 *>(cs + r * LD + c) = make_float2(acc[mt][nt][0], acc[mt][nt][1]);
-        *reinterpret_cast<float2 *>(cs + (r + 8) * LD + c) = make_float2(acc[mt][nt][2], acc[mt][nt][3]);
+        *reinterpret_cast<float2 *>(cs + r * LD + c) = make_float2((float)acc[mt][nt][0], (float)acc[mt][nt][1]);
+        *reinterpret_cast<float2 *>(cs + (r + 8) * LD + c) = make_float2((float)acc[mt][nt][2], (float)acc[mt][nt][3]);
       }
     __syncthreads();
     constexpr int kChunks = COUT / 16;
@@ -368,7 +439,8 @@ __global__ void __launch_bounds__(kV6Threads, 2) spconv_v6_kernel(const V6Params
           const float4 q = *reinterpret_cast<const float4 *>(cs + r * LD + 16 * j + e);
           v[e] = q.x; v[e + 1] = q.y; v[e + 2] = q.z; v[e + 3] = q.w;
         }
-        v6_store_chunk<16, MODE == 3>(p, v, orow, 16 * j);
+        if constexpr (MODE >= 4) v6_store_chunk_q8(p, v, orow, 16 * j);
+        else v6_store_chunk<16, MODE == 3>(p, v, orow, 16 * j);
       }
     }
     __syncthreads();                         // the transpose area is the next tile's ring
@@ -416,9 +488,9 @@ __device__ __forceinline__ void wgmma_nc(float (&d)[COUT / 2], uint64_t da, uint
   else wgmma_n128<F16>(d, da, db, accumulate);
 }
 
-// MODE 0 (BF16x3) or 3 (FP16)
+// MODE 0 (BF16x3), 3 (FP16), 4 (INT8) or 5 (FP16 with the INT8 epilogue)
 template <int MODE, int COUT>
-__global__ void __launch_bounds__(kWgThreads, 1) spconv_wg_kernel(const V6Params p) {
+__global__ void __launch_bounds__(kWgThreads, 1) spconv_wg_kernel(const v6_params_t<MODE> p) {
   using Sh = WgShape<COUT>;
   constexpr int S = Sh::kStages, MT = Sh::kMT, TM = Sh::kTileM;
   extern __shared__ uint8_t smem_raw[];
@@ -492,7 +564,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) spconv_wg_kernel(const V6Params
     // ------------------------------------ consumers -----------------------------------------------
     setmaxnreg_inc<232>();
     const int cw = wg - 1, warp = (tid >> 5) & 3;
-    float acc[MT][COUT / 2];
+    v6_acc_t<MODE> acc[MT][COUT / 2];
     uint32_t it = 0;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
       for (int kb = 0; kb < nkb; ++kb, ++it) {
@@ -502,13 +574,17 @@ __global__ void __launch_bounds__(kWgThreads, 1) spconv_wg_kernel(const V6Params
         fence_proxy_async_smem();
         wgmma_fence();
         const uint32_t a = smem + s * Sh::kStage + cw * (MT * 64 * 128), b = smem + s * Sh::kStage + Sh::kA;
-        if constexpr (MODE == 3) {
+        if constexpr (MODE >= 3) {
 #pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {  // the four k16 slices of the 64-channel K block, A and W alike
+          for (int ks = 0; ks < 4; ++ks) {  // the four k16 (INT8: k32) slices of the K block, A and W alike
             const uint64_t bd = wgmma_desc_sw128(b + 32 * ks);
 #pragma unroll
-            for (int m = 0; m < MT; ++m)
-              wgmma_nc<true, COUT>(acc[m], wgmma_desc_sw128(a + m * (64 * 128) + 32 * ks), bd, kb > 0 || ks > 0);
+            for (int m = 0; m < MT; ++m) {
+              const uint64_t ad = wgmma_desc_sw128(a + m * (64 * 128) + 32 * ks);
+              if constexpr (MODE != 4) wgmma_nc<true, COUT>(acc[m], ad, bd, kb > 0 || ks > 0);
+              else if constexpr (COUT == 64) wgmma_n64_i8(acc[m], ad, bd, kb > 0 || ks > 0);
+              else wgmma_n128_i8(acc[m], ad, bd, kb > 0 || ks > 0);
+            }
           }
         } else {
 #pragma unroll
@@ -544,8 +620,8 @@ __global__ void __launch_bounds__(kWgThreads, 1) spconv_wg_kernel(const V6Params
 #pragma unroll
           for (int i = 0; i < SW / 8; ++i) {
             const int r = lane >> 2, c = 8 * i + 2 * (lane & 3), q = 4 * (c0 / 8 + i);
-            *reinterpret_cast<float2 *>(buf + r * LD + c) = make_float2(acc[m][q], acc[m][q + 1]);
-            *reinterpret_cast<float2 *>(buf + (r + 8) * LD + c) = make_float2(acc[m][q + 2], acc[m][q + 3]);
+            *reinterpret_cast<float2 *>(buf + r * LD + c) = make_float2((float)acc[m][q], (float)acc[m][q + 1]);
+            *reinterpret_cast<float2 *>(buf + (r + 8) * LD + c) = make_float2((float)acc[m][q + 2], (float)acc[m][q + 3]);
           }
           __syncwarp();
           const int r = lane / CH, j = lane % CH;
@@ -556,7 +632,8 @@ __global__ void __launch_bounds__(kWgThreads, 1) spconv_wg_kernel(const V6Params
               const float4 q = *reinterpret_cast<const float4 *>(buf + r * LD + 16 * j + e);
               v[e] = q.x; v[e + 1] = q.y; v[e + 2] = q.z; v[e + 3] = q.w;
             }
-            v6_store_chunk<16, MODE == 3>(p, v, rbase + r, c0 + 16 * j);
+            if constexpr (MODE >= 4) v6_store_chunk_q8(p, v, rbase + r, c0 + 16 * j);
+            else v6_store_chunk<16, MODE == 3>(p, v, rbase + r, c0 + 16 * j);
           }
           __syncwarp();
         }
@@ -657,6 +734,34 @@ __global__ void spconv_v6_pack_f16_kernel(const float *__restrict__ w, int kvol,
   }
 }
 
+// Per-output-channel weight scale of the INT8 form: s_w[n] = fl(max |W[.., .., n]| / 127), or 1 when that max is 0
+__global__ void spconv_v6_i8_scales_kernel(const float *__restrict__ w, int kvol, int c_in, int c_out,
+                                           float *__restrict__ s_w) {
+  for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < c_out; n += gridDim.x * blockDim.x) {
+    float m = 0.f;
+    for (long long t = 0; t < (long long)kvol * c_in; ++t) m = fmaxf(m, fabsf(w[t * c_out + n]));
+    s_w[n] = m > 0.f ? __fdiv_rn(m, 127.f) : 1.f;
+  }
+}
+
+// Weight image of the INT8 form: one stage (Cout rows of 128 B) per 128-wide K block, row n = q_w of kk 0-127 with
+// q_w = clamp(rint(fl(W / s_w[n])), -127, 127) (ties to even), SWIZZLE_128B (16-byte chunk kk / 16 at (kk / 16) ^ (n & 7)).
+__global__ void spconv_v6_pack_i8_kernel(const float *__restrict__ w, const float *__restrict__ s_w, int kvol,
+                                         int c_in, int c_in_eff, int c_out, int nkb, int8_t *__restrict__ packed) {
+  const long long total = (long long)nkb * c_out * 128;
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total;
+       t += (long long)gridDim.x * blockDim.x) {
+    const int cc = (int)(t % 128);
+    const int n = (int)((t / 128) % c_out);
+    const int kb = (int)(t / (128ll * c_out));
+    const int kk = kb * 128 + cc;
+    const int k = kk / c_in_eff, ci = kk % c_in_eff;
+    const float v = (k < kvol && ci < c_in) ? w[((long long)k * c_in + ci) * c_out + n] : 0.f;
+    const float x = fminf(fmaxf(__fdiv_rn(v, __ldg(s_w + n)), -127.f), 127.f);
+    packed[((long long)kb * c_out + n) * 128 + ((((cc >> 4) ^ (n & 7)) << 4) | (cc & 15))] = (int8_t)__float2int_rn(x);
+  }
+}
+
 int spconv_v6_cin_eff(int c_in) {
   for (int e = 16; e <= 128; e <<= 1)
     if (c_in <= e) return e;
@@ -678,6 +783,24 @@ static int v6_nkb_f16(int c_eff, int kvol) { return v6_nkb(c_eff / 2, kvol); }
 size_t spconv_v6_packed_bytes_f16(int c_in, int c_out, int kvol) {
   if (!spconv_v6_shape_ok(c_in, c_out, kvol)) return 0;
   return (size_t)v6_nkb_f16(spconv_v6_cin_eff(c_in), kvol) * c_out * 128;
+}
+
+// K blocks of 128 u8 channels = 32 four-byte units
+static int v6_nkb_i8(int c_eff, int kvol) { return v6_nkb(c_eff / 4, kvol); }
+
+size_t spconv_v6_packed_bytes_i8(int c_in, int c_out, int kvol) {
+  if (!spconv_v6_shape_ok(c_in, c_out, kvol)) return 0;
+  return (size_t)v6_nkb_i8(spconv_v6_cin_eff(c_in), kvol) * c_out * 128;
+}
+
+int spconv_v6_pack_weights_i8(const float *weight, int c_in, int c_out, int kvol, float *s_w, void *packed,
+                              cudaStream_t st) {
+  const int ce = spconv_v6_cin_eff(c_in);
+  const int nkb = v6_nkb_i8(ce, kvol);
+  BEVB200_LAUNCH(spconv_v6_i8_scales_kernel, (c_out + 127) / 128, 128, 0, st, weight, kvol, c_in, c_out, s_w);
+  BEVB200_LAUNCH(spconv_v6_pack_i8_kernel, grid_for((long long)nkb * c_out * 128, 256), 256, 0, st, weight, s_w, kvol,
+                 c_in, ce, c_out, nkb, (int8_t *)packed);
+  return BEVB200_OK;
 }
 
 int spconv_v6_pack_weights_f16(const float *weight, int c_in, int c_out, int kvol, void *packed, cudaStream_t st) {
@@ -717,8 +840,8 @@ int spconv_v6_split_rows(const float *features, int n_cap, const int32_t *n_dev,
 
 // Both forward kernels launch with programmatic stream serialisation: the launch overlaps the tail of the previous
 // kernel in the stream (21 back-to-back convs per frame), and the kernel waits for its results (griddepcontrol.wait).
-static int v6_launch_kernel(void (*kernel)(V6Params), int grid, int threads, int smem, const V6Params &p,
-                            cudaStream_t st) {
+template <typename P>
+static int v6_launch_kernel(void (*kernel)(P), int grid, int threads, int smem, const P &p, cudaStream_t st) {
   BEVB200_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
@@ -737,14 +860,14 @@ static int v6_launch_kernel(void (*kernel)(V6Params), int grid, int threads, int
 }
 
 template <int MODE, int COUT>
-static int v6_launch_one(const V6Params &p, cudaStream_t st) {
+static int v6_launch_one(const v6_params_t<MODE> &p, cudaStream_t st) {
   const int n_tiles = (p.n_out + kV6TileM - 1) / kV6TileM;
   return v6_launch_kernel(spconv_v6_kernel<MODE, COUT>, n_tiles < 2 * kNumSMs ? n_tiles : 2 * kNumSMs, kV6Threads,
                           V6Shape<MODE, COUT>::kSmem, p, st);
 }
 
 template <int MODE>
-static int v6_launch(const V6Params &p, cudaStream_t st) {
+static int v6_launch(const v6_params_t<MODE> &p, cudaStream_t st) {
   switch (p.c_out) {
     case 16: return v6_launch_one<MODE, 16>(p, st);
     case 32: return v6_launch_one<MODE, 32>(p, st);
@@ -755,7 +878,7 @@ static int v6_launch(const V6Params &p, cudaStream_t st) {
 }
 
 template <int MODE, int COUT>
-static int wg_launch_one(const V6Params &p, cudaStream_t st) {
+static int wg_launch_one(const v6_params_t<MODE> &p, cudaStream_t st) {
   using Sh = WgShape<COUT>;
   const int n_tiles = (p.n_out + Sh::kTileM - 1) / Sh::kTileM;
   return v6_launch_kernel(spconv_wg_kernel<MODE, COUT>, n_tiles < kNumSMs ? n_tiles : kNumSMs, kWgThreads, Sh::kSmem,
@@ -763,7 +886,7 @@ static int wg_launch_one(const V6Params &p, cudaStream_t st) {
 }
 
 template <int MODE>
-static int wg_launch(const V6Params &p, cudaStream_t st) {
+static int wg_launch(const v6_params_t<MODE> &p, cudaStream_t st) {
   switch (p.c_out) {
     case 64: return wg_launch_one<MODE, 64>(p, st);
     case 128: return wg_launch_one<MODE, 128>(p, st);
@@ -833,6 +956,29 @@ int spconv_v6_forward_f16(const void *rows, const void *packed, const int32_t *n
   p.out_split = (uint8_t *)out_f16;
   // the same layers as BF16x3 take the wgmma kernel: >= kWgMinKBlocks K blocks of 32 channels (half as many fp16 blocks)
   return p.c_out >= 64 && v6_nkb(c_in, kvol) >= kWgMinKBlocks ? wg_launch<3>(p, st) : v6_launch<3>(p, st);
+}
+
+int spconv_v6_forward_i8(const void *rows, bool f16_rows, const void *packed, const int32_t *nbr, long long nbr_stride,
+                         int n_in, int n_out, const int32_t *n_out_dev, int c_in, int c_out, int kvol, const float *a,
+                         const float *shift, const float *qparams, const void *residual_u8, int relu, bool out_half,
+                         void *out_image, cudaStream_t st) {
+  BEVB200_REQUIRE(c_in == spconv_v6_cin_eff(c_in) && spconv_v6_shape_ok(c_in, c_out, kvol), "shape has no tensor-core form");
+  BEVB200_REQUIRE(rows && packed && nbr && a && shift && qparams && out_image, "null argument");
+  BEVB200_REQUIRE((uintptr_t)rows % 16 == 0 && (uintptr_t)out_image % 16 == 0 && (uintptr_t)packed % 16 == 0 &&
+                      (residual_u8 == nullptr || (uintptr_t)residual_u8 % 16 == 0),
+                  "operands must be 16-byte aligned");
+  if (n_out <= 0) return BEVB200_OK;
+  V6ParamsQ8 p;
+  // four-byte units of a row: c_in / 2 fp16 channels (the first conv), c_in / 4 u8 channels
+  v6_common(p, rows, packed, nbr, nbr_stride, n_in, n_out, n_out_dev, f16_rows ? c_in / 2 : c_in / 4, c_out, kvol, a,
+            shift, nullptr, relu, nullptr);
+  p.residual_split = (const uint8_t *)residual_u8;
+  p.out_split = (uint8_t *)out_image;
+  p.qparams = qparams;
+  p.out_half = out_half;
+  // the same layers as BF16x3 take the wgmma kernel: >= kWgMinKBlocks K blocks of 32 channels
+  if (p.c_out >= 64 && v6_nkb(c_in, kvol) >= kWgMinKBlocks) return f16_rows ? wg_launch<5>(p, st) : wg_launch<4>(p, st);
+  return f16_rows ? v6_launch<5>(p, st) : v6_launch<4>(p, st);
 }
 
 // TF32 (tf32x3 = false) / 3xTF32 forward on zero-padded fp32 rows [n_in][c_in] (c_in a power of two, 8 .. 128) and

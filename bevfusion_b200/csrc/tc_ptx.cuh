@@ -71,6 +71,16 @@ __device__ __forceinline__ void mma_f16_16816(float (&d)[4], const uint32_t (&a)
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
+// D += A (16x32 u8, row) x B (32x8 s8, col), exact int32 accumulate.  Both fragments hold the bytes of a 16-bit k16
+// fragment (four 8-bit values per register where there were two 16-bit ones), so the non-transposed ldmatrix loads
+// of the K-major fp16 operands load them unchanged.
+__device__ __forceinline__ void mma_u8s8_16832(int (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k32.row.col.s32.u8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
+      "{%0,%1,%2,%3};"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
 // D += A (16x8 tf32, row) x B (8x8 tf32, col), fp32 accumulate
 __device__ __forceinline__ void mma_tf32_1688(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile(
@@ -137,6 +147,11 @@ __device__ __forceinline__ void wgmma_pin(float (&d)[R]) {
 #pragma unroll
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+template <int R>
+__device__ __forceinline__ void wgmma_pin(int (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+r"(d[i])::"memory");
+}
 
 // D (64 x N fp32, the m64nNk16 register fragment) (+)= A (64 x 16 bf16 / fp16, descriptor) x B (16 x N, same type,
 // descriptor, K-major); accumulate = 0 overwrites D.  F16 picks fp16 operands (one MMA per k16 step of the fp16 path)
@@ -161,7 +176,27 @@ __device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t da, uint64_t
   if constexpr (F16) BEVB200_WGMMA_N128("f16");
   else BEVB200_WGMMA_N128("bf16");
 }
+// D (64 x N int32) (+)= A (64 x 32 u8, descriptor) x B (32 x N s8, descriptor, K-major), exact.  A k32 slice of
+// 8-bit values is 32 B of a row, as a k16 slice of 16-bit ones, so the descriptors are those of the fp16 path.
+#define BEVB200_WGMMA_I8_N64                                                                                         \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"                                                \
+               "wgmma.mma_async.sync.aligned.m64n64k32.s32.u8.s8 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p;\n\t}"     \
+               : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])                                                                                                 \
+               : "l"(da), "l"(db), "r"(accumulate))
+#define BEVB200_WGMMA_I8_N128                                                                                        \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"                                                \
+               "wgmma.mma_async.sync.aligned.m64n128k32.s32.u8.s8 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p;\n\t}"    \
+               : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])                                                                                                 \
+               : "l"(da), "l"(db), "r"(accumulate))
+__device__ __forceinline__ void wgmma_n64_i8(int (&d)[32], uint64_t da, uint64_t db, int accumulate) {
+  BEVB200_WGMMA_I8_N64;
+}
+__device__ __forceinline__ void wgmma_n128_i8(int (&d)[64], uint64_t da, uint64_t db, int accumulate) {
+  BEVB200_WGMMA_I8_N128;
+}
 #undef BEVB200_WGMMA_N64
 #undef BEVB200_WGMMA_N128
+#undef BEVB200_WGMMA_I8_N64
+#undef BEVB200_WGMMA_I8_N128
 
 }  // namespace bevb200

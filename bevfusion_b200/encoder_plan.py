@@ -6,16 +6,17 @@ spconv/conv.py:114-223 (one rulebook build + ~80 launches + one device->host cou
 forward_train() is the same chain in training mode (batch-statistics BatchNorm, running statistics updated
 in place) with a native whole-encoder backward, also sync-free and capturable.
 
-A plan runs one precision: BF16x3 (the default, fp32 rows in and out) or FP16 (fp16 operands with fp32
-accumulation, half rows in and out; the numerical contract is in include/bevfusion_b200.h).  Each plan packs its
-own weight image, so a module keeps one plan per precision."""
+A plan runs one precision: BF16x3 (the default, fp32 rows in and out), FP16 (fp16 operands with fp32
+accumulation, half rows in and out) or INT8 (eval only: u8 activations x s8 weights with int32 accumulation and the
+module's calibrated per-conv scales, half rows in and out); the numerical contracts are in include/bevfusion_b200.h.
+Each plan packs its own weight image, so a module keeps one plan per precision."""
 import ctypes
 
 import torch
 
 from . import _C
 from .sparse_block import SparseBasicBlock, bn_fold_key, bn_scale_shift
-from .spconv.ops import PREC_BF16X3, PREC_FP16
+from .spconv.ops import PREC_BF16X3, PREC_FP16, PREC_INT8
 
 
 class _ConvDesc(ctypes.Structure):
@@ -79,13 +80,16 @@ def supported(encoder):
 
 class EncoderPlan:
     def __init__(self, encoder, precision=PREC_BF16X3):
-        if precision not in (PREC_BF16X3, PREC_FP16):
-            raise ValueError("an encoder plan runs the bf16x3 or the fp16 precision")
+        if precision not in (PREC_BF16X3, PREC_FP16, PREC_INT8):
+            raise ValueError("an encoder plan runs the bf16x3, the fp16 or the int8 precision")
         self.encoder = encoder
         self.precision = precision
         self.f16 = precision == PREC_FP16
-        self.row_dtype = torch.float16 if self.f16 else torch.float32
+        self.i8 = precision == PREC_INT8
+        self.row_dtype = torch.float16 if self.f16 or self.i8 else torch.float32
         self.chain = _chain_of(encoder)
+        if self.i8 and not all(relu for _, _, relu, _ in self.chain):
+            raise ValueError("the int8 plan needs a ReLU after every conv (its activations are stored as u8)")
         L = _C.lib()
         descs = (_ConvDesc * len(self.chain))()
         for d, (conv, bn, relu, res) in zip(descs, self.chain):
@@ -99,8 +103,8 @@ class EncoderPlan:
         _C.check(L.bevb200_encoder_create(int(encoder.in_channels), shape, descs, len(self.chain),
                                           ctypes.byref(handle)), "encoder_create")
         self._h = handle
-        if self.f16:
-            _C.check(L.bevb200_encoder_set_precision(self._h, PREC_FP16), "encoder_set_precision")
+        if self.f16 or self.i8:
+            _C.check(L.bevb200_encoder_set_precision(self._h, precision), "encoder_set_precision")
         self.n_levels = L.bevb200_encoder_num_levels(self._h)
         oshape = (ctypes.c_int32 * 3)()
         oc = ctypes.c_int32()
@@ -124,7 +128,14 @@ class EncoderPlan:
 
     # -- parameters: packed once, re-packed when a weight / BN tensor changes -------------------
     def _sync_params(self, dev):
-        key = (str(dev),)
+        scales = None
+        if self.i8:
+            scales = self.encoder.int8_scales()
+            if scales is None:
+                raise ValueError("the int8 plan needs calibrated scales: SparseEncoder.calibrate_int8() or "
+                                 "set_int8_scales()")
+            scales = [float(v) for v in scales]
+        key = (str(dev), None if scales is None else tuple(scales))
         for conv, bn, _, _ in self.chain:
             key += tuple((t.data_ptr(), t._version) for t in (conv.weight, conv.bias) if t is not None)
             if bn is not None:
@@ -147,6 +158,13 @@ class EncoderPlan:
                 shift = shift.contiguous()
             w = conv.weight.detach().float().contiguous()
             keep += [w, scale, shift]
+            if self.i8:
+                res = self.chain[i][3]
+                _C.check(L.bevb200_encoder_set_conv_int8(self._h, i, _C.ptr(w), _C.ptr(scale), _C.ptr(shift),
+                                                         scales[i - 1] if i > 0 else 1.0, scales[i],
+                                                         scales[res] if res >= 0 else 1.0, _C.ptr(self._params),
+                                                         self._params.numel(), stream), "encoder_set_conv_int8")
+                continue
             _C.check(L.bevb200_encoder_set_conv(self._h, i, _C.ptr(w), _C.ptr(scale), _C.ptr(shift),
                                                 _C.ptr(self._params), self._params.numel(), stream),
                      "encoder_set_conv")
@@ -166,7 +184,7 @@ class EncoderPlan:
 
     def forward(self, voxel_features, coors, batch_size, n_voxels_dev=None, out=None, level_caps=None,
                 overlap_rulebooks=True):
-        """voxel_features [N, C] fp32 (an fp16 plan: fp16), coors [N, 4] int32 (b, x, y, z); with n_voxels_dev
+        """voxel_features [N, C] fp32 (an fp16 or int8 plan: fp16), coors [N, 4] int32 (b, x, y, z); with n_voxels_dev
         (device int32[1]) only the first n rows are valid -- nothing is read back.  Returns [B, C*D, H, W] in the
         rows' dtype."""
         _C.require_cuda(voxel_features, "voxel_features", self.row_dtype)
@@ -207,7 +225,7 @@ class EncoderPlan:
                 if self._side is None or self._side.device != dev:
                     self._side = torch.cuda.Stream(device=dev)
                 side = self._side.cuda_stream
-            fwd = L.bevb200_encoder_forward_f16 if self.f16 else L.bevb200_encoder_forward
+            fwd = L.bevb200_encoder_forward_f16 if self.f16 or self.i8 else L.bevb200_encoder_forward
             rc = fwd(self._h, _C.ptr(self._params), _C.ptr(voxel_features), _C.ptr(coors), n, _C.ptr(n_voxels_dev),
                      B, caps, _C.ptr(out), stride, _C.ptr(self.status), _C.ptr(self._ws), self._ws.numel(),
                      _C.current_stream(dev), side)
@@ -329,7 +347,9 @@ class EncoderPlan:
         forward's rulebooks.  Under torch.no_grad() it still normalises with batch statistics and updates the
         running statistics, and keeps nothing for a backward.
         An fp16 plan also takes half features, half conv weights and half BN modules; its output is half and the
-        gradients come back in each tensor's dtype."""
+        gradients come back in each tensor's dtype.  An int8 plan has no training form."""
+        if self.i8:
+            raise ValueError("the int8 plan runs the eval forward only")
         ok = (torch.float32, torch.float16) if self.f16 else (torch.float32,)
         if voxel_features.dtype not in ok:
             raise ValueError("voxel_features must be %s" % " or ".join(str(t) for t in ok))

@@ -48,6 +48,10 @@ class SparseEncoder(nn.Module):
         self.native_plan = os.environ.get("BEVB200_ENCODER_NATIVE", "1") != "0"
         self._plan = None
         self._plan_f16 = None        # the fp16 plan: its own weight image, never shared with the bf16x3 one
+        self._plan_int8 = None
+        # per-conv output scales of the int8 plan (calibrate_int8 / set_int8_scales): a plain attribute, not a buffer,
+        # so the state_dict stays the reference's and its checkpoints load with strict=True
+        self._int8_scales = None
         self.rulebook_lookahead = os.environ.get("BEVB200_RULEBOOK_LOOKAHEAD", "1") != "0"
         self.conv_out = make_sparse_convmodule(encoder_out_channels, self.output_channels,
                                                kernel_size=(1, 1, 3), stride=(1, 1, 2),
@@ -55,9 +59,9 @@ class SparseEncoder(nn.Module):
                                                indice_key="spconv_down2", conv_type="SparseConv3d")
 
     def plan(self, precision=sp_ops.PREC_BF16X3):
-        """The native EncoderPlan of this module for `precision` (bf16x3 or fp16, built lazily), or None when a
-        layer has no native form."""
-        attr = "_plan_f16" if precision == sp_ops.PREC_FP16 else "_plan"
+        """The native EncoderPlan of this module for `precision` (bf16x3, fp16 or int8, built lazily), or None when
+        a layer has no native form."""
+        attr = {sp_ops.PREC_FP16: "_plan_f16", sp_ops.PREC_INT8: "_plan_int8"}.get(precision, "_plan")
         if getattr(self, attr) is None:
             from . import encoder_plan
             setattr(self, attr, encoder_plan.EncoderPlan(self, precision) if encoder_plan.supported(self) else False)
@@ -76,12 +80,17 @@ class SparseEncoder(nn.Module):
 
         precision=sp_ops.PREC_FP16 runs the native plan in fp16 (fp32 accumulation; the contract is in
         include/bevfusion_b200.h) and returns half: in eval mode under no_grad, and in training mode with
-        `num_voxels=`.  Anything else raises a ValueError; there is no fp16 form of the per-conv path."""
+        `num_voxels=`.  Anything else raises a ValueError; there is no fp16 form of the per-conv path.
+
+        precision=sp_ops.PREC_INT8 runs the native plan on u8 activations and s8 weights with the scales of
+        calibrate_int8() / set_int8_scales() and returns half: in eval mode under no_grad only."""
         coors = coors.int()
         if fused is None:
             fused = not self.training and self.order == ("conv", "norm", "act")
         if precision is None:
             precision = sp_ops.default_precision()
+        if precision == sp_ops.PREC_INT8:
+            return self._forward_int8(voxel_features, coors, batch_size, fused, out, num_voxels)
         if precision == sp_ops.PREC_FP16:
             return self._forward_fp16(voxel_features, coors, batch_size, fused, out, num_voxels)
         if (fused and self.native_plan and precision == sp_ops.PREC_BF16X3 and not torch.is_grad_enabled()
@@ -157,6 +166,77 @@ class SparseEncoder(nn.Module):
             raise ValueError("out= of an fp16 forward must be half")
         return plan.forward(voxel_features.to(torch.float16).contiguous(), coors.contiguous(), batch_size,
                             n_voxels_dev=num_voxels, out=out, overlap_rulebooks=self.overlap_rulebooks)
+
+    def _forward_int8(self, voxel_features, coors, batch_size, fused, out, num_voxels):
+        """precision=PREC_INT8: the int8 plan, or a ValueError before anything runs."""
+        if self.training:
+            raise ValueError("the int8 precision runs in eval mode only (there is no int8 training)")
+        if not fused:
+            raise ValueError("the int8 precision runs on the native plan only (no per-conv path): fused must not be False")
+        if torch.is_grad_enabled():
+            raise ValueError("the int8 precision runs under torch.no_grad() only")
+        if voxel_features.dtype not in (torch.float32, torch.float16):
+            raise ValueError("the int8 plan takes fp32 or fp16 features")
+        plan = self.plan(sp_ops.PREC_INT8) if self.plan() is not None and self._relu_chain() else None
+        if plan is None:
+            raise ValueError("the int8 precision needs a chain of (conv, norm, act) modules with tensor-core channel "
+                             "counts and a ReLU after every conv")
+        if self._int8_scales is None:
+            raise ValueError("the int8 precision needs calibrated scales: call calibrate_int8() or set_int8_scales()")
+        if out is not None and out.dtype != torch.float16:
+            raise ValueError("out= of an int8 forward must be half")
+        return plan.forward(voxel_features.to(torch.float16).contiguous(), coors.contiguous(), batch_size,
+                            n_voxels_dev=num_voxels, out=out, overlap_rulebooks=self.overlap_rulebooks)
+
+    def _relu_chain(self):
+        from .encoder_plan import _chain_of
+        return all(relu for _, _, relu, _ in _chain_of(self))
+
+    def calibrate_int8(self, batches):
+        """Sets the int8 plan's per-conv output scales from an fp32 eval pass of the per-conv path (bf16x3, folded
+        BN) over `batches`, an iterable of (voxel_features, coors, batch_size): s_i = fl(amax_i / 255), amax_i the
+        largest output of chain conv i (after its residual and ReLU) over all batches, or 1 when that is 0.
+        Returns the scales (float32 [n_convs], on the host)."""
+        from .encoder_plan import _chain_of, supported
+        if not supported(self) or not self._relu_chain():
+            raise ValueError("int8 calibration needs a chain the int8 plan runs (ReLU after every conv)")
+        chain = _chain_of(self)
+        amax = torch.zeros(len(chain), dtype=torch.float64)
+        n = 0
+        with torch.no_grad():
+            for voxel_features, coors, batch_size in batches:
+                x = spconv.SparseConvTensor(voxel_features.float().contiguous(), coors.int().contiguous(),
+                                            self.sparse_shape, batch_size)
+                outs = []
+                for conv, bn, relu, res in chain:
+                    s, t = bn_scale_shift(bn) if bn is not None else (None, None)
+                    x = conv(x, scale=s, shift=t, residual=outs[res].features if res >= 0 else None, relu=relu,
+                             precision=sp_ops.PREC_BF16X3)
+                    outs.append(x)
+                m = torch.stack([o.features.max() if o.features.numel() else o.features.new_zeros(())
+                                 for o in outs]).double().cpu()
+                amax = torch.maximum(amax, m)
+                n += 1
+        if n == 0:
+            raise ValueError("calibrate_int8 needs at least one batch")
+        amax32 = amax.float()
+        scales = torch.where(amax32 > 0, amax32 / 255.0, torch.ones_like(amax32))   # fp32 division: fl(amax / 255)
+        self.set_int8_scales(scales)
+        return self.int8_scales()
+
+    def int8_scales(self):
+        """The int8 plan's per-conv output scales (float32 [n_convs], host), or None before calibration."""
+        return None if self._int8_scales is None else self._int8_scales.clone()
+
+    def set_int8_scales(self, scales):
+        """Restores scales saved from int8_scales(): one finite, positive value per chain conv."""
+        from .encoder_plan import _chain_of
+        t = torch.as_tensor(scales).detach().to("cpu", torch.float32).flatten().clone()
+        if t.numel() != len(_chain_of(self)):
+            raise ValueError("int8 scales: %d values for %d convs" % (t.numel(), len(_chain_of(self))))
+        if not bool((torch.isfinite(t) & (t > 0)).all()):
+            raise ValueError("int8 scales must be finite and > 0")
+        self._int8_scales = t
 
     @staticmethod
     def _convmodule_fused(seq, x, precision):

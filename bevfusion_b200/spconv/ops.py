@@ -21,6 +21,10 @@ PREC_FP32, PREC_TF32X3, PREC_TF32, PREC_BF16X3 = 0, 1, 2, 3
 # fp16 operands with fp32 accumulation: only the native encoder plan runs it (SparseEncoder.forward(precision=...));
 # it is not one of the BEVB200_SPCONV_PRECISION names, and the per-conv ops refuse it
 PREC_FP16 = 4
+# u8 activations x s8 weights with int32 accumulation: the native encoder plan's eval forward only, with calibrated
+# scales (SparseEncoder.calibrate_int8); like PREC_FP16 it is not a BEVB200_SPCONV_PRECISION name.  5 stays unused:
+# plans refuse it, as they did before INT8 existed
+PREC_INT8 = 6
 _PREC_NAMES = {"fp32": PREC_FP32, "tf32x3": PREC_TF32X3, "tf32": PREC_TF32, "bf16x3": PREC_BF16X3}
 
 

@@ -1004,6 +1004,9 @@ BEVB200_API int bevb200_pairs_to_nbr(const int32_t *indice_pairs, const int32_t 
 #define BEVB200_PREC_BF16X3 3 /* bf16 MMAs: a = bf16 hi + bf16 lo, hi*hi + hi*lo + lo*hi (3 MMAs per 16 K) */
 #define BEVB200_PREC_FP16 4   /* fp16 operands, fp32 accumulation (1 MMA per 16 K): the encoder plan only
                                  (bevb200_encoder_set_precision); the per-conv calls refuse it */
+/* 5 is not a precision: every plan refuses it */
+#define BEVB200_PREC_INT8 6   /* u8 activations x s8 weights, exact int32 accumulation: the encoder plan's eval forward
+                                 only (bevb200_encoder_set_precision); the per-conv calls refuse it */
 BEVB200_API int bevb200_spconv_forward(const float *features, const float *weight, const int32_t *nbr,
                            int n_in, int n_out, int c_in, int c_out, int kernel_volume,
                            const float *scale, const float *shift, const float *residual,
@@ -1160,6 +1163,28 @@ BEVB200_API void bevb200_encoder_destroy(bevb200_encoder_t *enc);
  *              with the ordered chunk reduce; grad_voxel_features rounded once to fp16; BN gradients fp32
  * train_saved on an fp16 plan gives the offsets of z16 ([cap, c_out] half) and of the fp16 image y16 ([cap, c_out]
  * half).  bevb200_encoder_precision returns the plan's precision. */
+/* INT8 plans (eval only).  bevb200_encoder_set_precision(enc, BEVB200_PREC_INT8) makes a plan INT8; it returns
+ * BEVB200_EINVAL, and leaves the plan as it was, when a conv of the chain has no ReLU (every stored activation must be
+ * >= 0).  Call it before the size queries, which then report the INT8 layout exactly.  An INT8 plan packs conv i
+ * with bevb200_encoder_set_conv_int8 (bevb200_encoder_set_conv refuses it) and runs bevb200_encoder_forward_f16
+ * (half voxel_features in, half dense_out out); every training call, and the training size queries (which return 0),
+ * refuse it before they read any other argument.
+ * Numerical contract.  fl(.) is one fp32 round-to-nearest op, with no FMA contraction.
+ *   weights    per output channel c, on the raw conv weight (before any BN fold), when set_conv_int8 packs it:
+ *              s_w[c] = fl(max |W[.., .., c]| / 127) (1 when that max is 0), q_w = clamp(rint(fl(W / s_w[c])), -127,
+ *              127), rint rounding half to even
+ *   scales     conv i has one per-tensor output scale s_i > 0 (calibrated by the caller); r_i = fl(1 / s_i).  Conv i
+ *              reads with s_in = s_{i-1}, its residual with s_res = s_{residual_from}
+ *   conv 0     the fp16 plan's first conv: features rounded once to fp16, fp16 weights, fp32 accumulation acc;
+ *              a[c] = bn_scale[c]
+ *   convs 1..  u8 rows x q_w, exact int32 accumulation acc; a[c] = fl(fl(s_in * s_w[c]) * bn_scale[c])
+ *   epilogue   v = fl(fl(float(acc) * a[c]) + shift[c]) (bn_scale 1 and shift 0 when absent);
+ *              with a residual v = fl(v + fl(float(res_u8) * s_res)); then v = max(v, 0)
+ *   output     q = clamp(rint(fl(v * r_i)), 0, 255) as u8 (+inf saturates to 255, NaN becomes 0); the last conv
+ *              writes half(v) instead, which dense_out holds exactly
+ * set_conv_int8 takes weight [K, c_in, c_out], scale / shift [c_out] (nullable) as set_conv does, and the host
+ * scales s_in (ignored for conv 0), s_out and s_res (ignored without a residual); a scale that is not finite and > 0
+ * returns BEVB200_EINVAL. */
 BEVB200_API int bevb200_encoder_set_precision(bevb200_encoder_t *enc, int precision);
 BEVB200_API int bevb200_encoder_precision(const bevb200_encoder_t *enc);
 BEVB200_API size_t bevb200_encoder_param_bytes(const bevb200_encoder_t *enc);
@@ -1167,6 +1192,9 @@ BEVB200_API int bevb200_encoder_num_levels(const bevb200_encoder_t *enc);
 BEVB200_API int bevb200_encoder_output_shape(const bevb200_encoder_t *enc, int32_t *shape_out, int32_t *channels_out);
 BEVB200_API int bevb200_encoder_set_conv(bevb200_encoder_t *enc, int conv, const float *weight, const float *scale,
                              const float *shift, void *params, size_t params_bytes, void *stream);
+BEVB200_API int bevb200_encoder_set_conv_int8(bevb200_encoder_t *enc, int conv, const float *weight, const float *scale,
+                                  const float *shift, float s_in, float s_out, float s_res, void *params,
+                                  size_t params_bytes, void *stream);
 BEVB200_API int bevb200_encoder_level_caps(const bevb200_encoder_t *enc, int max_voxels, int batch_size,
                                const int32_t *level_caps_host, int32_t *caps_out);
 BEVB200_API size_t bevb200_encoder_workspace_bytes(const bevb200_encoder_t *enc, int max_voxels, int batch_size,
