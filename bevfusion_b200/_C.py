@@ -175,6 +175,8 @@ _SIGNATURES = {
                                      + [_P, _P, _P, _P, c_int, c_int, c_int, _P, _P, c_size_t, _P, c_size_t, _P]),
     "bevb200_pillar_backward_train": (c_int, [_P, _P, _P, c_int, c_int, _P, c_int, c_int] + [c_float] * 4
                                       + [_P, c_int, c_int, c_int, _P, c_size_t] + [_P] * 6 + [_P, c_size_t, _P]),
+    "bevb200_image_aug_workspace_bytes": (c_size_t, [c_int] * 7),
+    "bevb200_image_aug": (c_int, [_P, c_int, c_int, c_int, _P] + [c_int] * 4 + [c_float] * 6 + [_P] * 4 + [c_size_t, _P]),
 }
 
 

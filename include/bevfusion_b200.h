@@ -1314,6 +1314,35 @@ BEVB200_API int bevb200_pillar_backward_train(const float *voxels, const int32_t
                                               float *grad_beta2, void *workspace, size_t workspace_bytes,
                                               void *stream);
 
+/* ---- ImageAug3D + ImageNormalize of the camera pipeline (transforms_3d.py:98-192, 992-1006) ----------------------
+ * For each of `cams` uint8 RGB images [in_h, in_w, 3] (images [cams, in_h, in_w, 3], HWC as Pillow holds them) and
+ * its draw (draws: DEVICE double [cams, BEVB200_IMAGE_AUG_DRAW_FIELDS] = resize, resize_w, resize_h, crop_x, crop_y,
+ * flip (0 / 1), rotate in degrees), out [cams, 3, out_h, out_w] fp32 equals bit for bit
+ *     TF.normalize(TF.to_tensor(img.resize((resize_w, resize_h)).crop((crop_x, crop_y, crop_x + out_w,
+ *                  crop_y + out_h))[.transpose(FLIP_LEFT_RIGHT)].rotate(rotate)), mean, std)
+ * with Pillow's default BICUBIC resample, its crop fill 0, Image.rotate's NEAREST / fill 0 / no-expand rule, and
+ * u8 / 255 then (x - mean) / std in fp32.  aug_matrix [cams, 4, 4] fp32 is ImageAug3D's img_aug_matrix from the same
+ * draw (resize is the float scale the matrix uses; resize_w / resize_h are the resized image's sides).
+ * Only the crop window's columns and rows (with the vertical filter's support) are resampled.  Three launches, no host
+ * synchronisation, no allocation: CUDA-graph capturable.  status [1] int32 (device) is zeroed, then gets
+ *   BEVB200_IMAGE_AUG_BAD_DRAW        a field is not finite, a size / crop / flip is not an integer in range
+ *                                     (1 <= resize_* < 2^19, |crop| <= 2^30, flip 0 or 1)
+ *   BEVB200_IMAGE_AUG_OVER_CAPACITY   the draw's filter is wider than the workspace was sized for (resize_w below
+ *                                     min_resize_w or resize_h below min_resize_h)
+ * and that camera's outputs and matrix are NaN.  Sizes: 1 <= out_h, out_w <= 16384, 1 <= in_h, in_w < 2^19,
+ * cams <= 65535.  Workspace: bevb200_image_aug_workspace_bytes(cams, in_h, in_w, out_h, out_w, min_resize_w,
+ * min_resize_h) (0 for unsupported sizes): per camera its parameters, coefficient tables for the crop window and
+ * in_h x out_w RGBx staging rows, in disjoint regions; a smaller one gives BEVB200_EWORKSPACE before any launch. */
+#define BEVB200_IMAGE_AUG_DRAW_FIELDS 7
+#define BEVB200_IMAGE_AUG_BAD_DRAW 1
+#define BEVB200_IMAGE_AUG_OVER_CAPACITY 2
+BEVB200_API size_t bevb200_image_aug_workspace_bytes(int cams, int in_h, int in_w, int out_h, int out_w,
+                                                     int min_resize_w, int min_resize_h);
+BEVB200_API int bevb200_image_aug(const uint8_t *images, int cams, int in_h, int in_w, const double *draws, int out_h,
+                                  int out_w, int min_resize_w, int min_resize_h, float mean0, float mean1,
+                                  float mean2, float std0, float std1, float std2, float *out, float *aug_matrix,
+                                  int32_t *status, void *workspace, size_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
