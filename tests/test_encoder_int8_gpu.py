@@ -43,9 +43,15 @@ INT8_RAW["tile"] = (TILE_CHAIN[0], _with_relu(TILE_CHAIN[1]))
 
 class RawI8:
     """One raw conv chain on an INT8 plan through the C ABI.  Rows past n_valid (up to n_rows) are NaN features at
-    coordinates outside the grid."""
+    coordinates outside the grid.
 
-    def __init__(self, dev, cin, shape, B, convs, coors, n_rows=None, seed=0, exact=True):
+    Optional overrides of the seeded draws (which are made all the same, so the other values do not move): feats
+    (fp32 [n_valid, cin], rounded to fp16), and per conv index the dicts weights (fp32 [K, cin, cout]), bn_scales
+    and shifts (fp32 [cout] or None); s_act replaces chain_scales, and its None entries are chosen by one pass of the
+    oracle (encoder_int8_oracle.run_chain)."""
+
+    def __init__(self, dev, cin, shape, B, convs, coors, n_rows=None, seed=0, exact=True, feats=None, weights=None,
+                 bn_scales=None, shifts=None, s_act=None):
         self.dev, self.cin, self.shape, self.B, self.convs = dev, cin, list(shape), B, convs
         self.coors = np.ascontiguousarray(coors, dtype=np.int32)
         self.n_valid = self.coors.shape[0]
@@ -60,6 +66,17 @@ class RawI8:
             self.w.append(_grid(w, 2.0 ** -8, 1.0, g) * 0.25 if i == 0 else w)
             self.s.append(torch.rand(c["cout"], generator=g) + 0.5 if c.get("scale", True) else None)
             self.t.append(torch.randn(c["cout"], generator=g) * 0.2 if c.get("shift", True) else None)
+        if feats is not None:
+            self.feats16 = torch.as_tensor(feats, dtype=torch.float32).half()
+        for dst, src in ((self.w, weights), (self.s, bn_scales), (self.t, shifts)):
+            for i, v in (src or {}).items():
+                dst[i] = None if v is None else torch.as_tensor(v, dtype=torch.float32)
+        self._stats = None
+        if s_act is not None:
+            self.s_act = list(s_act)
+            if any(v is None for v in self.s_act):
+                self.stats()
+            return
         self.s_act = chain_scales(convs, self.feats16.numpy(), self.coors, B, shape, [w.numpy() for w in self.w],
                                   [None if s is None else s.numpy() for s in self.s],
                                   [None if t is None else t.numpy() for t in self.t])
@@ -99,10 +116,21 @@ class RawI8:
         finally:
             L.bevb200_encoder_destroy(h)
 
-    def oracle(self, exact=True):
+    def oracle(self, exact=True, stats=None):
+        if exact and stats is None and self._stats is not None:
+            return self._stats[1]
         return run_chain(self.convs, self.feats16.numpy(), self.coors, self.B, self.shape,
                          [w.numpy() for w in self.w], [None if s is None else s.numpy() for s in self.s],
-                         [None if t is None else t.numpy() for t in self.t], self.s_act, exact=exact)
+                         [None if t is None else t.numpy() for t in self.t], self.s_act, exact=exact, stats=stats)
+
+    def stats(self):
+        """the exact oracle's per-conv stats (encoder_int8_oracle.STAT_KEYS); fixes the s_act it chose"""
+        if self._stats is None:
+            st = []
+            res = self.oracle(stats=st)
+            self.s_act = [d["s_act"] for d in st]
+            self._stats = (st, res)
+        return self._stats[0]
 
 
 def _check_exact(raw):
