@@ -62,6 +62,8 @@ _SIGNATURES = {
                               + [c_size_t, _P]),
     "bevb200_hard_voxelize_mean": (c_int, [_P, c_int, c_int, _P, _P, c_int, c_int, c_int, _P, _P, _P, _P,
                                            _P, c_size_t, _P]),
+    "bevb200_hard_voxelize_mean_dev": (c_int, [_P, _P, c_int, c_int, _P, _P, c_int, c_int, c_int, _P, _P, _P, _P,
+                                               _P, c_size_t, _P]),
     "bevb200_depth_rasterize_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "bevb200_depth_rasterize": (c_int, [_P, c_int, c_int, _P, _P, _P, c_int, c_int, c_int, c_int, c_int,
                                         c_int, _P, _P, c_size_t, _P]),
@@ -177,6 +179,9 @@ _SIGNATURES = {
                                       + [_P, c_int, c_int, c_int, _P, c_size_t] + [_P] * 6 + [_P, c_size_t, _P]),
     "bevb200_image_aug_workspace_bytes": (c_size_t, [c_int] * 7),
     "bevb200_image_aug": (c_int, [_P, c_int, c_int, c_int, _P] + [c_int] * 4 + [c_float] * 6 + [_P] * 4 + [c_size_t, _P]),
+    "bevb200_lidar_sweeps_workspace_bytes": (c_size_t, [c_int] * 3),
+    "bevb200_lidar_sweeps_assemble": (c_int, [_P, c_int, c_int, c_int, _P, _P, _P] + [c_int] * 4 + [_P] * 4
+                                      + [c_size_t, _P]),
 }
 
 

@@ -1,0 +1,242 @@
+// LoadPointsFromMultiSweeps + PointsRangeFilter of the LiDAR pipeline (loading.py:87-235, transforms_3d.py:585-614,
+// base_points.py:208-232) on the device, bit-exact to the reference's numpy / torch lines.
+//
+// The raw sweeps live in a store of [slots, slot_cap, load_dim] fp32 rows with a device row count per slot; a frame
+// names, per sample, its ordered entries (the key, then the chosen sweeps, or pad copies of the key) by slot, with
+// each sweep's float64 pose and time lag.  Every frame parameter is read from device memory, so the three launches
+// can be replayed as a CUDA graph with new entries:
+//   1. sweeps_count_kernel  one CTA per (1024-row tile, entry, sample): rows kept after remove_close, the transform
+//                           and the range filter.  Tiles past the slot's device row count write 0 and exit.
+//   2. sweeps_scan_kernel   one CTA per sample: exclusive scan of its tile counts in (entry, tile) order, which is
+//                           the reference's concatenation order; the sample's count is min(total, cap).
+//   3. sweeps_write_kernel  the grid of 1: each kept row is recomputed and written at its tile offset plus its rank
+//                           in the tile (ballot ranks, no atomics), if that is below cap.
+// The double expressions are written with _rn intrinsics, so nvcc cannot contract them differently from the FMA chain
+// numpy's dgemm evaluates (see DESIGN.md section 4.27).
+#include <math.h>
+
+#include "common.cuh"
+
+static_assert(sizeof(bevb200_sweep_entry_t) == BEVB200_SWEEP_ENTRY_BYTES, "entry layout");
+static_assert(sizeof(bevb200_sweep_params_t) == BEVB200_SWEEP_PARAMS_BYTES, "params layout");
+
+namespace bevb200 {
+namespace {
+
+constexpr int kThreads = 256;
+constexpr int kRounds = 4;
+constexpr int kTile = kThreads * kRounds;     // rows per CTA
+constexpr int kMaxLoadDim = 64;
+
+struct Frame {
+  const float *store;
+  const int32_t *slot_rows;
+  const bevb200_sweep_params_t *params;
+  const bevb200_sweep_entry_t *entries;
+  int slots, slot_cap, load_dim, max_entries, out_dim, tiles;
+};
+
+__device__ __forceinline__ bool params_ok(const bevb200_sweep_params_t &p, int load_dim, int out_dim) {
+  bool ok = true;
+#pragma unroll
+  for (int c = 0; c < 8; ++c)
+    ok = ok && (c >= out_dim || (p.key_cols[c] >= 0 && p.key_cols[c] < load_dim && p.sweep_cols[c] >= 0 &&
+                                 p.sweep_cols[c] < load_dim));
+  return ok;
+}
+
+// rows of the entry (0 for NONE or a malformed entry); *bad is set for a malformed one
+__device__ __forceinline__ int entry_rows(const Frame &f, const bevb200_sweep_entry_t &e, bool *bad) {
+  *bad = false;
+  if (e.kind == BEVB200_SWEEP_NONE) return 0;
+  if ((e.kind != BEVB200_SWEEP_KEY && e.kind != BEVB200_SWEEP_SWEEP && e.kind != BEVB200_SWEEP_PAD) || e.slot < 0 ||
+      e.slot >= f.slots) {
+    *bad = true;
+    return 0;
+  }
+  return min(max(f.slot_rows[e.slot], 0), f.slot_cap);
+}
+
+// One row of an entry: its output columns and whether it survives remove_close and the range filter
+__device__ __forceinline__ bool eval_row(const float *__restrict__ src, const bevb200_sweep_entry_t &e,
+                                         const bevb200_sweep_params_t &p, int out_dim, float v[8]) {
+  const bool sweep = e.kind == BEVB200_SWEEP_SWEEP;
+#pragma unroll
+  for (int c = 0; c < 8; ++c) v[c] = c < out_dim ? __ldg(src + (sweep ? p.sweep_cols[c] : p.key_cols[c])) : 0.f;
+  if (p.remove_close && e.kind != BEVB200_SWEEP_KEY) {
+    // loading.py:167-169 on the raw sweep row (before use_dim), or on the key's selected columns for a pad copy
+    const float x = sweep ? __ldg(src + 0) : v[0], y = sweep ? __ldg(src + 1) : v[1];
+    if (fabsf(x) < p.radius && fabsf(y) < p.radius) return false;
+  }
+  if (sweep) {
+    // points_sweep[:, :3] @ R.T (fp32 x fp64 -> dgemm), the fp32 store, then += t in float64 and the fp32 store
+    const double p0 = v[0], p1 = v[1], p2 = v[2];
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+      const double r = __fma_rn(p2, e.rotation[3 * j + 2], __fma_rn(p1, e.rotation[3 * j + 1],
+                                                                    __dmul_rn(p0, e.rotation[3 * j + 0])));
+      v[j] = __double2float_rn(__dadd_rn((double)__double2float_rn(r), e.translation[j]));
+    }
+    v[4] = __double2float_rn(e.lag);
+  } else {
+    v[4] = 0.0f;
+  }
+  if (p.has_range)   // in_range_3d: strict fp32 comparisons, NaN fails them all
+    return v[0] > p.range[0] && v[1] > p.range[1] && v[2] > p.range[2] && v[0] < p.range[3] && v[1] < p.range[4] &&
+           v[2] < p.range[5];
+  return true;
+}
+
+__global__ void __launch_bounds__(kThreads)
+sweeps_count_kernel(Frame f, int32_t *__restrict__ tile_counts, int32_t *__restrict__ status) {
+  const int t = blockIdx.x, ei = blockIdx.z * f.max_entries + blockIdx.y;
+  const bevb200_sweep_entry_t e = f.entries[ei];
+  const bevb200_sweep_params_t p = *f.params;
+  bool bad;
+  int n = entry_rows(f, e, &bad);
+  const bool pbad = !params_ok(p, f.load_dim, f.out_dim);
+  if (t == 0 && threadIdx.x == 0 && (bad || pbad))
+    atomicOr(status, (bad ? BEVB200_SWEEPS_BAD_ENTRY : 0) | (pbad ? BEVB200_SWEEPS_BAD_PARAMS : 0));
+  if (pbad) n = 0;
+  const int row0 = t * kTile;
+  int kept = 0;
+  if (row0 < n) {
+    const float *base = f.store + (size_t)e.slot * f.slot_cap * f.load_dim;
+    for (int r = 0; r < kRounds; ++r) {
+      const int i = row0 + r * kThreads + threadIdx.x;
+      float v[8];
+      kept += __syncthreads_count(i < n && eval_row(base + (size_t)i * f.load_dim, e, p, f.out_dim, v));
+    }
+  }
+  if (threadIdx.x == 0) tile_counts[(size_t)ei * f.tiles + t] = kept;
+}
+
+__global__ void __launch_bounds__(kThreads)
+sweeps_scan_kernel(int32_t *__restrict__ tile_counts, int len, int cap, int32_t *__restrict__ counts,
+                   int32_t *__restrict__ status) {
+  __shared__ int warp_sum[kThreads / 32];
+  int32_t *c = tile_counts + (size_t)blockIdx.x * len;
+  const int lane = lane_id(), warp = threadIdx.x >> 5;
+  int carry = 0;
+  for (int base = 0; base < len; base += kThreads) {
+    const int i = base + threadIdx.x;
+    const int v = i < len ? c[i] : 0;
+    int incl = v;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const int u = __shfl_up_sync(0xffffffffu, incl, d);
+      if (lane >= d) incl += u;
+    }
+    if (lane == 31) warp_sum[warp] = incl;
+    __syncthreads();
+    int before = 0, total = 0;
+#pragma unroll
+    for (int w = 0; w < kThreads / 32; ++w) {
+      before += w < warp ? warp_sum[w] : 0;
+      total += warp_sum[w];
+    }
+    if (i < len) c[i] = carry + before + incl - v;
+    carry += total;
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    counts[blockIdx.x] = min(carry, cap);
+    if (carry > cap) atomicOr(status, BEVB200_SWEEPS_OVERFLOW);
+  }
+}
+
+__global__ void __launch_bounds__(kThreads)
+sweeps_write_kernel(Frame f, const int32_t *__restrict__ tile_offsets, int cap, float *__restrict__ out) {
+  __shared__ int warp_sum[kThreads / 32];
+  const int t = blockIdx.x, ei = blockIdx.z * f.max_entries + blockIdx.y;
+  const bevb200_sweep_entry_t e = f.entries[ei];
+  const bevb200_sweep_params_t p = *f.params;
+  bool bad;
+  const int n = params_ok(p, f.load_dim, f.out_dim) ? entry_rows(f, e, &bad) : 0;
+  const int row0 = t * kTile;
+  int off = tile_offsets[(size_t)ei * f.tiles + t];
+  if (row0 >= n || off >= cap) return;   // uniform over the CTA
+  const float *base = f.store + (size_t)e.slot * f.slot_cap * f.load_dim;
+  float *dst = out + (size_t)blockIdx.z * cap * f.out_dim;
+  const int lane = lane_id(), warp = threadIdx.x >> 5;
+  for (int r = 0; r < kRounds; ++r) {
+    const int i = row0 + r * kThreads + threadIdx.x;
+    float v[8];
+    const bool keep = i < n && eval_row(base + (size_t)i * f.load_dim, e, p, f.out_dim, v);
+    const unsigned m = __ballot_sync(0xffffffffu, keep);
+    if (lane == 0) warp_sum[warp] = __popc(m);
+    __syncthreads();
+    int before = 0, total = 0;
+#pragma unroll
+    for (int w = 0; w < kThreads / 32; ++w) {
+      before += w < warp ? warp_sum[w] : 0;
+      total += warp_sum[w];
+    }
+    const int pos = off + before + __popc(m & ((1u << lane) - 1));
+    if (keep && pos < cap) {
+      float *o = dst + (size_t)pos * f.out_dim;
+#pragma unroll
+      for (int c = 0; c < 8; ++c)
+        if (c < f.out_dim) o[c] = v[c];
+    }
+    off += total;
+    __syncthreads();
+  }
+}
+
+int tiles_for(int slot_cap) { return (slot_cap + kTile - 1) / kTile; }
+
+bool sizes_ok(int batch, int max_entries, int slot_cap) {
+  return batch >= 0 && batch <= 65535 && max_entries >= 1 && max_entries <= 65535 && slot_cap >= 1 &&
+         (long long)max_entries * slot_cap <= 0x7fffffffLL;
+}
+
+}  // namespace
+}  // namespace bevb200
+
+using namespace bevb200;
+
+extern "C" {
+
+size_t bevb200_lidar_sweeps_workspace_bytes(int batch, int max_entries, int slot_cap) {
+  if (!sizes_ok(batch, max_entries, slot_cap)) return 0;
+  return align_up((size_t)batch * max_entries * tiles_for(slot_cap) * sizeof(int32_t));
+}
+
+int bevb200_lidar_sweeps_assemble(const float *store, int slots, int slot_cap, int load_dim, const int32_t *slot_rows,
+                                  const bevb200_sweep_params_t *params, const bevb200_sweep_entry_t *entries,
+                                  int batch, int max_entries, int out_dim, int cap, float *out, int32_t *counts,
+                                  int32_t *status, void *workspace, size_t workspace_bytes, void *stream) {
+  BEVB200_REQUIRE(sizes_ok(batch, max_entries, slot_cap) && slots >= 1,
+                  "sizes out of range (0 <= batch <= 65535, 1 <= max_entries <= 65535, slots >= 1, slot_cap >= 1, "
+                  "max_entries * slot_cap < 2^31)");
+  BEVB200_REQUIRE(load_dim >= 3 && load_dim <= kMaxLoadDim, "load_dim must be in 3..64");
+  BEVB200_REQUIRE(out_dim >= 5 && out_dim <= BEVB200_SWEEP_MAX_DIM, "out_dim must be in 5..8");
+  BEVB200_REQUIRE(cap >= 1, "cap must be positive");
+  BEVB200_REQUIRE(status, "null pointer");
+  if (batch == 0) {
+    BEVB200_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t), (cudaStream_t)stream));
+    return BEVB200_OK;
+  }
+  BEVB200_REQUIRE(store && slot_rows && params && entries && out && counts, "null pointer");
+  BEVB200_REQUIRE((uintptr_t)entries % alignof(bevb200_sweep_entry_t) == 0 &&
+                      (uintptr_t)params % alignof(bevb200_sweep_params_t) == 0,
+                  "misaligned parameter block");
+  const size_t need = bevb200_lidar_sweeps_workspace_bytes(batch, max_entries, slot_cap);
+  if (!workspace || workspace_bytes < need) {
+    snprintf(g_last_error, sizeof(g_last_error), "%s: workspace of %zu bytes, need %zu", __func__, workspace_bytes,
+             need);
+    return BEVB200_EWORKSPACE;
+  }
+  Frame f{store, slot_rows, params, entries, slots, slot_cap, load_dim, max_entries, out_dim, tiles_for(slot_cap)};
+  int32_t *tiles = (int32_t *)workspace;
+  cudaStream_t st = (cudaStream_t)stream;
+  BEVB200_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t), st));
+  const dim3 grid(f.tiles, max_entries, batch);
+  BEVB200_LAUNCH(sweeps_count_kernel, grid, kThreads, 0, st, f, tiles, status);
+  BEVB200_LAUNCH(sweeps_scan_kernel, batch, kThreads, 0, st, tiles, max_entries * f.tiles, cap, counts, status);
+  BEVB200_LAUNCH(sweeps_write_kernel, grid, kThreads, 0, st, f, tiles, cap, out);
+  return BEVB200_OK;
+}
+
+}  // extern "C"

@@ -146,7 +146,7 @@ int bevb200_hard_voxelize_pillars(const float *points, int num_points, int num_f
   }
   BEVB200_REQUIRE(points && packed && canvas, "null argument");
   VoxWs w;
-  int rc = vox_front("hard_voxelize_pillars", points, n, num_features, vp, max_points, workspace, workspace_bytes,
+  int rc = vox_front("hard_voxelize_pillars", points, n, nullptr, num_features, vp, max_points, workspace, workspace_bytes,
                      st, &w);
   if (rc) return rc;
   const PfnGeom g{vx, vy, x_off, y_off};

@@ -508,7 +508,7 @@ int bevb200_hard_voxelize_radar(const float *points, int num_points, int num_fea
   uint32_t *total = (uint32_t *)((uint8_t *)table + align_up((size_t)n * sizeof(int4)));
   BEVB200_CUDA(cudaMemsetAsync(total, 0, sizeof(uint32_t), st));
   VoxWs w;
-  int rc = vox_front("hard_voxelize_radar", points, n, num_features, vp, max_points, workspace, vox_bytes, st, &w);
+  int rc = vox_front("hard_voxelize_radar", points, n, nullptr, num_features, vp, max_points, workspace, vox_bytes, st, &w);
   if (rc) return rc;
   const int C = net.n[n_layers - 1];
   const float *vrow = (const float *)packed + net.vrow;

@@ -25,16 +25,22 @@ namespace bevb200 {
 constexpr unsigned long long kEmptyKey = 0xffffffffffffffffull;
 constexpr int kListEmpty = 0x7f7f7f7f;  // memset(0x7f) pattern, larger than any point index
 
+// rows the kernels work on: n, or the device count clamped to [0, n] when there is one
+__device__ __forceinline__ int live_rows(int n, const int32_t *__restrict__ n_dev) {
+  return n_dev ? min(max(*n_dev, 0), n) : n;
+}
+
 __device__ __forceinline__ uint32_t hash64(unsigned long long k) {
   k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
   return (uint32_t)k;
 }
 
 __global__ void __launch_bounds__(256)
-    vox_insert_kernel(const float *__restrict__ points, int n, int nf, VoxParams vp,
-                      unsigned long long *__restrict__ keys, int32_t *__restrict__ slot_pvid,
+    vox_insert_kernel(const float *__restrict__ points, int n, const int32_t *__restrict__ n_dev, int nf,
+                      VoxParams vp, unsigned long long *__restrict__ keys, int32_t *__restrict__ slot_pvid,
                       uint32_t table_mask, int32_t *__restrict__ point_slot,
                       int32_t *__restrict__ pvid_counter) {
+  n = live_rows(n, n_dev);
   const int lane = lane_id();
   for (int base = (blockIdx.x * blockDim.x + threadIdx.x) & ~31; base < n;
        base += gridDim.x * blockDim.x) {
@@ -70,9 +76,10 @@ __global__ void __launch_bounds__(256)
 }
 
 __global__ void __launch_bounds__(256)
-    vox_rank_kernel(int n, int P, const int32_t *__restrict__ point_slot,
+    vox_rank_kernel(int n, const int32_t *__restrict__ n_dev, int P, const int32_t *__restrict__ point_slot,
                     const int32_t *__restrict__ slot_pvid, int32_t *__restrict__ point_pvid,
                     int32_t *__restrict__ lists, int32_t *__restrict__ counts) {
+  n = live_rows(n, n_dev);
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     int slot = point_slot[i];
     int pv = slot >= 0 ? slot_pvid[slot] : -1;
@@ -92,14 +99,16 @@ __global__ void __launch_bounds__(256)
 }
 
 __global__ void __launch_bounds__(256)
-    vox_flags_kernel(int n, int P, const int32_t *__restrict__ point_pvid,
+    vox_flags_kernel(int n, const int32_t *__restrict__ n_dev, int P, const int32_t *__restrict__ point_pvid,
                      const int32_t *__restrict__ lists, uint32_t *__restrict__ first_bits) {
-  // one ballot word per 32 points (n rounded up to a multiple of 32 by the launch loop)
+  // one ballot word per 32 points (n rounded up to a multiple of 32 by the launch loop); every word up to n is
+  // written, so the scan's total counts only the live rows' voxels
+  const int live = live_rows(n, n_dev);
   for (int base = (blockIdx.x * blockDim.x + threadIdx.x) & ~31; base < n;
        base += gridDim.x * blockDim.x) {
     int i = base + lane_id();
     bool first = false;
-    if (i < n) {
+    if (i < live) {
       int pv = point_pvid[i];
       first = pv >= 0 && lists[(long long)pv * P] == i;
     }
@@ -148,14 +157,15 @@ __global__ void __launch_bounds__(256)
 // the count and writes the mean row + (batch, x, y, z): voxelize + `feats.sum(dim=1) / sizes` +
 // `F.pad(coords, (1, 0), value=k)` (bevfusion.py:178-195) without the [M, P, F] intermediate.
 __global__ void __launch_bounds__(256)
-    vox_mean_kernel(const float *__restrict__ points, int n, int nf, VoxParams vp, int P,
-                    int max_voxels, int batch_idx, const int32_t *__restrict__ point_pvid,
+    vox_mean_kernel(const float *__restrict__ points, int n, const int32_t *__restrict__ n_dev, int nf,
+                    VoxParams vp, int P, int max_voxels, int batch_idx, const int32_t *__restrict__ point_pvid,
                     const int32_t *__restrict__ lists, const int32_t *__restrict__ counts,
                     const uint32_t *__restrict__ first_bits,
                     const uint32_t *__restrict__ word_prefix,
                     const uint32_t *__restrict__ total_voxels, float *__restrict__ feats,
                     int32_t *__restrict__ coords4, int32_t *__restrict__ num_points,
                     int32_t *__restrict__ voxel_num) {
+  n = live_rows(n, n_dev);
   if (blockIdx.x == 0 && threadIdx.x == 0)
     *voxel_num = (int32_t)min(*total_voxels, (uint32_t)max_voxels);
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -253,8 +263,9 @@ static size_t vox_layout(int n, int P, void *ws, size_t ws_bytes, VoxWs *out) {
 }
 
 // K1-K4, shared by the plain, the mean-fused and the pillar-fused entry points
-int vox_front(const char *who, const float *points, int n, int num_features, const VoxParams &vp,
-              int max_points, void *workspace, size_t workspace_bytes, cudaStream_t st, VoxWs *wout) {
+int vox_front(const char *who, const float *points, int n, const int32_t *n_dev, int num_features,
+              const VoxParams &vp, int max_points, void *workspace, size_t workspace_bytes, cudaStream_t st,
+              VoxWs *wout) {
   VoxWs w;
   size_t need = vox_layout(n, max_points, workspace, workspace_bytes, &w);
   if (workspace == nullptr || workspace_bytes < need) {
@@ -268,11 +279,11 @@ int vox_front(const char *who, const float *points, int n, int num_features, con
   BEVB200_CUDA(cudaMemsetAsync(w.lists, 0x7f, (size_t)n * max_points * sizeof(int32_t), st));
   BEVB200_CUDA(cudaMemsetAsync(w.counts, 0, (char *)w.slot_pvid - (char *)w.counts, st));
   const int grid = grid_for(n, 256);
-  BEVB200_LAUNCH(vox_insert_kernel, grid, 256, 0, st, points, n, num_features, vp, w.keys,
+  BEVB200_LAUNCH(vox_insert_kernel, grid, 256, 0, st, points, n, n_dev, num_features, vp, w.keys,
                  w.slot_pvid, w.table_size - 1, w.point_slot, w.pvid_counter);
-  BEVB200_LAUNCH(vox_rank_kernel, grid, 256, 0, st, n, max_points, w.point_slot, w.slot_pvid,
+  BEVB200_LAUNCH(vox_rank_kernel, grid, 256, 0, st, n, n_dev, max_points, w.point_slot, w.slot_pvid,
                  w.point_pvid, w.lists, w.counts);
-  BEVB200_LAUNCH(vox_flags_kernel, grid, 256, 0, st, n, max_points, w.point_pvid, w.lists,
+  BEVB200_LAUNCH(vox_flags_kernel, grid, 256, 0, st, n, n_dev, max_points, w.point_pvid, w.lists,
                  w.first_bits);
   int rc = exclusive_scan_u32(w.first_bits, w.word_prefix, w.nwords, w.tiles, w.total, true, st);
   if (rc) return rc;
@@ -309,7 +320,7 @@ int bevb200_hard_voxelize(const float *points, int num_points, int num_features,
   }
   BEVB200_REQUIRE(points && voxels && coors && num_points_per_voxel, "null argument");
   VoxWs w;
-  int rc = vox_front("hard_voxelize", points, n, num_features, vp, max_points, workspace,
+  int rc = vox_front("hard_voxelize", points, n, nullptr, num_features, vp, max_points, workspace,
                      workspace_bytes, st, &w);
   if (rc) return rc;
   BEVB200_LAUNCH(vox_scatter_kernel, grid_for(n, 256), 256, 0, st, points, n, num_features, vp,
@@ -337,10 +348,39 @@ int bevb200_hard_voxelize_mean(const float *points, int num_points, int num_feat
   BEVB200_REQUIRE(points && feats && coords4, "null argument");
   BEVB200_REQUIRE((uintptr_t)coords4 % 16 == 0, "coords must be 16-byte aligned");
   VoxWs w;
-  int rc = vox_front("hard_voxelize_mean", points, n, num_features, vp, max_points, workspace,
+  int rc = vox_front("hard_voxelize_mean", points, n, nullptr, num_features, vp, max_points, workspace,
                      workspace_bytes, st, &w);
   if (rc) return rc;
-  BEVB200_LAUNCH(vox_mean_kernel, grid_for(n, 256), 256, 0, st, points, n, num_features, vp,
+  BEVB200_LAUNCH(vox_mean_kernel, grid_for(n, 256), 256, 0, st, points, n, nullptr, num_features, vp,
+                 max_points, max_voxels, batch_idx, w.point_pvid, w.lists, w.counts, w.first_bits,
+                 w.word_prefix, w.total, feats, coords4, num_points_per_voxel, voxel_num);
+  return BEVB200_OK;
+}
+
+int bevb200_hard_voxelize_mean_dev(const float *points, const int32_t *num_points_dev, int max_rows,
+                                   int num_features, const float *voxel_size_host,
+                                   const float *coors_range_host, int max_points, int max_voxels,
+                                   int batch_idx, float *feats, int32_t *coords4,
+                                   int32_t *num_points_per_voxel, int32_t *voxel_num, void *workspace,
+                                   size_t workspace_bytes, void *stream) {
+  BEVB200_REQUIRE(max_rows >= 0 && num_features >= 3 && num_features <= 8, "bad point tensor shape");
+  BEVB200_REQUIRE(max_points > 0 && max_voxels > 0, "max_points / max_voxels must be positive");
+  BEVB200_REQUIRE(voxel_size_host && coors_range_host && voxel_num, "null argument");
+  VoxParams vp;
+  BEVB200_REQUIRE(make_params(voxel_size_host, coors_range_host, &vp) == 0, "bad voxel grid");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int n = max_rows;
+  if (n == 0) {
+    BEVB200_CUDA(cudaMemsetAsync(voxel_num, 0, sizeof(int32_t), st));
+    return BEVB200_OK;
+  }
+  BEVB200_REQUIRE(points && num_points_dev && feats && coords4, "null argument");
+  BEVB200_REQUIRE((uintptr_t)coords4 % 16 == 0, "coords must be 16-byte aligned");
+  VoxWs w;
+  int rc = vox_front("hard_voxelize_mean_dev", points, n, num_points_dev, num_features, vp, max_points,
+                     workspace, workspace_bytes, st, &w);
+  if (rc) return rc;
+  BEVB200_LAUNCH(vox_mean_kernel, grid_for(n, 256), 256, 0, st, points, n, num_points_dev, num_features, vp,
                  max_points, max_voxels, batch_idx, w.point_pvid, w.lists, w.counts, w.first_bits,
                  w.word_prefix, w.total, feats, coords4, num_points_per_voxel, voxel_num);
   return BEVB200_OK;

@@ -38,9 +38,10 @@ struct VoxWs {
 
 int make_params(const float *vs, const float *range, VoxParams *vp);
 
-// K1-K4 on n > 0 points; BEVB200_EWORKSPACE when the workspace is smaller than
-// bevb200_hard_voxelize_workspace_bytes(n, max_points)
-int vox_front(const char *who, const float *points, int n, int num_features, const VoxParams &vp,
-              int max_points, void *workspace, size_t workspace_bytes, cudaStream_t st, VoxWs *wout);
+// K1-K4 on n > 0 points, or on the first min(*n_dev, n) of them when n_dev (device int32) is not null;
+// BEVB200_EWORKSPACE when the workspace is smaller than bevb200_hard_voxelize_workspace_bytes(n, max_points)
+int vox_front(const char *who, const float *points, int n, const int32_t *n_dev, int num_features,
+              const VoxParams &vp, int max_points, void *workspace, size_t workspace_bytes, cudaStream_t st,
+              VoxWs *wout);
 
 }  // namespace bevb200

@@ -228,7 +228,8 @@ def voxelize_mean(voxels, coors, num_points, batch_idx=0):
     return feats, coords4
 
 
-def voxelize_mean_fused(points, voxel_size, coors_range, max_points, max_voxels, batch_idx=0, sync=True):
+def voxelize_mean_fused(points, voxel_size, coors_range, max_points, max_voxels, batch_idx=0, sync=True,
+                        num_points=None):
     """hard voxelization + per-voxel mean + (batch, x, y, z) coords in one pass over the points
     (bevfusion.py:178-195 with voxelize_reduce), never materialising the [M, max_points, F]
     voxel tensor.  Returns (feats [M, F], coords [M, 4] int32, num_points [M] int32).
@@ -236,9 +237,17 @@ def voxelize_mean_fused(points, voxel_size, coors_range, max_points, max_voxels,
     sync=False keeps the voxel count on the device (the reference returns it as a host int,
     voxelization_cuda.cu:369-370): the tensors come back at their cap size [max_voxels, ...] together
     with `voxel_num` (device int32[1]); rows >= voxel_num are unspecified.  SparseEncoder takes that
-    count as `num_voxels=`, so a whole LiDAR frame needs no host round trip."""
+    count as `num_voxels=`, so a whole LiDAR frame needs no host round trip.
+
+    num_points (device int32[1]): voxelize only the first num_points rows of `points` (a cloud at its cap
+    size, e.g. one sample of SweepStore.assemble(sync=False)), reading the count on the device only; the
+    result equals the call on points[:num_points]."""
     _C.require_cuda(points, "points", torch.float32)
     n, f = points.shape
+    if num_points is not None:
+        _C.require_cuda(num_points, "num_points", torch.int32)
+        if num_points.numel() != 1 or num_points.device != points.device:
+            raise ValueError("num_points must be one int32 on the points' device")
     vs, cr = _floats(voxel_size, 3), _floats(coors_range, 6)
     dev = points.device
     with torch.cuda.device(dev):
@@ -248,10 +257,13 @@ def voxelize_mean_fused(points, voxel_size, coors_range, max_points, max_voxels,
         voxel_num = torch.zeros(1, dtype=torch.int32, device=dev)
         nbytes = _C.lib().bevb200_hard_voxelize_workspace_bytes(n, int(max_points))
         ws = torch.empty(max(nbytes, 256), dtype=torch.uint8, device=dev)
-        rc = _C.lib().bevb200_hard_voxelize_mean(
-            _C.ptr(points), n, f, ctypes.cast(vs, ctypes.c_void_p), ctypes.cast(cr, ctypes.c_void_p),
-            int(max_points), int(max_voxels), int(batch_idx), _C.ptr(feats), _C.ptr(coords4),
-            _C.ptr(num), _C.ptr(voxel_num), _C.ptr(ws), ws.numel(), _C.current_stream(dev))
+        args = (f, ctypes.cast(vs, ctypes.c_void_p), ctypes.cast(cr, ctypes.c_void_p), int(max_points),
+                int(max_voxels), int(batch_idx), _C.ptr(feats), _C.ptr(coords4), _C.ptr(num), _C.ptr(voxel_num),
+                _C.ptr(ws), ws.numel(), _C.current_stream(dev))
+        if num_points is None:
+            rc = _C.lib().bevb200_hard_voxelize_mean(_C.ptr(points), n, *args)
+        else:
+            rc = _C.lib().bevb200_hard_voxelize_mean_dev(_C.ptr(points), _C.ptr(num_points), n, *args)
     _C.check(rc, "hard_voxelize_mean")
     if not sync:
         return feats, coords4, num, voxel_num

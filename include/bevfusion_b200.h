@@ -356,6 +356,16 @@ BEVB200_API int bevb200_hard_voxelize_mean(const float *points, int num_points, 
                                int32_t *coords4, int32_t *num_points_per_voxel, int32_t *voxel_num,
                                void *workspace, size_t workspace_bytes, void *stream);
 
+/* bevb200_hard_voxelize_mean on the first *num_points_dev (DEVICE int32[1], clamped to [0, max_rows]) rows of
+ * points [max_rows, F]: the same outputs, bit for bit, as bevb200_hard_voxelize_mean with that host count, without
+ * reading the count on the host.  Workspace as bevb200_hard_voxelize_workspace_bytes(max_rows, max_points). */
+BEVB200_API int bevb200_hard_voxelize_mean_dev(const float *points, const int32_t *num_points_dev, int max_rows,
+                                               int num_features, const float *voxel_size_host,
+                                               const float *coors_range_host, int max_points, int max_voxels,
+                                               int batch_idx, float *feats, int32_t *coords4,
+                                               int32_t *num_points_per_voxel, int32_t *voxel_num, void *workspace,
+                                               size_t workspace_bytes, void *stream);
+
 /* Replaces voxelization::dynamic_voxelize_gpu (voxelization_cuda.cu:485-528):
  * coors[i] = (cx, cy, cz) or (-1,-1,-1) when the point is out of range.  (The reference
  * kernel only guarantees coors[i][0] == -1 for such points, :38-47.) */
@@ -1342,6 +1352,61 @@ BEVB200_API int bevb200_image_aug(const uint8_t *images, int cams, int in_h, int
                                   int out_w, int min_resize_w, int min_resize_h, float mean0, float mean1,
                                   float mean2, float std0, float std1, float std2, float *out, float *aug_matrix,
                                   int32_t *status, void *workspace, size_t workspace_bytes, void *stream);
+
+/* ---- LoadPointsFromMultiSweeps + PointsRangeFilter of the LiDAR pipeline (loading.py:87-235,
+ *      transforms_3d.py:585-614, base_points.py:208-232) ------------------------------------------------------------
+ * store [slots, slot_cap, load_dim] fp32 holds raw point rows (DEVICE), slot_rows [slots] int32 (DEVICE) the rows of
+ * each slot.  For each of `batch` samples, entries [batch, max_entries] (DEVICE) lists its entries in the reference's
+ * concatenation order: the key, then the chosen sweeps in the order of `choices`, or pad copies of the key; unused
+ * entries are BEVB200_SWEEP_NONE.  params (DEVICE) holds the column maps, remove_close and the range.  Per row:
+ *   KEY    out[c] = raw[key_cols[c]], out[4] = +0
+ *   SWEEP  dropped iff remove_close and |raw[0]| < radius and |raw[1]| < radius; out[c] = raw[sweep_cols[c]]; then
+ *          out[j] = fl32(fl32(fma(p2, R[j][2], fma(p1, R[j][1], p0 * R[j][0]))) + t[j]) in float64 for j < 3
+ *          (p = out[0..2]) and out[4] = fl32(lag)
+ *   PAD    a KEY row, dropped iff remove_close and |out[0]| < radius and |out[1]| < radius
+ * and with has_range a row is kept iff range[0] < x < range[3], range[1] < y < range[4], range[2] < z < range[5] in
+ * fp32 (NaN is dropped).  out [batch, cap, out_dim] receives each sample's kept rows in order, counts [batch] int32
+ * (DEVICE) min(kept, cap); rows past counts[b] are left untouched and nothing is written past cap.  status [1] int32
+ * (DEVICE) is zeroed, then gets
+ *   BEVB200_SWEEPS_OVERFLOW    a sample kept more than cap rows (its first cap rows are written)
+ *   BEVB200_SWEEPS_BAD_ENTRY   an entry has an unknown kind or a slot outside [0, slots) (it contributes no rows)
+ *   BEVB200_SWEEPS_BAD_PARAMS  a column map names a column outside [0, load_dim) (no sample gets rows)
+ * Three launches sized by (batch, max_entries, slot_cap), no atomics on the output order, no host synchronisation:
+ * CUDA-graph capturable with the store, params and entries refreshed between replays.  Sizes: 3 <= load_dim <= 64,
+ * 5 <= out_dim <= 8, cap >= 1, batch <= 65535, max_entries <= 65535, max_entries * slot_cap < 2^31.  Workspace:
+ * bevb200_lidar_sweeps_workspace_bytes(batch, max_entries, slot_cap) (0 for unsupported sizes): one int32 per
+ * 1024-row tile; a smaller one gives BEVB200_EWORKSPACE before any write. */
+#define BEVB200_SWEEP_NONE 0
+#define BEVB200_SWEEP_KEY 1
+#define BEVB200_SWEEP_SWEEP 2
+#define BEVB200_SWEEP_PAD 3
+#define BEVB200_SWEEP_MAX_DIM 8
+#define BEVB200_SWEEPS_OVERFLOW 1
+#define BEVB200_SWEEPS_BAD_ENTRY 2
+#define BEVB200_SWEEPS_BAD_PARAMS 4
+#define BEVB200_SWEEP_ENTRY_BYTES 112
+#define BEVB200_SWEEP_PARAMS_BYTES 100
+typedef struct {
+  int32_t kind;              /* BEVB200_SWEEP_* */
+  int32_t slot;
+  double rotation[9];        /* sensor2lidar_rotation, row-major (SWEEP) */
+  double translation[3];     /* sensor2lidar_translation (SWEEP) */
+  double lag;                /* timestamp / 1e6 - sweep timestamp / 1e6 (SWEEP) */
+} bevb200_sweep_entry_t;
+typedef struct {
+  int32_t key_cols[BEVB200_SWEEP_MAX_DIM];     /* LoadPointsFromFile's use_dim composed with the sweep loader's */
+  int32_t sweep_cols[BEVB200_SWEEP_MAX_DIM];   /* the sweep loader's use_dim */
+  int32_t remove_close;
+  int32_t has_range;
+  float radius;                                /* fl32(radius) */
+  float range[6];                              /* fl32(point_cloud_range) */
+} bevb200_sweep_params_t;
+BEVB200_API size_t bevb200_lidar_sweeps_workspace_bytes(int batch, int max_entries, int slot_cap);
+BEVB200_API int bevb200_lidar_sweeps_assemble(const float *store, int slots, int slot_cap, int load_dim,
+                                              const int32_t *slot_rows, const bevb200_sweep_params_t *params,
+                                              const bevb200_sweep_entry_t *entries, int batch, int max_entries,
+                                              int out_dim, int cap, float *out, int32_t *counts, int32_t *status,
+                                              void *workspace, size_t workspace_bytes, void *stream);
 
 #ifdef __cplusplus
 }
