@@ -32,6 +32,7 @@ constexpr int kSetupThreads = 256;
 constexpr int kHpassCols = 128;
 constexpr int kHpassRows = 8;
 constexpr int kVpassCols = 128;
+constexpr int kMaxGridY = 65535;          // CUDA's grid.y and grid.z limit: hpass row blocks, cameras
 
 enum RotateKind { kCopy = 0, kRot180 = 1, kRot90 = 2, kRot270 = 3, kScale = 4, kAffine = 5 };
 
@@ -288,19 +289,22 @@ image_aug_hpass_kernel(const uint8_t *__restrict__ images, int H, int W, int fW,
   const int2 b = T.hbounds[(size_t)cam * fW + j];
   if (b.y == 0) return;
   const int32_t *k = T.hcoef + ((size_t)cam * fW + j) * kcap_w;
-  const int rows = min(kHpassRows, p.band_rows - row0);
-  for (int r = 0; r < rows; ++r) {
-    const int y = p.band_first + row0 + r;
-    const uint8_t *src = images + (((size_t)cam * H + y) * W + b.x) * 3;
-    int s0 = 1 << (kPrecisionBits - 1), s1 = s0, s2 = s0;
-    for (int x = 0; x < b.y; ++x) {
-      const int kx = __ldg(k + x);
-      s0 += (int)__ldg(src + 3 * x + 0) * kx;
-      s1 += (int)__ldg(src + 3 * x + 1) * kx;
-      s2 += (int)__ldg(src + 3 * x + 2) * kx;
+  // a band taller than gridDim.y row blocks (in_h > 65535 * kHpassRows) is covered in gridDim.y strides
+  for (int first = row0; first < p.band_rows; first += gridDim.y * kHpassRows) {
+    const int rows = min(kHpassRows, p.band_rows - first);
+    for (int r = 0; r < rows; ++r) {
+      const int y = p.band_first + first + r;
+      const uint8_t *src = images + (((size_t)cam * H + y) * W + b.x) * 3;
+      int s0 = 1 << (kPrecisionBits - 1), s1 = s0, s2 = s0;
+      for (int x = 0; x < b.y; ++x) {
+        const int kx = __ldg(k + x);
+        s0 += (int)__ldg(src + 3 * x + 0) * kx;
+        s1 += (int)__ldg(src + 3 * x + 1) * kx;
+        s2 += (int)__ldg(src + 3 * x + 2) * kx;
+      }
+      T.band[((size_t)cam * H + first + r) * fW + j] =
+          make_uchar4((unsigned char)clip8(s0), (unsigned char)clip8(s1), (unsigned char)clip8(s2), 0);
     }
-    T.band[((size_t)cam * H + row0 + r) * fW + j] =
-        make_uchar4((unsigned char)clip8(s0), (unsigned char)clip8(s1), (unsigned char)clip8(s2), 0);
   }
 }
 
@@ -385,8 +389,8 @@ Tables carve(void *ws, int cams, int H, int fH, int fW, int kcap_w, int kcap_h, 
 }
 
 bool sizes_ok(int cams, int H, int W, int fH, int fW, int min_w, int min_h) {
-  return cams >= 0 && H >= 1 && W >= 1 && H < kMaxSource && W < kMaxSource && fH >= 1 && fW >= 1 &&
-         fH <= kMaxFrame && fW <= kMaxFrame && min_w >= 1 && min_h >= 1 && min_w < kMaxSource &&
+  return cams >= 0 && cams <= kMaxGridY && H >= 1 && W >= 1 && H < kMaxSource && W < kMaxSource && fH >= 1 &&
+         fW >= 1 && fH <= kMaxFrame && fW <= kMaxFrame && min_w >= 1 && min_h >= 1 && min_w < kMaxSource &&
          min_h < kMaxSource;
 }
 
@@ -409,7 +413,7 @@ int bevb200_image_aug(const uint8_t *images, int cams, int in_h, int in_w, const
                       int min_resize_w, int min_resize_h, float mean0, float mean1, float mean2, float std0,
                       float std1, float std2, float *out, float *aug_matrix, int32_t *status, void *workspace,
                       size_t workspace_bytes, void *stream) {
-  BEVB200_REQUIRE(sizes_ok(cams, in_h, in_w, out_h, out_w, min_resize_w, min_resize_h) && cams <= 65535,
+  BEVB200_REQUIRE(sizes_ok(cams, in_h, in_w, out_h, out_w, min_resize_w, min_resize_h),
                   "sizes out of range (cams <= 65535; 1 <= out_h, out_w <= 16384; 1 <= in_h, in_w, min_resize_* < 2^19)");
   if (cams == 0) return BEVB200_OK;
   BEVB200_REQUIRE(images && draws && out && aug_matrix && status, "null pointer");
@@ -426,7 +430,8 @@ int bevb200_image_aug(const uint8_t *images, int cams, int in_h, int in_w, const
   BEVB200_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t), st));
   BEVB200_LAUNCH(image_aug_setup_kernel, cams, kSetupThreads, 0, st, draws, in_h, in_w, out_h, out_w, kcap_w, kcap_h,
                  T, aug_matrix, status);
-  const dim3 hgrid((out_w + kHpassCols - 1) / kHpassCols, (in_h + kHpassRows - 1) / kHpassRows, cams);
+  const int row_blocks = min((in_h + kHpassRows - 1) / kHpassRows, kMaxGridY);   // the kernel strides past 65535
+  const dim3 hgrid((out_w + kHpassCols - 1) / kHpassCols, row_blocks, cams);
   BEVB200_LAUNCH(image_aug_hpass_kernel, hgrid, kHpassCols, 0, st, images, in_h, in_w, out_w, kcap_w, T);
   const dim3 vgrid((out_w + kVpassCols - 1) / kVpassCols, out_h, cams);
   BEVB200_LAUNCH(image_aug_vpass_kernel, vgrid, kVpassCols, 0, st, in_h, out_h, out_w, kcap_h, T, mean0, mean1, mean2,

@@ -69,12 +69,13 @@ __device__ __forceinline__ bool eval_row(const float *__restrict__ src, const be
     if (fabsf(x) < p.radius && fabsf(y) < p.radius) return false;
   }
   if (sweep) {
-    // points_sweep[:, :3] @ R.T (fp32 x fp64 -> dgemm), the fp32 store, then += t in float64 and the fp32 store
+    // points_sweep[:, :3] @ R.T (fp32 x fp64 -> dgemm), the fp32 store, then += t in float64 and the fp32 store.
+    // The dgemm's accumulator starts at +0.0, so a zero dot product is +0.0 even when every term is -0.0.
     const double p0 = v[0], p1 = v[1], p2 = v[2];
 #pragma unroll
     for (int j = 0; j < 3; ++j) {
       const double r = __fma_rn(p2, e.rotation[3 * j + 2], __fma_rn(p1, e.rotation[3 * j + 1],
-                                                                    __dmul_rn(p0, e.rotation[3 * j + 0])));
+                                                                    __fma_rn(p0, e.rotation[3 * j + 0], 0.0)));
       v[j] = __double2float_rn(__dadd_rn((double)__double2float_rn(r), e.translation[j]));
     }
     v[4] = __double2float_rn(e.lag);

@@ -1361,8 +1361,8 @@ BEVB200_API int bevb200_image_aug(const uint8_t *images, int cams, int in_h, int
  * entries are BEVB200_SWEEP_NONE.  params (DEVICE) holds the column maps, remove_close and the range.  Per row:
  *   KEY    out[c] = raw[key_cols[c]], out[4] = +0
  *   SWEEP  dropped iff remove_close and |raw[0]| < radius and |raw[1]| < radius; out[c] = raw[sweep_cols[c]]; then
- *          out[j] = fl32(fl32(fma(p2, R[j][2], fma(p1, R[j][1], p0 * R[j][0]))) + t[j]) in float64 for j < 3
- *          (p = out[0..2]) and out[4] = fl32(lag)
+ *          out[j] = fl32(fl32(fma(p2, R[j][2], fma(p1, R[j][1], fma(p0, R[j][0], +0.0)))) + t[j]) in float64 for
+ *          j < 3 (p = out[0..2]) and out[4] = fl32(lag)
  *   PAD    a KEY row, dropped iff remove_close and |out[0]| < radius and |out[1]| < radius
  * and with has_range a row is kept iff range[0] < x < range[3], range[1] < y < range[4], range[2] < z < range[5] in
  * fp32 (NaN is dropped).  out [batch, cap, out_dim] receives each sample's kept rows in order, counts [batch] int32
