@@ -87,6 +87,8 @@ _SIGNATURES = {
     "bevb200_hard_voxelize_radar_workspace_bytes": (c_size_t, [c_int, c_int]),
     "bevb200_hard_voxelize_radar": (c_int, [_P, c_int, c_int, _P, _P, c_int, c_int, c_int, _P] + [c_float] * 4
                                     + [_P, _P, _P, _P, c_int, c_int, _P, _P, c_size_t, _P]),
+    "bevb200_hard_voxelize_radar_dev": (c_int, [_P, _P, c_int, c_int, _P, _P, c_int, c_int, c_int, _P]
+                                        + [c_float] * 4 + [_P, _P, _P, _P, c_int, c_int, _P, _P, c_size_t, _P]),
     "bevb200_boxes_iou_bev": (c_int, [_P, c_int, _P, c_int, _P, _P]),
     "bevb200_boxes_overlap_bev": (c_int, [_P, c_int, _P, c_int, _P, _P]),
     "bevb200_nms_workspace_bytes": (c_size_t, [c_int, c_int]),
@@ -181,6 +183,9 @@ _SIGNATURES = {
     "bevb200_image_aug": (c_int, [_P, c_int, c_int, c_int, _P] + [c_int] * 4 + [c_float] * 6 + [_P] * 4 + [c_size_t, _P]),
     "bevb200_lidar_sweeps_workspace_bytes": (c_size_t, [c_int] * 3),
     "bevb200_lidar_sweeps_assemble": (c_int, [_P, c_int, c_int, c_int, _P, _P, _P] + [c_int] * 4 + [_P] * 4
+                                      + [c_size_t, _P]),
+    "bevb200_radar_sweeps_workspace_bytes": (c_size_t, [c_int] * 3),
+    "bevb200_radar_sweeps_assemble": (c_int, [_P, c_int, c_int, _P, _P, _P] + [c_int] * 4 + [_P] * 4
                                       + [c_size_t, _P]),
 }
 

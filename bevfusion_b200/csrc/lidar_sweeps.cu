@@ -15,7 +15,7 @@
 // numpy's dgemm evaluates (see DESIGN.md section 4.27).
 #include <math.h>
 
-#include "common.cuh"
+#include "sweeps_scan.cuh"
 
 static_assert(sizeof(bevb200_sweep_entry_t) == BEVB200_SWEEP_ENTRY_BYTES, "entry layout");
 static_assert(sizeof(bevb200_sweep_params_t) == BEVB200_SWEEP_PARAMS_BYTES, "params layout");
@@ -193,6 +193,13 @@ bool sizes_ok(int batch, int max_entries, int slot_cap) {
 }
 
 }  // namespace
+
+int sweeps_scan(int32_t *tile_counts, int batch, int len, int cap, int32_t *counts, int32_t *status,
+                cudaStream_t st) {
+  BEVB200_LAUNCH(sweeps_scan_kernel, batch, kThreads, 0, st, tile_counts, len, cap, counts, status);
+  return BEVB200_OK;
+}
+
 }  // namespace bevb200
 
 using namespace bevb200;
@@ -235,7 +242,8 @@ int bevb200_lidar_sweeps_assemble(const float *store, int slots, int slot_cap, i
   BEVB200_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t), st));
   const dim3 grid(f.tiles, max_entries, batch);
   BEVB200_LAUNCH(sweeps_count_kernel, grid, kThreads, 0, st, f, tiles, status);
-  BEVB200_LAUNCH(sweeps_scan_kernel, batch, kThreads, 0, st, tiles, max_entries * f.tiles, cap, counts, status);
+  const int rc = sweeps_scan(tiles, batch, max_entries * f.tiles, cap, counts, status, st);
+  if (rc) return rc;
   BEVB200_LAUNCH(sweeps_write_kernel, grid, kThreads, 0, st, f, tiles, cap, out);
   return BEVB200_OK;
 }

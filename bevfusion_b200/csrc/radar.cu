@@ -480,22 +480,22 @@ size_t bevb200_hard_voxelize_radar_workspace_bytes(int num_points, int max_point
   return align_up(bevb200_hard_voxelize_workspace_bytes(num_points, max_points)) + rfn_table_bytes(num_points);
 }
 
-int bevb200_hard_voxelize_radar(const float *points, int num_points, int num_features, const float *voxel_size_host,
-                                const float *coors_range_host, int max_points, int max_voxels, int n_layers,
-                                const int *widths, float vx, float vy, float x_off, float y_off, const float *pc_min,
-                                const float *pc_span, const void *packed, float *canvas, int nx, int ny,
-                                int32_t *voxel_num, void *workspace, size_t workspace_bytes, void *stream) {
+// the host-count and device-count fused entries: n rows (the host count, or the row cap with n_dev)
+static int hard_voxelize_radar(const char *who, const float *points, int n, const int32_t *n_dev, int num_features,
+                               const float *voxel_size_host, const float *coors_range_host, int max_points,
+                               int max_voxels, int n_layers, const int *widths, float vx, float vy, float x_off,
+                               float y_off, const float *pc_min, const float *pc_span, const void *packed,
+                               float *canvas, int nx, int ny, int32_t *voxel_num, void *workspace,
+                               size_t workspace_bytes, cudaStream_t st) {
   RfnNet net;
   BEVB200_RADAR_UNSUPPORTED(rfn_layout(num_features, n_layers, widths, &net), kRfnShapeMsg);
   BEVB200_RADAR_UNSUPPORTED(max_points >= 1 && max_points <= kRfnMaxP, kRfnShapeMsg);
-  BEVB200_REQUIRE(num_points >= 0 && max_voxels > 0, "bad sizes");
+  BEVB200_REQUIRE(n >= 0 && max_voxels > 0, "bad sizes");
   BEVB200_REQUIRE(voxel_size_host && coors_range_host && voxel_num && pc_min && pc_span, "null argument");
   VoxParams vp;
   BEVB200_REQUIRE(make_params(voxel_size_host, coors_range_host, &vp) == 0, "bad voxel grid");
   BEVB200_RADAR_UNSUPPORTED(vp.grid[2] == 1, "radar pillars need a voxel grid one cell high");
   BEVB200_REQUIRE(vp.grid[0] == nx && vp.grid[1] == ny, "canvas shape differs from the voxel grid");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int n = num_points;
   if (n == 0) {
     BEVB200_CUDA(cudaMemsetAsync(voxel_num, 0, sizeof(int32_t), st));
     return BEVB200_OK;
@@ -508,7 +508,9 @@ int bevb200_hard_voxelize_radar(const float *points, int num_points, int num_fea
   uint32_t *total = (uint32_t *)((uint8_t *)table + align_up((size_t)n * sizeof(int4)));
   BEVB200_CUDA(cudaMemsetAsync(total, 0, sizeof(uint32_t), st));
   VoxWs w;
-  int rc = vox_front("hard_voxelize_radar", points, n, nullptr, num_features, vp, max_points, workspace, vox_bytes, st, &w);
+  // with a device count of 0 no point is a voxel's first: the table stays empty, voxel_num becomes 0 and the
+  // tiles kernel finds no rows, so the host early-out above needs no device twin
+  int rc = vox_front(who, points, n, n_dev, num_features, vp, max_points, workspace, vox_bytes, st, &w);
   if (rc) return rc;
   const int C = net.n[n_layers - 1];
   const float *vrow = (const float *)packed + net.vrow;
@@ -519,6 +521,30 @@ int bevb200_hard_voxelize_radar(const float *points, int num_points, int num_fea
                  rfn_geom(vx, vy, x_off, y_off, pc_min, pc_span), net, (const uint8_t *)packed, table, total, n,
                  canvas, 1ll, (long long)nx * ny);
   return BEVB200_OK;
+}
+
+int bevb200_hard_voxelize_radar(const float *points, int num_points, int num_features, const float *voxel_size_host,
+                                const float *coors_range_host, int max_points, int max_voxels, int n_layers,
+                                const int *widths, float vx, float vy, float x_off, float y_off, const float *pc_min,
+                                const float *pc_span, const void *packed, float *canvas, int nx, int ny,
+                                int32_t *voxel_num, void *workspace, size_t workspace_bytes, void *stream) {
+  return hard_voxelize_radar("hard_voxelize_radar", points, num_points, nullptr, num_features, voxel_size_host,
+                             coors_range_host, max_points, max_voxels, n_layers, widths, vx, vy, x_off, y_off, pc_min,
+                             pc_span, packed, canvas, nx, ny, voxel_num, workspace, workspace_bytes,
+                             (cudaStream_t)stream);
+}
+
+int bevb200_hard_voxelize_radar_dev(const float *points, const int32_t *num_points_dev, int max_rows,
+                                    int num_features, const float *voxel_size_host, const float *coors_range_host,
+                                    int max_points, int max_voxels, int n_layers, const int *widths, float vx,
+                                    float vy, float x_off, float y_off, const float *pc_min, const float *pc_span,
+                                    const void *packed, float *canvas, int nx, int ny, int32_t *voxel_num,
+                                    void *workspace, size_t workspace_bytes, void *stream) {
+  BEVB200_REQUIRE(max_rows == 0 || num_points_dev, "null argument");
+  return hard_voxelize_radar("hard_voxelize_radar_dev", points, max_rows, num_points_dev, num_features,
+                             voxel_size_host, coors_range_host, max_points, max_voxels, n_layers, widths, vx, vy,
+                             x_off, y_off, pc_min, pc_span, packed, canvas, nx, ny, voxel_num, workspace,
+                             workspace_bytes, (cudaStream_t)stream);
 }
 
 }  // extern "C"

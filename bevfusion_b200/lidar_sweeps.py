@@ -22,7 +22,8 @@ import torch
 
 from . import _C
 
-__all__ = ["SweepStore", "assemble_sweeps", "choose_sweeps", "time_lag", "OVERFLOW", "BAD_ENTRY", "BAD_PARAMS"]
+__all__ = ["SlotStore", "SweepStore", "assemble_sweeps", "choose_sweeps", "time_lag", "OVERFLOW", "BAD_ENTRY",
+           "BAD_PARAMS"]
 
 NONE, KEY, SWEEP, PAD = 0, 1, 2, 3            # BEVB200_SWEEP_*
 MAX_DIM = 8                                   # BEVB200_SWEEP_MAX_DIM: F <= 8, as the fused voxelizer takes
@@ -70,28 +71,21 @@ def _check_loader_options(reduce_beams, load_augmented):
         raise ValueError("load_augmented=%r is not supported" % load_augmented)
 
 
-class SweepStore:
-    """Raw LiDAR rows on the device, one sweep (or key) per slot, and the parameter block of the frame being
-    assembled.  max_batch and max_entries size the block: a sample has at most max_entries entries (its key and its
-    sweeps or pad copies)."""
+class SlotStore:
+    """Raw sweep rows on the device, one sweep per slot ([slots, slot_cap, load_dim] fp32 plus a device row count per
+    slot), and a device block of block_bytes for the parameters of the frame being assembled.  SweepStore and
+    radar_sweeps.RadarSweepStore build on it."""
 
-    def __init__(self, slots, slot_cap, load_dim=5, device="cuda", max_batch=4, max_entries=11):
-        if slots < 1 or slot_cap < 1 or max_batch < 1 or max_entries < 1:
-            raise ValueError("slots, slot_cap, max_batch and max_entries must be positive")
-        if not 3 <= load_dim <= 64:
-            raise ValueError("load_dim must be in 3..64, got %d" % load_dim)
-        if max_entries * slot_cap >= 2 ** 31:
-            raise ValueError("max_entries * slot_cap must be below 2^31")
+    def __init__(self, slots, slot_cap, load_dim, device, block_bytes):
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise ValueError("SweepStore lives on a CUDA device: bevfusion_b200 has no CPU implementation")
+            raise ValueError("%s lives on a CUDA device: bevfusion_b200 has no CPU implementation"
+                             % type(self).__name__)
         self.slots, self.slot_cap, self.load_dim = int(slots), int(slot_cap), int(load_dim)
-        self.max_batch, self.max_entries = int(max_batch), int(max_entries)
         self.rows = torch.zeros((slots, slot_cap, load_dim), dtype=torch.float32, device=self.device)
         self.slot_rows = torch.zeros((slots,), dtype=torch.int32, device=self.device)
         self.host_rows = [0] * slots          # what put() stored, for the default cap
-        nbytes = _ENTRIES_AT + max_batch * max_entries * ENTRY_DTYPE.itemsize
-        self.block = torch.empty((nbytes,), dtype=torch.uint8, device=self.device)
+        self.block = torch.empty((block_bytes,), dtype=torch.uint8, device=self.device)
 
     def put(self, slot, points):
         """Store `points` [n, load_dim] fp32 (pinned host or CUDA; other host memory is copied synchronously) in
@@ -111,6 +105,28 @@ class SweepStore:
                 self.rows[slot, :n].copy_(points, non_blocking=True)
             self.slot_rows[slot:slot + 1].fill_(n)
         self.host_rows[slot] = n
+
+    def _write_block(self, host):
+        # one pinned asynchronous copy into the block the assemble launches read
+        with torch.cuda.device(self.device):
+            self.block[:host.size].copy_(torch.from_numpy(host).pin_memory(), non_blocking=True)
+
+
+class SweepStore(SlotStore):
+    """Raw LiDAR rows on the device, one sweep (or key) per slot, and the parameter block of the frame being
+    assembled.  max_batch and max_entries size the block: a sample has at most max_entries entries (its key and its
+    sweeps or pad copies)."""
+
+    def __init__(self, slots, slot_cap, load_dim=5, device="cuda", max_batch=4, max_entries=11):
+        if slots < 1 or slot_cap < 1 or max_batch < 1 or max_entries < 1:
+            raise ValueError("slots, slot_cap, max_batch and max_entries must be positive")
+        if not 3 <= load_dim <= 64:
+            raise ValueError("load_dim must be in 3..64, got %d" % load_dim)
+        if max_entries * slot_cap >= 2 ** 31:
+            raise ValueError("max_entries * slot_cap must be below 2^31")
+        self.max_batch, self.max_entries = int(max_batch), int(max_entries)
+        super().__init__(slots, slot_cap, load_dim, device,
+                         _ENTRIES_AT + max_batch * max_entries * ENTRY_DTYPE.itemsize)
 
     def _pack(self, samples, use_dim, key_use_dim, sweeps_num, pad_empty_sweeps, remove_close, point_cloud_range,
               radius):
@@ -166,8 +182,7 @@ class SweepStore:
         _check_loader_options(reduce_beams, load_augmented)
         host, F, bound = self._pack(samples, use_dim, key_use_dim, sweeps_num, pad_empty_sweeps, remove_close,
                                     point_cloud_range, radius)
-        with torch.cuda.device(self.device):
-            self.block[:host.size].copy_(torch.from_numpy(host).pin_memory(), non_blocking=True)
+        self._write_block(host)
         return len(samples), F, bound
 
     def launch(self, batch, out_dim, cap):

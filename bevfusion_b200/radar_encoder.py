@@ -212,13 +212,17 @@ class RadarEncoder(nn.Module):
         x = self.pts_voxel_encoder(feats, sizes, coords)
         return self.pts_middle_encoder(x, coords, batch_size)
 
-    def forward_points(self, points_list, voxelize, return_voxel_num=False):
+    def forward_points(self, points_list, voxelize, return_voxel_num=False, num_points=None):
         """Voxelize (hard, `voxelize` = Voxelization) -> radar net -> scatter for each sample of
         `points_list` ([N_k, F] fp32 CUDA tensors), straight into one zeroed [B, C, nx, ny] canvas.
         Same result as voxelize_batch(voxelize_reduce=False) -> forward(), bit for bit, without the
         [M, P, F] voxel tensor and without a host synchronisation (CUDA-graph capturable).  Eval mode
         and no autograd only; the voxel grid must be (nx, ny, 1).  return_voxel_num: also return the
-        device int32 [B] pillar counts."""
+        device int32 [B] pillar counts.
+
+        num_points (device int32 [B]): points_list is one padded [B, cap, F] tensor (RadarSweepStore.assemble with
+        sync=False) and sample k is its first num_points[k] rows, read on the device only; the result equals the
+        call on [points[k, :num_points[k]] for k in range(B)]."""
         enc, scat = self.pts_voxel_encoder, self.pts_middle_encoder
         if not isinstance(voxelize, Voxelization) or voxelize.max_num_points <= 0:
             raise ValueError("forward_points needs a hard Voxelization module")
@@ -232,10 +236,18 @@ class RadarEncoder(nn.Module):
         if not enc.native_supported(P):
             raise ValueError("forward_points needs a native radar net shape (1..4 layers of widths that are "
                              "multiples of 16 up to 128, F + 2 <= 128, P <= 32)")
-        for k, pts in enumerate(points_list):
-            _C.require_cuda(pts, "points[%d]" % k, torch.float32)
-            if pts.dim() != 2 or pts.shape[1] != enc.in_channels:
-                raise ValueError("points[%d] must be [N, %d]" % (k, enc.in_channels))
+        if num_points is not None:
+            _C.require_cuda(points_list, "points", torch.float32)
+            _C.require_cuda(num_points, "num_points", torch.int32)
+            if points_list.dim() != 3 or points_list.shape[2] != enc.in_channels:
+                raise ValueError("points must be [B, cap, %d] with num_points" % enc.in_channels)
+            if num_points.shape != (points_list.shape[0],) or num_points.device != points_list.device:
+                raise ValueError("num_points must be int32 [B] on the points' device")
+        else:
+            for k, pts in enumerate(points_list):
+                _C.require_cuda(pts, "points[%d]" % k, torch.float32)
+                if pts.dim() != 2 or pts.shape[1] != enc.in_channels:
+                    raise ValueError("points[%d] must be [N, %d]" % (k, enc.in_channels))
         dev = points_list[0].device
         B, C, L = len(points_list), enc.rfn_layers[-1].units, len(enc.rfn_layers)
         packed = enc.packed_weights()
@@ -249,10 +261,13 @@ class RadarEncoder(nn.Module):
             nbytes = _C.lib().bevb200_hard_voxelize_radar_workspace_bytes(nmax, P)
             ws = torch.empty(max(nbytes, 256), dtype=torch.uint8, device=dev)
             for k, pts in enumerate(points_list):
-                rc = _C.lib().bevb200_hard_voxelize_radar(
-                    _C.ptr(pts), int(pts.shape[0]), enc.in_channels, ctypes.cast(vs, ctypes.c_void_p),
-                    ctypes.cast(cr, ctypes.c_void_p), P, mv, L, enc._widths(), *geom, _C.ptr(packed),
-                    _C.ptr(canvas[k]), int(scat.nx), int(scat.ny), _C.ptr(voxel_num[k:k + 1]), _C.ptr(ws),
-                    ws.numel(), _C.current_stream(dev))
+                args = (enc.in_channels, ctypes.cast(vs, ctypes.c_void_p), ctypes.cast(cr, ctypes.c_void_p), P, mv, L,
+                        enc._widths(), *geom, _C.ptr(packed), _C.ptr(canvas[k]), int(scat.nx), int(scat.ny),
+                        _C.ptr(voxel_num[k:k + 1]), _C.ptr(ws), ws.numel(), _C.current_stream(dev))
+                if num_points is None:
+                    rc = _C.lib().bevb200_hard_voxelize_radar(_C.ptr(pts), int(pts.shape[0]), *args)
+                else:
+                    rc = _C.lib().bevb200_hard_voxelize_radar_dev(_C.ptr(pts), _C.ptr(num_points[k:k + 1]),
+                                                                  int(pts.shape[0]), *args)
                 _C.check(rc, "hard_voxelize_radar")
         return (canvas, voxel_num) if return_voxel_num else canvas

@@ -463,6 +463,18 @@ BEVB200_API int bevb200_hard_voxelize_radar(const float *points, int num_points,
                                             int ny, int32_t *voxel_num, void *workspace, size_t workspace_bytes,
                                             void *stream);
 
+/* bevb200_hard_voxelize_radar on the first *num_points_dev (DEVICE int32[1], clamped to [0, max_rows]) rows of
+ * points [max_rows, F]: the same canvas and voxel_num, bit for bit, as bevb200_hard_voxelize_radar with that host
+ * count, without reading the count on the host (a device count of 0 leaves the canvas as it is and sets voxel_num
+ * to 0).  Workspace: bevb200_hard_voxelize_radar_workspace_bytes(max_rows, P) device bytes. */
+BEVB200_API int bevb200_hard_voxelize_radar_dev(const float *points, const int32_t *num_points_dev, int max_rows,
+                                                int num_features, const float *voxel_size_host,
+                                                const float *coors_range_host, int max_points, int max_voxels,
+                                                int n_layers, const int *widths, float vx, float vy, float x_off,
+                                                float y_off, const float *pc_min, const float *pc_span,
+                                                const void *packed, float *canvas, int nx, int ny, int32_t *voxel_num,
+                                                void *workspace, size_t workspace_bytes, void *stream);
+
 /* ---- Rotated BEV IoU and NMS (mmdet3d/ops/iou3d/src/{iou3d.cpp,iou3d_kernel.cu},
  *      core/post_processing/box3d_nms.py:180-219 circle_nms) ----------------------------------------
  * Boxes are [x1, y1, x2, y2, ry] fp32 (xywhr2xyxyr form): the axis-aligned extent turned by ry about its
@@ -1405,6 +1417,70 @@ BEVB200_API size_t bevb200_lidar_sweeps_workspace_bytes(int batch, int max_entri
 BEVB200_API int bevb200_lidar_sweeps_assemble(const float *store, int slots, int slot_cap, int load_dim,
                                               const int32_t *slot_rows, const bevb200_sweep_params_t *params,
                                               const bevb200_sweep_entry_t *entries, int batch, int max_entries,
+                                              int out_dim, int cap, float *out, int32_t *counts, int32_t *status,
+                                              void *workspace, size_t workspace_bytes, void *stream);
+
+/* ---- LoadRadarPointsMultiSweeps + the radar face of PointsRangeFilter (loading.py:717-790,
+ *      transforms_3d.py:607-612, radar_points.py:92-107) -----------------------------------------------------------
+ * store [slots, slot_cap, 18] fp32 holds raw radar rows (DEVICE), slot_rows [slots] int32 (DEVICE) the rows of each
+ * slot.  For each of `batch` samples, entries [batch, max_entries] (DEVICE) lists its sweeps in the reference's
+ * concatenation order (radars in the order of results['radar'], within each its first min(len, sweeps_num) sweeps);
+ * kind is BEVB200_SWEEP_SWEEP, or BEVB200_SWEEP_NONE for unused entries.  Per raw row r, with R, t and td the entry's
+ * rotation, translation and time_diff and chain_j(p) = fma(p2, R[j][2], fma(p1, R[j][1], fma(p0, R[j][0], +0.0)))
+ * in float64, the reference's 58-column float64 row is
+ *   0-2    x_j = fl32(fl32(chain_j(r0, r1, r2)) + t[j]); with compensate_velocity x_j = fl32(x_j + vc_j * td), j < 2
+ *   3-5, 10-17  the raw values          6-7  velo_j = chain_j(r6, r7, +0)      8-9  vc_j = chain_j(r8, r9, +0)
+ *   18     td                            19-26, 27-31, 32-49  one-hot of rint(r3) (8), rint(r11) (5), rint(r14) (18)
+ *   50-56  rint(r15) > i, i = 0..6       57   r14 == 0 && r3 < 7 && r11 == 3
+ * (rint rounds half to even; one-hot indices in [-w, -1] wrap as numpy's do).  params (DEVICE) gives, per output
+ * column c < out_dim, an op code naming one of these values (kind | arg << 8 | block << 16, plus
+ * BEVB200_RADAR_OP_NORMALIZE for (v - norm_min[c]) / norm_span[c] in float64), then fl32; with has_range a row is
+ * kept iff range[0] < out[0] < range[2] and range[1] < out[1] < range[3] in fp32 (NaN is dropped).  out [batch, cap,
+ * out_dim] receives each sample's kept rows in order, counts [batch] int32 (DEVICE) min(kept, cap); rows past
+ * counts[b] are left untouched and nothing is written past cap.  status [1] int32 (DEVICE) is zeroed, then gets
+ *   BEVB200_SWEEPS_OVERFLOW              a sample kept more than cap rows (its first cap rows are written)
+ *   BEVB200_SWEEPS_BAD_ENTRY             an entry has an unknown kind or a slot outside [0, slots) (no rows)
+ *   BEVB200_SWEEPS_BAD_PARAMS            an op code of the first out_dim columns is malformed (no sample gets rows)
+ *   BEVB200_RADAR_SWEEPS_BAD_CATEGORY    a row's one-hot source is NaN or rounds outside [-w, w), where the
+ *                                        reference raises IndexError; that block of the row stays zero
+ * Three launches sized by (batch, max_entries, slot_cap), no atomics on the output order, no host synchronisation:
+ * CUDA-graph capturable with the store, params and entries refreshed between replays.  Sizes: 3 <= out_dim <= 64,
+ * cap >= 1, cap * out_dim < 2^31, batch <= 65535, max_entries <= 65535, max_entries * slot_cap < 2^31.  Workspace:
+ * bevb200_radar_sweeps_workspace_bytes(batch, max_entries, slot_cap) (0 for unsupported sizes): one int32 per
+ * 128-row tile; a smaller one gives BEVB200_EWORKSPACE before any write. */
+#define BEVB200_RADAR_LOAD_DIM 18
+#define BEVB200_RADAR_SWEEP_MAX_DIM 64
+#define BEVB200_RADAR_OP_RAW 0          /* arg: raw column */
+#define BEVB200_RADAR_OP_XYZ 1          /* arg: j in 0..2 */
+#define BEVB200_RADAR_OP_VELO 2         /* arg: j in 0..1 */
+#define BEVB200_RADAR_OP_VELO_COMP 3    /* arg: j in 0..1 */
+#define BEVB200_RADAR_OP_LAG 4
+#define BEVB200_RADAR_OP_ONE_HOT 5      /* block: 0 (r3, 8), 1 (r11, 5), 2 (r14, 18); arg: the value */
+#define BEVB200_RADAR_OP_ORDINAL 6      /* arg: the threshold i */
+#define BEVB200_RADAR_OP_NUSC 7
+#define BEVB200_RADAR_OP_NORMALIZE (1 << 24)
+#define BEVB200_RADAR_SWEEPS_BAD_CATEGORY 8
+#define BEVB200_RADAR_SWEEP_ENTRY_BYTES 112
+#define BEVB200_RADAR_SWEEP_PARAMS_BYTES 1304
+typedef struct {
+  int32_t kind;              /* BEVB200_SWEEP_SWEEP or BEVB200_SWEEP_NONE */
+  int32_t slot;
+  double rotation[9];        /* sensor2lidar_rotation, row-major */
+  double translation[3];     /* sensor2lidar_translation */
+  double time_diff;          /* sweeps[0]['timestamp'] * 1e-6 - sweep['timestamp'] * 1e-6 */
+} bevb200_radar_sweep_entry_t;
+typedef struct {
+  double norm_min[BEVB200_RADAR_SWEEP_MAX_DIM];    /* normalize_dims min, as float64 */
+  double norm_span[BEVB200_RADAR_SWEEP_MAX_DIM];   /* max - min, computed as Python does */
+  int32_t ops[BEVB200_RADAR_SWEEP_MAX_DIM];        /* per output column: the op code above */
+  int32_t compensate_velocity;
+  int32_t has_range;
+  float range[4];                                  /* fl32(x_min, y_min, x_max, y_max) */
+} bevb200_radar_sweep_params_t;
+BEVB200_API size_t bevb200_radar_sweeps_workspace_bytes(int batch, int max_entries, int slot_cap);
+BEVB200_API int bevb200_radar_sweeps_assemble(const float *store, int slots, int slot_cap, const int32_t *slot_rows,
+                                              const bevb200_radar_sweep_params_t *params,
+                                              const bevb200_radar_sweep_entry_t *entries, int batch, int max_entries,
                                               int out_dim, int cap, float *out, int32_t *counts, int32_t *status,
                                               void *workspace, size_t workspace_bytes, void *stream);
 
