@@ -31,10 +31,19 @@ def _first_argmax(v):
     return v.argmax(axis=1)  # numpy returns the first index attaining the max
 
 
+def inside_canvas(coors, canvas_shape):
+    """[M] bool: the pillar's (b, x, y) lies on the canvas.  Pillars off it count in both BNs but write nothing
+    and take no gradient."""
+    c = np.asarray(coors, np.int64)
+    B, _, nx, ny = canvas_shape
+    return (c[:, 0] >= 0) & (c[:, 0] < B) & (c[:, 1] >= 0) & (c[:, 1] < nx) & (c[:, 2] >= 0) & (c[:, 2] < ny)
+
+
 def train_step(features, num_voxels, coors, params, geom, canvas_shape, grad_canvas, eps=1e-3, momentum=0.01):
     """features [M, P, F], num_voxels [M], coors [M, 4] (b, x, y, z); params: W1 [32, F+5], W2 [64, 64], g1, b1,
     g2, b2, rm1, rv1, rm2, rv2 (running statistics); geom (vx, vy, x_offset, y_offset); grad_canvas [B, 64, nx, ny].
-    Returns a dict: canvas, dW1, dW2, dg1, db1, dg2, db2, rm1, rv1, rm2, rv2 (updated)."""
+    Returns a dict: canvas, dW1, dW2, dg1, db1, dg2, db2, rm1, rv1, rm2, rv2 (updated), and the batch statistics
+    mu1, var1, mu2, var2."""
     x = np.asarray(features, np.float64)
     num = np.asarray(num_voxels, np.int64)
     c = np.asarray(coors, np.int64)
@@ -43,6 +52,7 @@ def train_step(features, num_voxels, coors, params, geom, canvas_shape, grad_can
     g1, b1, g2, b2 = (np.asarray(params[k], np.float64) for k in ("g1", "b1", "g2", "b2"))
     W2a, W2b = W2[:, :32], W2[:, 32:]
     gc = np.asarray(grad_canvas, np.float64)
+    ins = inside_canvas(c, canvas_shape)
     N = float(m * p)
     blocks = [(i, min(i + BLOCK, m)) for i in range(0, m, BLOCK)]
 
@@ -92,8 +102,9 @@ def train_step(features, num_voxels, coors, params, geom, canvas_shape, grad_can
         return np.take_along_axis(a, idx[:, None, :], axis=1)[:, 0, :]
 
     def g2_of(i0, i1, pre2, am2):
-        cc = c[i0:i1]
-        G = gc[cc[:, 0], :, cc[:, 1], cc[:, 2]]
+        cc, k = c[i0:i1], ins[i0:i1]
+        G = np.zeros((i1 - i0, gc.shape[1]))
+        G[k] = gc[cc[k, 0], :, cc[k, 1], cc[k, 2]]
         g2 = np.zeros_like(pre2)
         np.put_along_axis(g2, am2[:, None, :], G[:, None, :], axis=1)
         return g2 * (pre2 > 0)
@@ -104,8 +115,8 @@ def train_step(features, num_voxels, coors, params, geom, canvas_shape, grad_can
     for i0, i1 in blocks:
         h, w = rows(i0, i1)
         *_, z2, pre2, y2, am2 = layer2_full(h)
-        cc = c[i0:i1]
-        canvas[cc[:, 0], :, cc[:, 1], cc[:, 2]] = y2.max(axis=1)
+        cc, k = c[i0:i1], ins[i0:i1]
+        canvas[cc[k, 0], :, cc[k, 1], cc[k, 2]] = y2.max(axis=1)[k]
         gg2 = g2_of(i0, i1, pre2, am2)
         xh2 = (z2 - mu2) * inv2
         sg2 += (w * gg2).sum(axis=(0, 1)); sgx2 += (w * gg2 * xh2).sum(axis=(0, 1))
@@ -139,7 +150,8 @@ def train_step(features, num_voxels, coors, params, geom, canvas_shape, grad_can
         dz1 = g1 * inv1 * (gg1 - sg1 / N - xh1 * sgx1 / N)
         dW1 += np.einsum("vsc,vsj->cj", dz1, h)
 
-    out = dict(canvas=canvas, dW1=dW1, dW2=dW2, dg1=sgx1, db1=sg1, dg2=sgx2, db2=sg2)
+    out = dict(canvas=canvas, dW1=dW1, dW2=dW2, dg1=sgx1, db1=sg1, dg2=sgx2, db2=sg2, mu1=mu1, var1=var1, mu2=mu2,
+               var2=var2)
     for k, mu, var in (("1", mu1, var1), ("2", mu2, var2)):
         out["rm" + k] = (1 - momentum) * np.asarray(params["rm" + k], np.float64) + momentum * mu
         out["rv" + k] = (1 - momentum) * np.asarray(params["rv" + k], np.float64) + momentum * var * N / (N - 1)
@@ -154,3 +166,19 @@ def params_from_state_dict(sd, prefix=""):
                 g2=sd[k % 1 + "norm.weight"], b2=sd[k % 1 + "norm.bias"],
                 rm1=sd[k % 0 + "norm.running_mean"], rv1=sd[k % 0 + "norm.running_var"],
                 rm2=sd[k % 1 + "norm.running_mean"], rv2=sd[k % 1 + "norm.running_var"])
+
+
+def slot_values(features, num_voxels, coors, params, geom, out, eps=1e-3):
+    """Per-slot values of a step whose batch statistics train_step returned in `out`: decorated rows h [M, P, F+5]
+    (zero past n), BN-normalised pre-activations pre1 [M, P, 32] and pre2 [M, P, 64], y1 and the layer-1 max m1."""
+    x = np.asarray(features, np.float64)
+    num = np.asarray(num_voxels, np.int64)
+    h = _decorate(x, num.astype(np.float64), np.asarray(coors, np.float64), geom)
+    W1, W2 = (np.asarray(params[k], np.float64) for k in ("W1", "W2"))
+    g1, b1, g2, b2 = (np.asarray(params[k], np.float64) for k in ("g1", "b1", "g2", "b2"))
+    pre1 = (h @ W1.T - out["mu1"]) / np.sqrt(out["var1"] + eps) * g1 + b1
+    y1 = np.maximum(pre1, 0.0)
+    m1 = y1.max(axis=1)
+    z2 = y1 @ W2[:, :32].T + (m1 @ W2[:, 32:].T)[:, None, :]
+    pre2 = (z2 - out["mu2"]) / np.sqrt(out["var2"] + eps) * g2 + b2
+    return h, pre1, y1, m1, pre2
