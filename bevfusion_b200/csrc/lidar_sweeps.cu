@@ -11,10 +11,13 @@
 //                           the reference's concatenation order; the sample's count is min(total, cap).
 //   3. sweeps_write_kernel  the grid of 1: each kept row is recomputed and written at its tile offset plus its rank
 //                           in the tile (ballot ranks, no atomics), if that is below cap.
+// With a per-sample augmentation record (GlobalRotScaleTrans + RandomFlip3D, lidar_aug.cuh), eval_row applies it to
+// the row's x, y, z before the range test, in both the count and the write kernel, so counts and rows agree.
 // The double expressions are written with _rn intrinsics, so nvcc cannot contract them differently from the FMA chain
 // numpy's dgemm evaluates (see DESIGN.md section 4.27).
 #include <math.h>
 
+#include "lidar_aug.cuh"
 #include "sweeps_scan.cuh"
 
 static_assert(sizeof(bevb200_sweep_entry_t) == BEVB200_SWEEP_ENTRY_BYTES, "entry layout");
@@ -33,6 +36,7 @@ struct Frame {
   const int32_t *slot_rows;
   const bevb200_sweep_params_t *params;
   const bevb200_sweep_entry_t *entries;
+  const bevb200_lidar_aug_t *aug;   // [batch] or NULL
   int slots, slot_cap, load_dim, max_entries, out_dim, tiles;
 };
 
@@ -57,9 +61,11 @@ __device__ __forceinline__ int entry_rows(const Frame &f, const bevb200_sweep_en
   return min(max(f.slot_rows[e.slot], 0), f.slot_cap);
 }
 
-// One row of an entry: its output columns and whether it survives remove_close and the range filter
+// One row of an entry: its output columns and whether it survives remove_close, the augmentation and the range
+// filter
 __device__ __forceinline__ bool eval_row(const float *__restrict__ src, const bevb200_sweep_entry_t &e,
-                                         const bevb200_sweep_params_t &p, int out_dim, float v[8]) {
+                                         const bevb200_sweep_params_t &p, const bevb200_lidar_aug_t &a, int out_dim,
+                                         float v[8]) {
   const bool sweep = e.kind == BEVB200_SWEEP_SWEEP;
 #pragma unroll
   for (int c = 0; c < 8; ++c) v[c] = c < out_dim ? __ldg(src + (sweep ? p.sweep_cols[c] : p.key_cols[c])) : 0.f;
@@ -82,17 +88,20 @@ __device__ __forceinline__ bool eval_row(const float *__restrict__ src, const be
   } else {
     v[4] = 0.0f;
   }
+  aug_point<false>(a, v);
   if (p.has_range)   // in_range_3d: strict fp32 comparisons, NaN fails them all
     return v[0] > p.range[0] && v[1] > p.range[1] && v[2] > p.range[2] && v[0] < p.range[3] && v[1] < p.range[4] &&
            v[2] < p.range[5];
   return true;
 }
 
+template <bool kAug>
 __global__ void __launch_bounds__(kThreads)
 sweeps_count_kernel(Frame f, int32_t *__restrict__ tile_counts, int32_t *__restrict__ status) {
   const int t = blockIdx.x, ei = blockIdx.z * f.max_entries + blockIdx.y;
   const bevb200_sweep_entry_t e = f.entries[ei];
   const bevb200_sweep_params_t p = *f.params;
+  const bevb200_lidar_aug_t a = aug_record(kAug ? f.aug : nullptr, blockIdx.z);
   bool bad;
   int n = entry_rows(f, e, &bad);
   const bool pbad = !params_ok(p, f.load_dim, f.out_dim);
@@ -106,7 +115,7 @@ sweeps_count_kernel(Frame f, int32_t *__restrict__ tile_counts, int32_t *__restr
     for (int r = 0; r < kRounds; ++r) {
       const int i = row0 + r * kThreads + threadIdx.x;
       float v[8];
-      kept += __syncthreads_count(i < n && eval_row(base + (size_t)i * f.load_dim, e, p, f.out_dim, v));
+      kept += __syncthreads_count(i < n && eval_row(base + (size_t)i * f.load_dim, e, p, a, f.out_dim, v));
     }
   }
   if (threadIdx.x == 0) tile_counts[(size_t)ei * f.tiles + t] = kept;
@@ -146,12 +155,14 @@ sweeps_scan_kernel(int32_t *__restrict__ tile_counts, int len, int cap, int32_t 
   }
 }
 
+template <bool kAug>
 __global__ void __launch_bounds__(kThreads)
 sweeps_write_kernel(Frame f, const int32_t *__restrict__ tile_offsets, int cap, float *__restrict__ out) {
   __shared__ int warp_sum[kThreads / 32];
   const int t = blockIdx.x, ei = blockIdx.z * f.max_entries + blockIdx.y;
   const bevb200_sweep_entry_t e = f.entries[ei];
   const bevb200_sweep_params_t p = *f.params;
+  const bevb200_lidar_aug_t a = aug_record(kAug ? f.aug : nullptr, blockIdx.z);
   bool bad;
   const int n = params_ok(p, f.load_dim, f.out_dim) ? entry_rows(f, e, &bad) : 0;
   const int row0 = t * kTile;
@@ -163,7 +174,7 @@ sweeps_write_kernel(Frame f, const int32_t *__restrict__ tile_offsets, int cap, 
   for (int r = 0; r < kRounds; ++r) {
     const int i = row0 + r * kThreads + threadIdx.x;
     float v[8];
-    const bool keep = i < n && eval_row(base + (size_t)i * f.load_dim, e, p, f.out_dim, v);
+    const bool keep = i < n && eval_row(base + (size_t)i * f.load_dim, e, p, a, f.out_dim, v);
     const unsigned m = __ballot_sync(0xffffffffu, keep);
     if (lane == 0) warp_sum[warp] = __popc(m);
     __syncthreads();
@@ -215,6 +226,16 @@ int bevb200_lidar_sweeps_assemble(const float *store, int slots, int slot_cap, i
                                   const bevb200_sweep_params_t *params, const bevb200_sweep_entry_t *entries,
                                   int batch, int max_entries, int out_dim, int cap, float *out, int32_t *counts,
                                   int32_t *status, void *workspace, size_t workspace_bytes, void *stream) {
+  return bevb200_lidar_sweeps_assemble_aug(store, slots, slot_cap, load_dim, slot_rows, params, entries, nullptr,
+                                           batch, max_entries, out_dim, cap, out, counts, status, workspace,
+                                           workspace_bytes, stream);
+}
+
+int bevb200_lidar_sweeps_assemble_aug(const float *store, int slots, int slot_cap, int load_dim,
+                                      const int32_t *slot_rows, const bevb200_sweep_params_t *params,
+                                      const bevb200_sweep_entry_t *entries, const bevb200_lidar_aug_t *aug, int batch,
+                                      int max_entries, int out_dim, int cap, float *out, int32_t *counts,
+                                      int32_t *status, void *workspace, size_t workspace_bytes, void *stream) {
   BEVB200_REQUIRE(sizes_ok(batch, max_entries, slot_cap) && slots >= 1,
                   "sizes out of range (0 <= batch <= 65535, 1 <= max_entries <= 65535, slots >= 1, slot_cap >= 1, "
                   "max_entries * slot_cap < 2^31)");
@@ -230,21 +251,25 @@ int bevb200_lidar_sweeps_assemble(const float *store, int slots, int slot_cap, i
   BEVB200_REQUIRE((uintptr_t)entries % alignof(bevb200_sweep_entry_t) == 0 &&
                       (uintptr_t)params % alignof(bevb200_sweep_params_t) == 0,
                   "misaligned parameter block");
+  BEVB200_REQUIRE((uintptr_t)aug % alignof(bevb200_lidar_aug_t) == 0, "misaligned augmentation records");
   const size_t need = bevb200_lidar_sweeps_workspace_bytes(batch, max_entries, slot_cap);
   if (!workspace || workspace_bytes < need) {
     snprintf(g_last_error, sizeof(g_last_error), "%s: workspace of %zu bytes, need %zu", __func__, workspace_bytes,
              need);
     return BEVB200_EWORKSPACE;
   }
-  Frame f{store, slot_rows, params, entries, slots, slot_cap, load_dim, max_entries, out_dim, tiles_for(slot_cap)};
+  Frame f{store, slot_rows, params, entries, aug, slots, slot_cap, load_dim, max_entries, out_dim, tiles_for(slot_cap)};
   int32_t *tiles = (int32_t *)workspace;
   cudaStream_t st = (cudaStream_t)stream;
   BEVB200_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t), st));
   const dim3 grid(f.tiles, max_entries, batch);
-  BEVB200_LAUNCH(sweeps_count_kernel, grid, kThreads, 0, st, f, tiles, status);
+  // the plain path is its own instance, with the registers it had before the augmentation existed
+  const auto count_kernel = aug ? sweeps_count_kernel<true> : sweeps_count_kernel<false>;
+  const auto write_kernel = aug ? sweeps_write_kernel<true> : sweeps_write_kernel<false>;
+  BEVB200_LAUNCH(count_kernel, grid, kThreads, 0, st, f, tiles, status);
   const int rc = sweeps_scan(tiles, batch, max_entries * f.tiles, cap, counts, status, st);
   if (rc) return rc;
-  BEVB200_LAUNCH(sweeps_write_kernel, grid, kThreads, 0, st, f, tiles, cap, out);
+  BEVB200_LAUNCH(write_kernel, grid, kThreads, 0, st, f, tiles, cap, out);
   return BEVB200_OK;
 }
 

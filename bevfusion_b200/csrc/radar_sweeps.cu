@@ -13,10 +13,14 @@
 //   3. radar_write_kernel  the grid of 1: each kept row's output columns go to shared memory at its ballot rank in
 //                          the tile, then the tile's kept rows, consecutive in the output, are stored with
 //                          consecutive threads on consecutive floats.
+// With a per-sample augmentation record (GlobalRotScaleTrans + RandomFlip3D, lidar_aug.cuh), output columns 0..4 are
+// computed first and augmented as RadarPoints does, and the range test reads the augmented x, y; the count and the
+// write kernel share aug_head, so counts and rows agree.
 // The double expressions are written with _rn intrinsics, so nvcc cannot contract them differently from the FMA
 // chain numpy's dgemm evaluates (DESIGN.md sections 4.27, 4.28).
 #include <math.h>
 
+#include "lidar_aug.cuh"
 #include "sweeps_scan.cuh"
 
 static_assert(sizeof(bevb200_radar_sweep_entry_t) == BEVB200_RADAR_SWEEP_ENTRY_BYTES, "entry layout");
@@ -37,6 +41,7 @@ struct Frame {
   const int32_t *slot_rows;
   const bevb200_radar_sweep_params_t *params;
   const bevb200_radar_sweep_entry_t *entries;
+  const bevb200_lidar_aug_t *aug;   // [batch] or NULL; out_dim >= 5 when set
   int slots, slot_cap, max_entries, out_dim, tiles;
 };
 
@@ -161,16 +166,28 @@ __device__ __forceinline__ bool in_range(const float *__restrict__ src, const De
   return x > p->range[0] && y > p->range[1] && x < p->range[2] && y < p->range[3];
 }
 
+// with an enabled record: output columns 0..4 augmented into v, and in_range_bev on the augmented x, y
+__device__ __forceinline__ bool aug_head(const float *__restrict__ src, const Derived &d,
+                                         const bevb200_radar_sweep_params_t *__restrict__ p,
+                                         const bevb200_lidar_aug_t &a, float v[5]) {
+#pragma unroll
+  for (int c = 0; c < 5; ++c) v[c] = column(src, d, p, c);
+  aug_point<true>(a, v);
+  return !p->has_range || (v[0] > p->range[0] && v[1] > p->range[1] && v[0] < p->range[2] && v[1] < p->range[3]);
+}
+
 // every thread of the CTA: whether the op codes of the first out_dim columns are malformed
 __device__ __forceinline__ bool params_bad(const Frame &f) {
   return __syncthreads_or(threadIdx.x < f.out_dim && !op_ok(__ldg(f.params->ops + threadIdx.x)));
 }
 
+template <bool kAug>
 __global__ void __launch_bounds__(kThreads)
 radar_count_kernel(Frame f, int32_t *__restrict__ tile_counts, int32_t *__restrict__ status) {
   const int t = blockIdx.x, ei = blockIdx.z * f.max_entries + blockIdx.y;
   const bevb200_radar_sweep_entry_t e = f.entries[ei];
   const bevb200_radar_sweep_params_t *p = f.params;
+  const bevb200_lidar_aug_t a = aug_record(kAug ? f.aug : nullptr, blockIdx.z);
   bool bad;
   int n = entry_rows(f, e, &bad);
   const bool pbad = params_bad(f);
@@ -183,13 +200,15 @@ radar_count_kernel(Frame f, int32_t *__restrict__ tile_counts, int32_t *__restri
     const float *src = f.store + ((size_t)e.slot * f.slot_cap + i) * kLoadDim;
     const Derived d = derive(src, e, p->compensate_velocity != 0);
     bad_category = d.hot0 < 0 || d.hot1 < 0 || d.hot2 < 0;
-    keep = in_range(src, d, p);
+    float v[5];
+    keep = a.enabled ? aug_head(src, d, p, a, v) : in_range(src, d, p);
   }
   const int kept = __syncthreads_count(keep);
   if (__syncthreads_or(bad_category) && threadIdx.x == 0) atomicOr(status, BEVB200_RADAR_SWEEPS_BAD_CATEGORY);
   if (threadIdx.x == 0) tile_counts[(size_t)ei * f.tiles + t] = kept;
 }
 
+template <bool kAug>
 __global__ void __launch_bounds__(kThreads)
 radar_write_kernel(Frame f, const int32_t *__restrict__ tile_offsets, int cap, float *__restrict__ out) {
   __shared__ float rows[kTile * kPitch];
@@ -197,6 +216,7 @@ radar_write_kernel(Frame f, const int32_t *__restrict__ tile_offsets, int cap, f
   const int t = blockIdx.x, ei = blockIdx.z * f.max_entries + blockIdx.y;
   const bevb200_radar_sweep_entry_t e = f.entries[ei];
   const bevb200_radar_sweep_params_t *p = f.params;
+  const bevb200_lidar_aug_t a = aug_record(kAug ? f.aug : nullptr, blockIdx.z);
   bool bad;
   const int n = params_bad(f) ? 0 : entry_rows(f, e, &bad);
   const int row0 = t * kTile, off = tile_offsets[(size_t)ei * f.tiles + t];
@@ -204,10 +224,11 @@ radar_write_kernel(Frame f, const int32_t *__restrict__ tile_offsets, int cap, f
   const int i = row0 + threadIdx.x, D = f.out_dim, pitch = D | 1;
   const float *src = f.store + ((size_t)e.slot * f.slot_cap + i) * kLoadDim;
   Derived d;
+  float v[5];
   bool keep = false;
   if (i < n) {
     d = derive(src, e, p->compensate_velocity != 0);
-    keep = in_range(src, d, p);
+    keep = a.enabled ? aug_head(src, d, p, a, v) : in_range(src, d, p);
   }
   const int lane = lane_id(), warp = threadIdx.x >> 5;
   const unsigned m = __ballot_sync(0xffffffffu, keep);
@@ -222,8 +243,14 @@ radar_write_kernel(Frame f, const int32_t *__restrict__ tile_offsets, int cap, f
   const int rank = before + __popc(m & ((1u << lane) - 1));
   if (keep && off + rank < cap) {
     float *r = rows + rank * pitch;
+    int c0 = 0;
+    if (a.enabled) {
+#pragma unroll
+      for (int c = 0; c < 5; ++c) r[c] = v[c];
+      c0 = 5;
+    }
 #pragma unroll 1
-    for (int c = 0; c < D; ++c) r[c] = column(src, d, p, c);
+    for (int c = c0; c < D; ++c) r[c] = column(src, d, p, c);
   }
   __syncthreads();
   // the tile's kept rows are consecutive in the output: one coalesced copy of min(total, cap - off) rows
@@ -259,10 +286,21 @@ int bevb200_radar_sweeps_assemble(const float *store, int slots, int slot_cap, c
                                   const bevb200_radar_sweep_entry_t *entries, int batch, int max_entries,
                                   int out_dim, int cap, float *out, int32_t *counts, int32_t *status,
                                   void *workspace, size_t workspace_bytes, void *stream) {
+  return bevb200_radar_sweeps_assemble_aug(store, slots, slot_cap, slot_rows, params, entries, nullptr, batch,
+                                           max_entries, out_dim, cap, out, counts, status, workspace,
+                                           workspace_bytes, stream);
+}
+
+int bevb200_radar_sweeps_assemble_aug(const float *store, int slots, int slot_cap, const int32_t *slot_rows,
+                                      const bevb200_radar_sweep_params_t *params,
+                                      const bevb200_radar_sweep_entry_t *entries, const bevb200_lidar_aug_t *aug,
+                                      int batch, int max_entries, int out_dim, int cap, float *out, int32_t *counts,
+                                      int32_t *status, void *workspace, size_t workspace_bytes, void *stream) {
   BEVB200_REQUIRE(sizes_ok(batch, max_entries, slot_cap) && slots >= 1,
                   "sizes out of range (0 <= batch <= 65535, 1 <= max_entries <= 65535, slots >= 1, slot_cap >= 1, "
                   "max_entries * slot_cap < 2^31)");
   BEVB200_REQUIRE(out_dim >= 3 && out_dim <= kMaxDim, "out_dim must be in 3..64");
+  BEVB200_REQUIRE(!aug || out_dim >= 5, "the augmentation reads output columns 3 and 4: out_dim must be >= 5");
   BEVB200_REQUIRE(cap >= 1 && (long long)cap * out_dim <= 0x7fffffffLL, "cap must be positive, cap * out_dim < 2^31");
   BEVB200_REQUIRE(status, "null pointer");
   if (batch == 0) {
@@ -273,21 +311,25 @@ int bevb200_radar_sweeps_assemble(const float *store, int slots, int slot_cap, c
   BEVB200_REQUIRE((uintptr_t)entries % alignof(bevb200_radar_sweep_entry_t) == 0 &&
                       (uintptr_t)params % alignof(bevb200_radar_sweep_params_t) == 0,
                   "misaligned parameter block");
+  BEVB200_REQUIRE((uintptr_t)aug % alignof(bevb200_lidar_aug_t) == 0, "misaligned augmentation records");
   const size_t need = bevb200_radar_sweeps_workspace_bytes(batch, max_entries, slot_cap);
   if (!workspace || workspace_bytes < need) {
     snprintf(g_last_error, sizeof(g_last_error), "%s: workspace of %zu bytes, need %zu", __func__, workspace_bytes,
              need);
     return BEVB200_EWORKSPACE;
   }
-  Frame f{store, slot_rows, params, entries, slots, slot_cap, max_entries, out_dim, tiles_for(slot_cap)};
+  Frame f{store, slot_rows, params, entries, aug, slots, slot_cap, max_entries, out_dim, tiles_for(slot_cap)};
   int32_t *tiles = (int32_t *)workspace;
   cudaStream_t st = (cudaStream_t)stream;
   BEVB200_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t), st));
   const dim3 grid(f.tiles, max_entries, batch);
-  BEVB200_LAUNCH(radar_count_kernel, grid, kThreads, 0, st, f, tiles, status);
+  // the plain path is its own instance, with the registers it had before the augmentation existed
+  const auto count_kernel = aug ? radar_count_kernel<true> : radar_count_kernel<false>;
+  const auto write_kernel = aug ? radar_write_kernel<true> : radar_write_kernel<false>;
+  BEVB200_LAUNCH(count_kernel, grid, kThreads, 0, st, f, tiles, status);
   const int rc = sweeps_scan(tiles, batch, max_entries * f.tiles, cap, counts, status, st);
   if (rc) return rc;
-  BEVB200_LAUNCH(radar_write_kernel, grid, kThreads, 0, st, f, tiles, cap, out);
+  BEVB200_LAUNCH(write_kernel, grid, kThreads, 0, st, f, tiles, cap, out);
   return BEVB200_OK;
 }
 

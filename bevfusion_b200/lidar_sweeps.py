@@ -8,6 +8,8 @@ transforms_3d.py:585-614, base_points.py:208-232) on the device (csrc/lidar_swee
         assemble(samples, use_dim, ...) -> per sample the reference's results["points"].tensor
         write_frame(samples, use_dim, ...) + launch(batch, out_dim, cap): the same split in two, for CUDA graphs: the
         frame's parameters go to a device block at a fixed address in one copy, and launch() reads them from there.
+        aug= (a lidar_aug.LidarAug) applies GlobalRotScaleTrans + RandomFlip3D to every row before the range filter,
+        as the reference's training pipeline orders them.
     assemble_sweeps(key, sweeps, rotations, translations, lags, use_dim, ...)   one sample from host or device arrays
     choose_sweeps(n_sweeps, sweeps_num, test_mode)   the reference's sweep draw, on numpy's global RNG
     time_lag(timestamp, sweep_timestamp)             the reference's ts - sweep_ts (float64)
@@ -185,11 +187,13 @@ class SweepStore(SlotStore):
         self._write_block(host)
         return len(samples), F, bound
 
-    def launch(self, batch, out_dim, cap):
+    def launch(self, batch, out_dim, cap, aug=None):
         """Assemble the frame the block holds: (points [batch, cap, out_dim], counts [batch] int32, status [1]
-        int32), all on the device, no host synchronisation; CUDA-graph capturable."""
+        int32), all on the device, no host synchronisation; CUDA-graph capturable.  With aug (a LidarAug whose
+        records write() refreshed) each row is augmented before the range test."""
         if not 0 <= batch <= self.max_batch or not 5 <= out_dim <= MAX_DIM or cap < 1:
             raise ValueError("batch %d, out_dim %d or cap %d out of range" % (batch, out_dim, cap))
+        _check_aug(aug, batch, self.device)
         dev = self.device
         L = _C.lib()
         ws_bytes = L.bevb200_lidar_sweeps_workspace_bytes(batch, self.max_entries, self.slot_cap)
@@ -199,15 +203,23 @@ class SweepStore(SlotStore):
         ws = torch.empty((max(ws_bytes, 1),), dtype=torch.uint8, device=dev)
         base = self.block.data_ptr()
         with torch.cuda.device(dev):
-            _C.check(L.bevb200_lidar_sweeps_assemble(
-                _C.ptr(self.rows), self.slots, self.slot_cap, self.load_dim, _C.ptr(self.slot_rows), base,
-                base + _ENTRIES_AT, batch, self.max_entries, out_dim, cap, _C.ptr(out), _C.ptr(counts), _C.ptr(status),
-                _C.ptr(ws), ws.numel(), _C.current_stream(dev)), "lidar_sweeps_assemble")
+            if aug is None:
+                _C.check(L.bevb200_lidar_sweeps_assemble(
+                    _C.ptr(self.rows), self.slots, self.slot_cap, self.load_dim, _C.ptr(self.slot_rows), base,
+                    base + _ENTRIES_AT, batch, self.max_entries, out_dim, cap, _C.ptr(out), _C.ptr(counts),
+                    _C.ptr(status), _C.ptr(ws), ws.numel(), _C.current_stream(dev)), "lidar_sweeps_assemble")
+            else:
+                _C.check(L.bevb200_lidar_sweeps_assemble_aug(
+                    _C.ptr(self.rows), self.slots, self.slot_cap, self.load_dim, _C.ptr(self.slot_rows), base,
+                    base + _ENTRIES_AT, aug.ptr(), batch, self.max_entries, out_dim, cap, _C.ptr(out), _C.ptr(counts),
+                    _C.ptr(status), _C.ptr(ws), ws.numel(), _C.current_stream(dev)), "lidar_sweeps_assemble_aug")
         return out, counts, status
 
     def assemble(self, samples, use_dim, key_use_dim=None, sweeps_num=9, pad_empty_sweeps=True, remove_close=True,
-                 point_cloud_range=None, cap=None, sync=True, radius=1.0, reduce_beams=None, load_augmented=None):
-        """LoadPointsFromMultiSweeps (+ PointsRangeFilter with point_cloud_range) for each sample.
+                 point_cloud_range=None, cap=None, sync=True, radius=1.0, reduce_beams=None, load_augmented=None,
+                 aug=None):
+        """LoadPointsFromMultiSweeps (+ GlobalRotScaleTrans and RandomFlip3D with aug, a LidarAug holding one draw
+        per sample) (+ PointsRangeFilter with point_cloud_range) for each sample.
 
         sync=True: a list of [n_k, len(use_dim)] tensors, the reference's results["points"].tensor; raises when a
         sample keeps more than cap rows.  sync=False: (points [B, cap, F], counts [B] int32, status [1] int32) on
@@ -215,7 +227,7 @@ class SweepStore(SlotStore):
         rows a sample can keep, so no sample overflows it."""
         batch, F, bound = self.write_frame(samples, use_dim, key_use_dim, sweeps_num, pad_empty_sweeps, remove_close,
                                            point_cloud_range, radius, reduce_beams, load_augmented)
-        out, counts, status = self.launch(batch, F, max(bound, 1) if cap is None else int(cap))
+        out, counts, status = self.launch(batch, F, max(bound, 1) if cap is None else int(cap), aug)
         if not sync:
             return out, counts, status
         st = int(status.item())
@@ -224,6 +236,17 @@ class SweepStore(SlotStore):
                 name for bit, name in ((OVERFLOW, "a sample keeps more than cap rows"), (BAD_ENTRY, "a bad entry"),
                                        (BAD_PARAMS, "bad column maps")) if st & bit)))
         return [out[k, :n] for k, n in enumerate(counts.tolist())]
+
+
+def _check_aug(aug, batch, device):
+    if aug is None:
+        return
+    if not hasattr(aug, "ptr") or not hasattr(aug, "check_batch"):
+        raise TypeError("aug must be a lidar_aug.LidarAug")
+    from .lidar_aug import cuda_device
+    if aug.device != cuda_device(device):
+        raise ValueError("aug is on %s, the store on %s" % (aug.device, device))
+    aug.check_batch(batch)
 
 
 def assemble_sweeps(key, sweeps, rotations, translations, lags, use_dim, key_use_dim=None, sweeps_num=9,

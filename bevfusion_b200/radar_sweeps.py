@@ -8,6 +8,8 @@ transforms_3d.py:607-612, radar_points.py:92-107) on the device (csrc/radar_swee
         assemble(samples, use_dim, ...) -> per sample the reference's results["radar"].tensor after PointsRangeFilter
         write_frame(samples, use_dim, ...) + launch(batch, out_dim, cap): the same split in two, for CUDA graphs: the
         frame's parameters go to a device block at a fixed address in one copy, and launch() reads them from there.
+        aug= (a lidar_aug.LidarAug) applies GlobalRotScaleTrans + RandomFlip3D to output columns 0..4 of every row
+        (RadarPoints' rotate, scale and flip) before the range filter; it needs len(use_dim) >= 5.
     radar_entries(radars_dict, sweeps_num, slot_of)   one sample's entries: the reference's sweep choice and time lags
     assemble_radar_sweeps(radars_dict, points_of, sweeps_num, use_dim, ...)   one sample, in one call
 
@@ -27,7 +29,7 @@ import numpy as np
 import torch
 
 from . import _C
-from .lidar_sweeps import SlotStore, SWEEP
+from .lidar_sweeps import SlotStore, SWEEP, _check_aug
 
 __all__ = ["RadarSweepStore", "radar_entries", "assemble_radar_sweeps", "column_ops", "OVERFLOW",
            "BAD_ENTRY", "BAD_PARAMS", "BAD_CATEGORY"]
@@ -177,11 +179,15 @@ class RadarSweepStore(SlotStore):
         self._write_block(host)
         return len(samples), F, bound
 
-    def launch(self, batch, out_dim, cap):
+    def launch(self, batch, out_dim, cap, aug=None):
         """Assemble the frame the block holds: (points [batch, cap, out_dim], counts [batch] int32, status [1]
-        int32), all on the device, no host synchronisation; CUDA-graph capturable."""
+        int32), all on the device, no host synchronisation; CUDA-graph capturable.  With aug (a LidarAug whose
+        records write() refreshed) output columns 0..4 are augmented before the range test."""
         if not 0 <= batch <= self.max_batch or not 3 <= out_dim <= MAX_DIM or cap < 1:
             raise ValueError("batch %d, out_dim %d or cap %d out of range" % (batch, out_dim, cap))
+        _check_aug(aug, batch, self.device)
+        if aug is not None and out_dim < 5:
+            raise ValueError("the augmentation reads columns 3 and 4 (RadarPoints.rotate): out_dim must be >= 5")
         dev = self.device
         L = _C.lib()
         ws_bytes = L.bevb200_radar_sweeps_workspace_bytes(batch, self.max_entries, self.slot_cap)
@@ -191,16 +197,23 @@ class RadarSweepStore(SlotStore):
         ws = torch.empty((max(ws_bytes, 1),), dtype=torch.uint8, device=dev)
         base = self.block.data_ptr()
         with torch.cuda.device(dev):
-            _C.check(L.bevb200_radar_sweeps_assemble(
-                _C.ptr(self.rows), self.slots, self.slot_cap, _C.ptr(self.slot_rows), base, base + _ENTRIES_AT,
-                batch, self.max_entries, out_dim, cap, _C.ptr(out), _C.ptr(counts), _C.ptr(status), _C.ptr(ws),
-                ws.numel(), _C.current_stream(dev)), "radar_sweeps_assemble")
+            if aug is None:
+                _C.check(L.bevb200_radar_sweeps_assemble(
+                    _C.ptr(self.rows), self.slots, self.slot_cap, _C.ptr(self.slot_rows), base, base + _ENTRIES_AT,
+                    batch, self.max_entries, out_dim, cap, _C.ptr(out), _C.ptr(counts), _C.ptr(status), _C.ptr(ws),
+                    ws.numel(), _C.current_stream(dev)), "radar_sweeps_assemble")
+            else:
+                _C.check(L.bevb200_radar_sweeps_assemble_aug(
+                    _C.ptr(self.rows), self.slots, self.slot_cap, _C.ptr(self.slot_rows), base, base + _ENTRIES_AT,
+                    aug.ptr(), batch, self.max_entries, out_dim, cap, _C.ptr(out), _C.ptr(counts), _C.ptr(status),
+                    _C.ptr(ws), ws.numel(), _C.current_stream(dev)), "radar_sweeps_assemble_aug")
         return out, counts, status
 
     def assemble(self, samples, use_dim, compensate_velocity=False, normalize=False, normalize_dims=NORMALIZE_DIMS,
-                 bev_range=BEV_RANGE, cap=None, sync=True, max_num=None):
-        """LoadRadarPointsMultiSweeps (+ PointsRangeFilter's radar face with bev_range; None gives the cloud before
-        any augmentation or filter) for each sample.
+                 bev_range=BEV_RANGE, cap=None, sync=True, max_num=None, aug=None):
+        """LoadRadarPointsMultiSweeps (+ GlobalRotScaleTrans and RandomFlip3D with aug, a LidarAug holding one draw
+        per sample) (+ PointsRangeFilter's radar face with bev_range; None gives the cloud before any filter) for
+        each sample.
 
         sync=True: a list of [n_k, len(use_dim)] tensors, the reference's results["radar"].tensor; raises when a
         sample keeps more than cap rows or the reference would raise.  sync=False: (points [B, cap, F], counts [B]
@@ -208,7 +221,7 @@ class RadarSweepStore(SlotStore):
         cap defaults to the most rows a sample can keep, so no sample overflows it."""
         batch, F, bound = self.write_frame(samples, use_dim, compensate_velocity, normalize, normalize_dims,
                                            bev_range, max_num)
-        out, counts, status = self.launch(batch, F, max(bound, 1) if cap is None else int(cap))
+        out, counts, status = self.launch(batch, F, max(bound, 1) if cap is None else int(cap), aug)
         if not sync:
             return out, counts, status
         st = int(status.item())

@@ -1484,6 +1484,71 @@ BEVB200_API int bevb200_radar_sweeps_assemble(const float *store, int slots, int
                                               int out_dim, int cap, float *out, int32_t *counts, int32_t *status,
                                               void *workspace, size_t workspace_bytes, void *stream);
 
+/* ---- GlobalRotScaleTrans + RandomFlip3D on the LiDAR and radar clouds and the GT boxes, ObjectRangeFilter and
+ *      ObjectNameFilter (transforms_3d.py:195-232, 323-353, 534-636; base_points.py:137-272, lidar_points.py:29-34,
+ *      radar_points.py:27-90, base_box3d.py:148-232, lidar_box3d.py:140-205, utils.py:6-19) ------------------------
+ * One record per sample (DEVICE).  Every scalar is computed on the host with the reference's torch CPU calls: the
+ * device evaluates no sine or cosine.  With enabled = 0 the sample is left exactly as it is (no identity matrix is
+ * applied: it would change signed zeros and infinities).  Otherwise, in fp32 with one rounding per operation and
+ * chain_j(p, R) = fma(p2, R[2][j], fma(p1, R[1][j], fma(p0, R[0][j], +0))) (every term evaluated, the zero entries
+ * included; a 2-term chain for 2-vectors):
+ *   rot_scale_trans  xyz = chain(xyz, point_rot); xyz += translation; xyz *= scale
+ *                    radar also: c34 = chain(c34, point_rot[:2, :2]); c34 *= scale (output columns 3 and 4)
+ *                    boxes: xyz = chain(xyz, box_rot); yaw += yaw_inc; vel = chain(vel, box_rot[:2, :2]) (9 columns);
+ *                    xyz += translation; columns :6 and 7: *= scale
+ *   flip_horizontal  y = -y (radar: and column 4; boxes: columns 1::7, then yaw = -yaw + fl32(pi))
+ *   flip_vertical    x = -x (radar: and column 3; boxes: columns 0::7, then yaw = -yaw)
+ * The sweep entry points below apply the record to each assembled row before the range test, so the range filter
+ * sees the augmented row, as PointsRangeFilter does after RandomFlip3D.  A NULL aug pointer is the plain path. */
+#define BEVB200_LIDAR_AUG_BYTES 108
+typedef struct {
+  int32_t enabled;           /* 0: leave the sample untouched */
+  int32_t rot_scale_trans;   /* GlobalRotScaleTrans drew (is_train) */
+  int32_t flip_horizontal;
+  int32_t flip_vertical;
+  float translation[3];      /* fl32(translation) */
+  float scale;               /* fl32(scale) */
+  float yaw_inc;             /* fl32(theta) */
+  float point_rot[9];        /* rot_mat_T of BasePoints.rotate(fl32(-theta)), row-major */
+  float box_rot[9];          /* rot_mat_T of LiDARInstance3DBoxes.rotate(fl32(theta)), row-major */
+} bevb200_lidar_aug_t;
+
+/* bevb200_lidar_sweeps_assemble with the sweep rows augmented by aug [batch] (DEVICE, or NULL for none) between the
+ * transform and the range test.  Everything else is as bevb200_lidar_sweeps_assemble, which is this call with NULL. */
+BEVB200_API int bevb200_lidar_sweeps_assemble_aug(const float *store, int slots, int slot_cap, int load_dim,
+                                                  const int32_t *slot_rows, const bevb200_sweep_params_t *params,
+                                                  const bevb200_sweep_entry_t *entries,
+                                                  const bevb200_lidar_aug_t *aug, int batch, int max_entries,
+                                                  int out_dim, int cap, float *out, int32_t *counts,
+                                                  int32_t *status, void *workspace, size_t workspace_bytes,
+                                                  void *stream);
+/* bevb200_radar_sweeps_assemble with output columns 0..4 augmented by aug [batch] (DEVICE, or NULL for none) after
+ * normalisation and before the range test; with aug, out_dim must be >= 5 (RadarPoints reads columns 3 and 4).
+ * bevb200_radar_sweeps_assemble is this call with NULL. */
+BEVB200_API int bevb200_radar_sweeps_assemble_aug(const float *store, int slots, int slot_cap,
+                                                  const int32_t *slot_rows, const bevb200_radar_sweep_params_t *params,
+                                                  const bevb200_radar_sweep_entry_t *entries,
+                                                  const bevb200_lidar_aug_t *aug, int batch, int max_entries,
+                                                  int out_dim, int cap, float *out, int32_t *counts,
+                                                  int32_t *status, void *workspace, size_t workspace_bytes,
+                                                  void *stream);
+
+/* GT boxes: boxes [batch, nmax, box_dim] fp32, labels [batch, nmax] int32, counts [batch] int32 (DEVICE; the padded
+ * layout of head_targets.pad_gt), box_dim 7 or 9, 0 <= nmax <= BEVB200_HEAD_TARGETS_MAX_BOXES.  Per box in order:
+ * the record's transforms (above), then ObjectRangeFilter (kept iff range[0] < x < range[2] and range[1] < y <
+ * range[3] in fp32; NaN is dropped) with limit_yaw(0.5, 2 pi): yaw - floor(yaw / fl32(2 pi) + 0.5) * fl32(2 pi), then
+ * ObjectNameFilter (kept iff 0 <= label < num_classes).  The survivors go in order to out_boxes [batch, nmax,
+ * box_dim] / out_labels [batch, nmax], out_counts [batch] their number; the rest of each sample's rows are zeroed.
+ * aug may be NULL (no augmentation).  One CTA per sample, ballot ranks, no atomics on the output order, no host
+ * synchronisation.  status [1] int32 (DEVICE) is zeroed, then gets
+ *   BEVB200_BOX_AUG_BAD_COUNT  a count outside [0, nmax] (read as clamped to it)
+ * In and out must not overlap. */
+#define BEVB200_BOX_AUG_BAD_COUNT 1
+BEVB200_API int bevb200_box_aug(const float *boxes, const int32_t *labels, const int32_t *counts, int batch, int nmax,
+                                int box_dim, const bevb200_lidar_aug_t *aug, float range_x_min, float range_y_min,
+                                float range_x_max, float range_y_max, int num_classes, float *out_boxes,
+                                int32_t *out_labels, int32_t *out_counts, int32_t *status, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
