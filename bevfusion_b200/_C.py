@@ -192,6 +192,9 @@ _SIGNATURES = {
     "bevb200_radar_sweeps_assemble_aug": (c_int, [_P, c_int, c_int, _P, _P, _P, _P] + [c_int] * 4 + [_P] * 4
                                           + [c_size_t, _P]),
     "bevb200_box_aug": (c_int, [_P, _P, _P, c_int, c_int, c_int, _P] + [c_float] * 4 + [c_int] + [_P] * 5),
+    "bevb200_lidar_sweeps_paste_workspace_bytes": (c_size_t, [c_int] * 5),
+    "bevb200_lidar_sweeps_assemble_paste": (c_int, [_P, c_int, c_int, c_int, _P, _P, _P, _P, _P, c_int, c_int, _P,
+                                                    c_int, c_int, _P, _P] + [c_int] * 5 + [_P] * 4 + [c_size_t, _P]),
 }
 
 

@@ -10,6 +10,8 @@ transforms_3d.py:585-614, base_points.py:208-232) on the device (csrc/lidar_swee
         frame's parameters go to a device block at a fixed address in one copy, and launch() reads them from there.
         aug= (a lidar_aug.LidarAug) applies GlobalRotScaleTrans + RandomFlip3D to every row before the range filter,
         as the reference's training pipeline orders them.
+        paste= (an object_paste.PasteBlock) applies ObjectPaste first: the rows inside each sample's kept boxes are
+        removed and the kept objects' rows come first, then every row is augmented and range-filtered.
     assemble_sweeps(key, sweeps, rotations, translations, lags, use_dim, ...)   one sample from host or device arrays
     choose_sweeps(n_sweeps, sweeps_num, test_mode)   the reference's sweep draw, on numpy's global RNG
     time_lag(timestamp, sweep_timestamp)             the reference's ts - sweep_ts (float64)
@@ -25,11 +27,11 @@ import torch
 from . import _C
 
 __all__ = ["SlotStore", "SweepStore", "assemble_sweeps", "choose_sweeps", "time_lag", "OVERFLOW", "BAD_ENTRY",
-           "BAD_PARAMS"]
+           "BAD_PARAMS", "BAD_PASTE"]
 
 NONE, KEY, SWEEP, PAD = 0, 1, 2, 3            # BEVB200_SWEEP_*
 MAX_DIM = 8                                   # BEVB200_SWEEP_MAX_DIM: F <= 8, as the fused voxelizer takes
-OVERFLOW, BAD_ENTRY, BAD_PARAMS = 1, 2, 4     # BEVB200_SWEEPS_*: status bits
+OVERFLOW, BAD_ENTRY, BAD_PARAMS, BAD_PASTE = 1, 2, 4, 8    # BEVB200_SWEEPS_*: status bits
 
 # bevb200_sweep_entry_t / bevb200_sweep_params_t, C layout (align=True)
 ENTRY_DTYPE = np.dtype([("kind", "<i4"), ("slot", "<i4"), ("rotation", "<f8", (9,)), ("translation", "<f8", (3,)),
@@ -177,25 +179,32 @@ class SweepStore(SlotStore):
         return host, F, bound
 
     def write_frame(self, samples, use_dim, key_use_dim=None, sweeps_num=9, pad_empty_sweeps=True, remove_close=True,
-                    point_cloud_range=None, radius=1.0, reduce_beams=None, load_augmented=None):
+                    point_cloud_range=None, radius=1.0, reduce_beams=None, load_augmented=None, paste=None):
         """Pack the frame's parameters and copy them, in one pinned asynchronous copy, into the device block that
         launch() reads.  Returns (batch, out_dim, bound): bound is the most rows a sample can keep, from the row
-        counts put() stored."""
+        counts put() stored, plus the rows paste's last write() pastes into a sample."""
         _check_loader_options(reduce_beams, load_augmented)
         host, F, bound = self._pack(samples, use_dim, key_use_dim, sweeps_num, pad_empty_sweeps, remove_close,
                                     point_cloud_range, radius)
+        if paste is not None:
+            _check_paste(paste, len(samples), F, self.device)
+            bound += max(paste.rows[:len(samples)], default=0)
         self._write_block(host)
         return len(samples), F, bound
 
-    def launch(self, batch, out_dim, cap, aug=None):
+    def launch(self, batch, out_dim, cap, aug=None, paste=None):
         """Assemble the frame the block holds: (points [batch, cap, out_dim], counts [batch] int32, status [1]
         int32), all on the device, no host synchronisation; CUDA-graph capturable.  With aug (a LidarAug whose
-        records write() refreshed) each row is augmented before the range test."""
+        records write() refreshed) each row is augmented before the range test.  With paste (a PasteBlock whose
+        write() covered the batch) each sample's kept objects are pasted and the rows in their boxes removed first."""
         if not 0 <= batch <= self.max_batch or not 5 <= out_dim <= MAX_DIM or cap < 1:
             raise ValueError("batch %d, out_dim %d or cap %d out of range" % (batch, out_dim, cap))
         _check_aug(aug, batch, self.device)
         dev = self.device
         L = _C.lib()
+        if paste is not None:
+            _check_paste(paste, batch, out_dim, dev)
+            return self._launch_paste(batch, out_dim, cap, aug, paste)
         ws_bytes = L.bevb200_lidar_sweeps_workspace_bytes(batch, self.max_entries, self.slot_cap)
         out = torch.empty((batch, cap, out_dim), dtype=torch.float32, device=dev)
         counts = torch.empty((batch,), dtype=torch.int32, device=dev)
@@ -215,26 +224,49 @@ class SweepStore(SlotStore):
                     _C.ptr(status), _C.ptr(ws), ws.numel(), _C.current_stream(dev)), "lidar_sweeps_assemble_aug")
         return out, counts, status
 
+    def _launch_paste(self, batch, out_dim, cap, aug, paste):
+        dev, ps = self.device, paste.store
+        L = _C.lib()
+        ws_bytes = L.bevb200_lidar_sweeps_paste_workspace_bytes(batch, self.max_entries, self.slot_cap,
+                                                                paste.max_paste, ps.object_cap)
+        if ws_bytes == 0 and batch:
+            raise ValueError("max_entries + max_paste or the object cap out of range")
+        out = torch.empty((batch, cap, out_dim), dtype=torch.float32, device=dev)
+        counts = torch.empty((batch,), dtype=torch.int32, device=dev)
+        status = torch.empty((1,), dtype=torch.int32, device=dev)
+        ws = torch.empty((max(ws_bytes, 1),), dtype=torch.uint8, device=dev)
+        base = self.block.data_ptr()
+        with torch.cuda.device(dev):
+            _C.check(L.bevb200_lidar_sweeps_assemble_paste(
+                _C.ptr(self.rows), self.slots, self.slot_cap, self.load_dim, _C.ptr(self.slot_rows), base,
+                base + _ENTRIES_AT, 0 if aug is None else aug.ptr(), _C.ptr(ps.rows), ps.max_rows, ps.load_dim,
+                _C.ptr(ps.table), ps.max_objects, ps.object_cap, paste.samples_ptr(), paste.objects_ptr(),
+                paste.max_paste, batch, self.max_entries, out_dim, cap, _C.ptr(out), _C.ptr(counts), _C.ptr(status),
+                _C.ptr(ws), ws.numel(), _C.current_stream(dev)), "lidar_sweeps_assemble_paste")
+        return out, counts, status
+
     def assemble(self, samples, use_dim, key_use_dim=None, sweeps_num=9, pad_empty_sweeps=True, remove_close=True,
                  point_cloud_range=None, cap=None, sync=True, radius=1.0, reduce_beams=None, load_augmented=None,
-                 aug=None):
-        """LoadPointsFromMultiSweeps (+ GlobalRotScaleTrans and RandomFlip3D with aug, a LidarAug holding one draw
-        per sample) (+ PointsRangeFilter with point_cloud_range) for each sample.
+                 aug=None, paste=None):
+        """LoadPointsFromMultiSweeps (+ ObjectPaste with paste, a PasteBlock holding one draw per sample)
+        (+ GlobalRotScaleTrans and RandomFlip3D with aug, a LidarAug holding one draw per sample)
+        (+ PointsRangeFilter with point_cloud_range) for each sample.
 
         sync=True: a list of [n_k, len(use_dim)] tensors, the reference's results["points"].tensor; raises when a
         sample keeps more than cap rows.  sync=False: (points [B, cap, F], counts [B] int32, status [1] int32) on
         the device, with no host synchronisation; rows past counts[k] are unspecified.  cap defaults to the most
         rows a sample can keep, so no sample overflows it."""
         batch, F, bound = self.write_frame(samples, use_dim, key_use_dim, sweeps_num, pad_empty_sweeps, remove_close,
-                                           point_cloud_range, radius, reduce_beams, load_augmented)
-        out, counts, status = self.launch(batch, F, max(bound, 1) if cap is None else int(cap), aug)
+                                           point_cloud_range, radius, reduce_beams, load_augmented, paste)
+        out, counts, status = self.launch(batch, F, max(bound, 1) if cap is None else int(cap), aug, paste)
         if not sync:
             return out, counts, status
         st = int(status.item())
         if st:
             raise ValueError("lidar_sweeps_assemble status %d: %s" % (st, ", ".join(
                 name for bit, name in ((OVERFLOW, "a sample keeps more than cap rows"), (BAD_ENTRY, "a bad entry"),
-                                       (BAD_PARAMS, "bad column maps")) if st & bit)))
+                                       (BAD_PARAMS, "bad column maps"), (BAD_PASTE, "a bad paste block"))
+                if st & bit)))
         return [out[k, :n] for k, n in enumerate(counts.tolist())]
 
 
@@ -247,6 +279,16 @@ def _check_aug(aug, batch, device):
     if aug.device != cuda_device(device):
         raise ValueError("aug is on %s, the store on %s" % (aug.device, device))
     aug.check_batch(batch)
+
+
+def _check_paste(paste, batch, out_dim, device):
+    from .lidar_aug import cuda_device
+    from .object_paste import PasteBlock
+    if not isinstance(paste, PasteBlock):
+        raise TypeError("paste must be an object_paste.PasteBlock")
+    if paste.device != cuda_device(device):
+        raise ValueError("paste is on %s, the store on %s" % (paste.device, device))
+    paste.check_batch(batch, out_dim)
 
 
 def assemble_sweeps(key, sweeps, rotations, translations, lags, use_dim, key_use_dim=None, sweeps_num=9,

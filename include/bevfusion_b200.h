@@ -1549,6 +1549,58 @@ BEVB200_API int bevb200_box_aug(const float *boxes, const int32_t *labels, const
                                 float range_x_max, float range_y_max, int num_classes, float *out_boxes,
                                 int32_t *out_labels, int32_t *out_counts, int32_t *status, void *stream);
 
+/* ---- ObjectPaste (GT-database sampling) on the assembled LiDAR cloud (transforms_3d.py:357-449, dbsampler.py,
+ *      box_np_ops.py:430-451, 692-775) -------------------------------------------------------------------------------
+ * The draw and the collision test run on the host (bevfusion_b200/object_paste.py); the device receives the kept
+ * objects.  objects [max_rows, obj_dim] fp32 (DEVICE) holds raw object rows as the database files store them;
+ * object_table [num_objects, 2] int32 (DEVICE) gives each object's first row and row count (an object is valid iff
+ * first >= 0, 0 <= rows <= object_cap and first + rows <= max_rows).  paste [batch] (DEVICE) gives per sample the
+ * count S of kept objects and the column map of points_loader.use_dim; paste_objects [batch, max_paste] (DEVICE) the
+ * kept objects in the reference's order, each with its store index, fl32(box[:3]) and its 6 face planes (n, d) from
+ * points_in_rbbox(origin (0.5, 0.5, 0), z axis), computed on the host with the reference's numpy calls.
+ * Per sample, with S >= 1:
+ *   KEY, SWEEP and PAD rows, after the pose transform and before the augmentation, are dropped iff they lie in any
+ *   kept box: a row is in a box unless one face gives ((x * n0 + y * n1) + z * n2) + d >= 0, each operation one fp32
+ *   rounding with no contraction.  So a row exactly on a face is kept, and a row with a NaN coordinate is dropped.
+ *   Pasted rows come first, object by object in order: out[c] = row[cols[c]], out[j] += translation[j] (j < 3, fp32),
+ *   then the augmentation and the range test as for every other row (no remove_close, no pose transform).
+ * A sample with S = 0 is assembled exactly as bevb200_lidar_sweeps_assemble_aug assembles it.  status also gets
+ *   BEVB200_SWEEPS_BAD_PASTE   a sample's count is outside [0, max_paste], a column of its map outside [0, obj_dim),
+ *                              or a kept object's index or table entry invalid: that block pastes and removes nothing
+ * Everything else is as bevb200_lidar_sweeps_assemble_aug, which is this call with a NULL paste block (the object
+ * arguments are then ignored).  The grid gains max_paste entries per sample, tiled as the sweep entries are, over
+ * 1024-row tiles of max(slot_cap, object_cap) rows.  Sizes: 1 <= max_paste <= BEVB200_PASTE_MAX_OBJECTS,
+ * 1 <= obj_dim <= 64, object_cap >= 1, max_entries + max_paste <= 65535, (max_entries + max_paste) * object_cap
+ * < 2^31.  Workspace: bevb200_lidar_sweeps_paste_workspace_bytes(batch, max_entries, slot_cap, max_paste,
+ * object_cap) (0 for unsupported sizes). */
+#define BEVB200_SWEEPS_BAD_PASTE 8
+#define BEVB200_PASTE_MAX_OBJECTS 256
+#define BEVB200_PASTE_SAMPLE_BYTES 48
+#define BEVB200_PASTE_OBJECT_BYTES 112
+typedef struct {
+  int32_t count;                           /* kept objects, 0..max_paste */
+  int32_t cols[BEVB200_SWEEP_MAX_DIM];     /* points_loader.use_dim: output column c = object row[cols[c]] */
+  int32_t reserved[3];
+} bevb200_paste_sample_t;
+typedef struct {
+  int32_t index;                           /* the object in object_table */
+  float translation[3];                    /* fl32(box[:3]) */
+  float planes[6][4];                      /* per face: normal[3], d (surface_equ_3d's normal and -einsum) */
+} bevb200_paste_object_t;
+BEVB200_API size_t bevb200_lidar_sweeps_paste_workspace_bytes(int batch, int max_entries, int slot_cap, int max_paste,
+                                                              int object_cap);
+BEVB200_API int bevb200_lidar_sweeps_assemble_paste(const float *store, int slots, int slot_cap, int load_dim,
+                                                    const int32_t *slot_rows, const bevb200_sweep_params_t *params,
+                                                    const bevb200_sweep_entry_t *entries,
+                                                    const bevb200_lidar_aug_t *aug, const float *objects,
+                                                    int max_rows, int obj_dim, const int32_t *object_table,
+                                                    int num_objects, int object_cap,
+                                                    const bevb200_paste_sample_t *paste,
+                                                    const bevb200_paste_object_t *paste_objects, int max_paste,
+                                                    int batch, int max_entries, int out_dim, int cap, float *out,
+                                                    int32_t *counts, int32_t *status, void *workspace,
+                                                    size_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
